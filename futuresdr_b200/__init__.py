@@ -1,4 +1,4 @@
-"""futuresdr_b200 -- B200-native (sm_100a) backend for FutureSDR's FIR / decimator / resampler /
+"""futuresdr_b200 -- H100-native (sm_90a) backend for FutureSDR's FIR / decimator / resampler /
 FFT / Apply / PfbArbResampler hot path.
 
 Python host layer above the C ABI (include/b200sdr.h).  Class and method names mirror the

@@ -39,8 +39,8 @@ static int32_t ctx_create(int device, void *stream, bool own, b2s_ctx **out) {
     B2S_CUDA(ctx, cudaGetDeviceProperties(&prop, device));
     ctx->sm_count = prop.multiProcessorCount;
     ctx->smem_optin = prop.sharedMemPerBlockOptin;
-    if (prop.major < 10) {
-        return b2s_fail(nullptr, B2S_EUNSUPPORTED, "device %d is sm_%d%d; libb200sdr is built for sm_100a only",
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code (wgmma) runs on compute capability 9.0 only
+        return b2s_fail(nullptr, B2S_EUNSUPPORTED, "device %d is sm_%d%d; libb200sdr is built for sm_90a only",
                         device, prop.major, prop.minor);
     }
     if (!own) {
@@ -143,9 +143,9 @@ int32_t b2s_memcpy_d2h(b2s_ctx *ctx, void *hptr, const void *dptr, size_t bytes)
 /* ------------------------------------------------------------------------------------------
  * FIR
  * ---------------------------------------------------------------------------------------- */
-// Crossover measured on B200 (profiles/bench_configs_r1.jsonl, 64 Mi c32 samples): 16 taps direct 0.237 ms /
-// tensor 0.227 ms, 32 taps 0.290 / 0.226, 64 taps 0.423 / 0.230.  Below ~24 taps the CUDA-core kernel is
-// HBM-bound as well and keeps plain FP32 products, so it stays the default there.
+// Short filters: the CUDA-core kernel is HBM-bound as well and keeps plain FP32 products, so it stays the
+// default below this many taps.  The value is carried over from the previous (B200) tuning; the crossover has not
+// been re-measured on H100.
 static constexpr size_t kTensorMinTaps = 24;
 // Long filters (beyond the tensor kernel's 257 taps) go to the overlap-save FFT kernel.
 static constexpr size_t kFftMinTaps = 258;
@@ -273,11 +273,10 @@ static void fir_counts(const b2s_fir *f, size_t n_in, size_t n_out_cap, size_t *
 static int32_t fir_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out,
                           cudaStream_t stream) {
     if (f->kind == B2S_F64_F64) return fir_f64_launch(f, d_in, n_in, d_out, n_out, stream);
-    // SMALL slices under AUTO: the tensor kernel has a fixed cost of ~12 us per launch (TMEM allocation, Toeplitz fill,
-    // 148 persistent CTAs) against ~7 us for the CUDA-core kernel, whose time then grows with n_out * ntaps
-    // (scripts/small_sweep.py on B200: 6.9e-14 s per f32 sample-tap, 1.15e-13 per c32 one).  Below ~10 us of estimated
-    // CUDA-core time the direct form wins -- the perf/fir regime (1 M-sample calls of a 64-tap filter: 12.3 -> 7.3 us).
-    // An explicit B2S_ALGO_TENSOR request is always honoured.
+    // SMALL slices under AUTO: the tensor kernel has a fixed per-launch cost (Toeplitz fill, one persistent CTA per
+    // SM) that the CUDA-core kernel does not pay; the latter's time grows with n_out * ntaps (per_tap: estimated
+    // seconds per sample-tap, scripts/small_sweep.py; carried over from the previous (B200) tuning, not re-measured
+    // on H100).  Below ~10 us of estimated CUDA-core time the direct form is used.  An explicit B2S_ALGO_TENSOR request is always honoured.
     if (f->algo == B2S_ALGO_TENSOR && f->algo_req == B2S_ALGO_AUTO) {
         const double per_tap = f->kind == B2S_F32_F32 ? 6.9e-14 : 1.15e-13;
         if ((double)n_out * (double)f->ntaps * per_tap < 10e-6) return fir_direct_launch(f, d_in, n_in, d_out, n_out, stream);
@@ -320,8 +319,7 @@ int32_t b2s_fir_filter_host(b2s_fir *f, const void *h_in, size_t n_in, void *h_o
     const size_t isz = kind_in_bytes(f->kind), D = f->decim, N = f->ntaps;
     constexpr int NSLOT = 4;
     // chunk: ~32 MiB of input per slot (B2S_HOST_CHUNK_MB overrides), whole multiples of the direct kernel's
-    // 1024-output tile.  Measured on B200 / PCIe Gen5 (64 Mi c32 samples, 256 taps): 32 MiB 5.69, 8 MiB 5.35,
-    // 4 MiB 4.73 Gsamples/s -- shorter chunks shorten the un-overlapped first H2D / last D2H but lose more to
+    // 1024-output tile.  Shorter chunks shorten the un-overlapped first H2D / last D2H but lose more to
     // per-copy overhead.
     static const size_t chunk_mb = [] { const char *e = getenv("B2S_HOST_CHUNK_MB"); const long v = e ? atol(e) : 32; return (size_t)(v > 0 ? v : 32); }();
     size_t CH = round_up(std::max<size_t>((chunk_mb << 20) / (isz * D), 1024), 1024);

@@ -223,10 +223,9 @@ __global__ void chan_transpose_kernel(const float2 *__restrict__ spec, float2 *_
 // Outputs whose windows still reach into the previous call's history (the first T-1 of a call) take the generic
 // three-kernel path.
 // ---------------------------------------------------------------------------------------------------------------
-// Row stride of the FFT buffers = the padded transform length.  (Tried: the exact, odd stride N + N/16 - 1, which puts
-// the 512/N transforms a warp works on at distinct bank offsets -- ncu counts 17 M store conflicts on 30 M store
-// wavefronts with 68 -- but rows that start 8 bytes off a 16-byte boundary cost more than the conflicts: 64 channels
-// 195 -> 182 Gsamples/s, 16 channels 262 -> 193.  Also: at 68 the 64-channel kernel sits at EXACTLY two CTAs per SM,
+// Row stride of the FFT buffers = the padded transform length.  (The exact, odd stride N + N/16 - 1 puts the 512/N
+// transforms a warp works on at distinct bank offsets, but its rows start 8 bytes off a 16-byte boundary, which cost
+// more than the bank conflicts it removes.  Also: at 68 the 64-channel kernel sits at EXACTLY two CTAs per SM,
 // 2 x (2 x 40448 + 64 x 68 x 8 + 1024 reserved) = 233472 bytes; one float2 more per row halves the occupancy.)
 __host__ __device__ constexpr int chan_row_stride(int n) { return n + n / 16; }
 
@@ -238,7 +237,7 @@ __device__ __forceinline__ void chan_cp_async16(void *dst_smem, const void *src,
 
 // Persistent: a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... and the input tile of the NEXT one is fetched
 // with cp.async into the other half of a double buffer while the current one is filtered, transformed and stored
-// (the first version loaded, waited, computed: ncu showed 60 % of the stall samples on the global loads and 2.4 TB/s).
+// (a load, wait, compute sequence leaves the CTA stalled on its global loads).
 template <int LOG2N, int TPAD>
 __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restrict__ in, const float *__restrict__ arms_pad,
                                                          const float2 *__restrict__ tw, float2 *__restrict__ out, int base0,
@@ -262,9 +261,9 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
     const int b = tid % N, run = tid / N;
     int r = (base0 - b) % N; if (r < 0) r += N;              // window b receives samples == r (mod N)
     int arm = (b - base0 - 1) % N; if (arm < 0) arm += N;    // and always meets this arm
-    unsigned long long tap[TPAD];            // (t, t) pairs: one FFMA2 per complex x real MAC (common.cuh cmac2)
+    float tap[TPAD];
 #pragma unroll
-    for (int j = 0; j < TPAD; j++) tap[j] = dup2(__ldg(arms_pad + (size_t)j * N + arm));
+    for (int j = 0; j < TPAD; j++) tap[j] = __ldg(arms_pad + (size_t)j * N + arm);
 
     auto fetch = [&](int tile, float2 *X) {                  // A: the (OB + TPAD - 1) * N samples tile `tile` depends on
         const long long base = (o_first + (long long)tile * OB - (TPAD - 1)) * N;   // rows in front of the call meet zero taps
@@ -303,7 +302,7 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
 #pragma unroll
                 for (int u = 0; u < RL; u++) {
                     const int j = u + TPAD - 1 - k;          // output u sees this row as its j-th newest sample
-                    if (j >= 0 && j < TPAD) cmac2(acc[u], x, tap[j]);
+                    if (j >= 0 && j < TPAD) mac(acc[u], x, tap[j]);
                 }
             }
 #pragma unroll

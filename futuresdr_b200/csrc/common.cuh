@@ -45,20 +45,10 @@ struct PerDeviceOnce {
 };
 
 #ifdef __CUDACC__
-// acc += x * t for a Complex<f32> sample and a REAL tap as ONE packed instruction (sm_100 FFMA2: both lanes are IEEE
-// fused multiply-adds, bit-identical to the two scalar FFMAs).  The packed form runs at the same lane rate as FFMA
-// (scripts/microbench/f32x2_rate.cu: 35 T lane-op/s either way) but takes one issue slot instead of two, which is what
-// the sliding-window kernels are short of (ncu: 80 % of the issue slots busy, 43 % of them FFMA).
-// tt = (t, t); build it once per tap with dup2() so the register pair is reused by every MAC of that tap.
-__device__ __forceinline__ unsigned long long dup2(float t) {
-    unsigned long long d;
-    asm("mov.b64 %0, {%1, %1};" : "=l"(d) : "f"(t));
-    return d;
-}
-__device__ __forceinline__ void cmac2(float2 &acc, float2 x, unsigned long long tt) {
-    unsigned long long a = *reinterpret_cast<unsigned long long *>(&acc);
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a) : "l"(*reinterpret_cast<unsigned long long *>(&x)), "l"(tt));
-    acc = *reinterpret_cast<float2 *>(&a);
+// acc += x * t for a Complex<f32> sample and a REAL tap: two IEEE fused multiply-adds (sm_90 has no packed FFMA2).
+__device__ __forceinline__ void mac(float2 &acc, float2 x, float t) {
+    acc.x = fmaf(x.x, t, acc.x);
+    acc.y = fmaf(x.y, t, acc.y);
 }
 #endif
 

@@ -1,4 +1,4 @@
-// fft.cu -- batched power-of-two Complex<f32> FFT, one pass through shared memory (sm_100a).
+// fft.cu -- batched power-of-two Complex<f32> FFT, one pass through shared memory (sm_90a).
 //
 // Device version of the reference's Fft block (src/blocks/fft.rs:160-221), whose arithmetic is
 // rustfft 6.4 (crates.io): forward X[k] = sum_n x[n] e^{-2 pi i kn/N}, inverse un-normalised
@@ -113,10 +113,9 @@ __device__ __forceinline__ void fft_pass(const FftArgs &a, const float2 *gin, fl
 constexpr int kFftThreads = 256;
 
 // threads per CTA / CTAs per SM the register allocation must allow, per size.  8192: the unconstrained build takes
-// 171 registers = one 256-thread CTA per SM although shared memory admits three -> cap at 128 (16 B of spills), two
-// CTAs.  16384: one transform fills 139 KiB of shared memory, so one CTA per SM whatever we do -- 512 threads halve
+// one 256-thread CTA per SM by registers although shared memory admits more -> cap at 128 registers, two CTAs.  16384: one transform fills 139 KiB of shared memory, so one CTA per SM whatever we do -- 512 threads halve
 // the butterflies (and registers) per thread and double the warps that hide latency.
-// (<= 4096: three CTAs per SM as before -- naming a minimum of 1 let ptxas take 111 registers and cost 15 % at 4096.)
+// (<= 4096: three CTAs per SM -- naming a minimum of 1 lets ptxas take more registers than three CTAs allow.)
 template <int LOG2N> struct FftCfg { static constexpr int THREADS = LOG2N >= 14 ? 512 : 256, MINB = LOG2N >= 14 ? 1 : (LOG2N == 13 ? 2 : 3); };
 
 template <int LOG2N, int TH, int MINB>

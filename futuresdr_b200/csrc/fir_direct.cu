@@ -1,4 +1,4 @@
-// fir_direct.cu -- CUDA-core direct-form FIR / decimating FIR for sm_100a.
+// fir_direct.cu -- CUDA-core direct-form FIR / decimating FIR for sm_90a.
 //
 // Computes the reference's   o[k] = sum_t i[D-1 + k*D + t] * taps[N-1-t]
 // (crates/futuredsp/src/fir.rs:77-88 for D == 1, decimating_fir.rs:80-92 for D > 1) for the
@@ -25,11 +25,8 @@ namespace {
 
 __device__ __forceinline__ int swz(int chunk) { return chunk ^ ((chunk >> 3) & 7); }
 
+using ::mac;   // complex sample x real tap (common.cuh)
 __device__ __forceinline__ void mac(float &a, float x, float t) { a = fmaf(x, t, a); }
-__device__ __forceinline__ void mac(float2 &a, float2 x, float t) {
-    a.x = fmaf(x.x, t, a.x);
-    a.y = fmaf(x.y, t, a.y);
-}
 // Complex tap: accum + sample*tap, re = xr*tr - xi*ti, im = xr*ti + xi*tr (fir.rs:257-276)
 __device__ __forceinline__ void mac(float2 &a, float2 x, float2 t) {
     a.x = fmaf(x.x, t.x, a.x);
@@ -80,14 +77,8 @@ template <typename S, typename T, int R>
 __device__ __forceinline__ void mac_chunk(S (&acc)[R], const S (&lo)[R], const S (&hi)[R], const T (&tp)[R]) {
 #pragma unroll
     for (int j = 0; j < R; j++) {
-        if constexpr (sizeof(S) == 8 && sizeof(T) == 4) {          // complex sample x real tap: one FFMA2 per MAC
-            const unsigned long long tt = dup2(tp[j]);
 #pragma unroll
-            for (int r = 0; r < R; r++) cmac2(acc[r], (r + j < R) ? lo[(r + j) % R] : hi[(r + j) % R], tt);
-        } else {
-#pragma unroll
-            for (int r = 0; r < R; r++) mac(acc[r], (r + j < R) ? lo[(r + j) % R] : hi[(r + j) % R], tp[j]);
-        }
+        for (int r = 0; r < R; r++) mac(acc[r], (r + j < R) ? lo[(r + j) % R] : hi[(r + j) % R], tp[j]);
     }
 }
 // one phase row: nchunk chunks of R taps against the thread's sliding window starting at segment seg0
@@ -219,8 +210,8 @@ fir_direct_kernel(const S *__restrict__ in, S *__restrict__ out, const T *__rest
             *reinterpret_cast<float4 *>(xs + swz(c) * 16) = v;
         }
     } else if (vec_ok) {
-        // Decimator: 16-byte loads, four in flight per thread (the scalar loop below kept too few bytes
-        // in flight to cover HBM latency: 43 % of the roofline for D = 4), then scatter the EPC items of
+        // Decimator: 16-byte loads, four in flight per thread (the scalar loop below keeps too few bytes
+        // in flight to cover HBM latency), then scatter the EPC items of
         // each chunk into their phase rows.  (q, m) of a thread's chunks advance by a fixed step, so
         // there is one integer division per thread, not per item.  s0 * sizeof(S) is a multiple of 16.
         const int total = D * W;

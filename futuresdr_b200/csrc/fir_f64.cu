@@ -1,6 +1,6 @@
 // fir_f64.cu -- the f64 x f64 Filter impls (crates/futuredsp/src/fir.rs:217-226, decimating_fir.rs:117-130):
 //     o[k] = sum_t i[D-1 + k*D + t] * taps[N-1-t]      accumulated in tap order, `accum + sample * tap`
-// B200 has little FP64 throughput and no SDR graph of the reference runs its hot path in f64 (the impl exists for
+// The GPU has little FP64 throughput and no SDR graph of the reference runs its hot path in f64 (the impl exists for
 // the known-answer tests, fir.rs:343-365), so this is the plain form: one thread per output, taps in shared memory,
 // UN-FUSED multiply and add in the reference's order -- bit-identical to the stable-Rust loop.
 #include "fir.cuh"

@@ -7,8 +7,7 @@
 // outputs that do not wrap.  One CTA owns one block: forward transform, spectrum product and
 // inverse transform all happen in ONE kernel with the block resident in (padded) shared memory
 // -- HBM sees 8 B in (x NF/V overlap, mostly L2 hits) + 8 B out per sample, instead of the
-// 4*N FLOP per sample of the direct form (4096 FLOP/sample at 1024 taps: 15 Gsamples/s on CUDA
-// cores).  Radix-16 Stockham passes from fft_common.cuh; H is computed in f64 on the host.
+// 4*N FLOP per sample of the direct form (4096 FLOP/sample at 1024 taps).  Radix-16 Stockham passes from fft_common.cuh; H is computed in f64 on the host.
 // Parity: |err| <~ 1e-6 * rms(y) * sqrt(log2 NF), far inside 1e-5 * ||taps||_1 * max|x|.
 #include <cmath>
 #include <cstdlib>
@@ -33,8 +32,8 @@ struct FftFirArgs {
     int V;              // valid outputs per block
 };
 
-// MINB = CTAs per SM the register allocation must allow: the unconstrained build took 171 registers = ONE 256-thread
-// CTA per SM (ncu: 12 % of the warp slots active); 128 registers (no spills) give two, 80 (288 B of spills) three.
+// MINB = CTAs per SM the register allocation must allow: the unconstrained build takes ONE 256-thread CTA per SM by
+// registers; MINB = 2 caps it at 128 registers for two.
 template <int MINB>
 __global__ void __launch_bounds__(kFfThreads, MINB) fir_fft_kernel(const FftFirArgs a) {
     constexpr int N = kNF, T = kFfThreads;

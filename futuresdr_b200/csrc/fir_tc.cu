@@ -1,4 +1,4 @@
-// fir_tc.cu -- tcgen05 (5th-gen tensor core) FIR for 16..257 real taps on sm_100a.
+// fir_tc.cu -- wgmma (Hopper tensor core) FIR for 16..257 real taps on sm_90a.
 //
 // Computes the same  o[k] = sum_t i[k+t] * taps[N-1-t]  as crates/futuredsp/src/fir.rs:77-88
 // (Complex<f32> or f32 samples, f32 taps; decimating_fir.rs:80-92 for a decimation D | 128: the epilogue keeps
@@ -10,26 +10,26 @@
 //                                    extended by the following blocks)         -- "samples"
 //      => D[p][c] = y[128*block(c) + p]
 //
-//  * A is constant: it lives in TENSOR MEMORY for the whole (persistent) kernel, written once
-//    per CTA with tcgen05.st -- the MMAs are issued in the .ts form (A from TMEM, B from smem),
-//    so the only shared-memory operand traffic is the sample tile itself.
+//  * A is constant and Toeplitz, so it is stored ALIASED: the rows are kept in reversed order
+//    (row p' = 127 - p), which makes A[p'][kappa] a function of kappa + p' alone.  In the
+//    no-swizzle K-major layout (8x8 core matrices of 128 bytes) core matrix (row group a, K group j)
+//    then only depends on a + j, and one descriptor with LBO = SBO = 128 bytes walks a strip of
+//    K/8 + 15 core matrices (~8 KiB per precision instead of 96 KiB for the full 128 x 384 matrix).
 //  * FP32 accuracy on bf16 tensor cores: x = x_hi + x_lo, g = g_hi + g_lo (bf16 each) and
-//    x*g ~= x_hi*g_hi + x_lo*g_hi + x_hi*g_lo, three kind::f16 MMAs accumulating in FP32 in
-//    TMEM.  Dropped terms are O(2^-17) relative per product (DESIGN.md "tensor FIR numerics").
+//    x*g ~= x_hi*g_hi + x_lo*g_hi + x_hi*g_lo, three bf16 wgmma accumulating in FP32 registers.
+//    Dropped terms are O(2^-17) relative per product (DESIGN.md "tensor FIR numerics").
 //  * B rows are K-major, 128-byte swizzled.  K-block d of row (stream, block b) is row
 //    (stream, block b+d): a shifted view of the same tile.  Rows are stored so that the shift
 //    is a whole 8-row swizzle atom: physical atom gamma holds blocks {gamma + 16*jb}; the view
 //    for shift d starts at atom d (descriptor base + 1024*d bytes).  Atoms 16, 17 duplicate the
 //    rows they alias (12 % extra conversion work, no extra HBM traffic).
-//  * 18 warps, one persistent CTA per SM, everything handed over with mbarriers:
-//      warp 17    TMA loader : cp.async.bulk (UBLKCP) of the raw f32 samples into a 6 x 8 KiB ring
+//  * 17 warps, one persistent CTA per SM, everything handed over with mbarriers:
+//      warp 16    TMA loader : cp.async.bulk of the raw f32 samples into a 6 x 8 KiB ring
 //      warps 8-15 converters : LDS.128 -> bf16 hi/lo split (cvt.rn.bf16x2) -> swizzled st.shared
 //                              into one of two 72 KiB operand stages
-//      warp 16    MMA issuer : 72 tcgen05.mma per tile (DK x 8 K-steps x 3 products), one elected thread
-//      warps 0-7  epilogue   : tcgen05.ld -> 16 KiB staging -> cp.async.bulk shared->global stores
-//  * What bounds it (profiles/README.md, DESIGN.md section 7): with 256 taps the tensor pipe is busy 86 %
-//    of the time and the SM clock sits at ~1.4 GHz under the board power cap (3 products x K = 384 is
-//    0.31 TFLOP per 64 Mi-sample chunk); below ~130 taps the HBM stream is the bound.
+//      warps 0-7  two math warpgroups, 64 output phases (M rows) each: 72 wgmma.m64n128k16 per tile
+//                 (DK x 8 K-steps x 3 products) into 64 FP32 accumulator registers per thread, then the
+//                 stores of those outputs straight from the registers.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -47,51 +47,23 @@ constexpr int kStages = 2;                  // bf16 operand stages (72 KiB each)
 constexpr int kRawSlots = B2S_RAW_SLOTS;    // raw f32 staging ring, 8 KiB per slot (TMA bulk copies)
 constexpr int kRawSlotBytes = 8192;
 constexpr int kNumProducerThreads = 256;    // 8 converter warps
-constexpr int kNumEpilogueThreads = 256;    // 8 warps: two per TMEM lane quarter, 64 columns each
-constexpr int kThreadsTC = kNumProducerThreads + kNumEpilogueThreads + 64;   // + MMA warp + TMA warp = 576
+constexpr int kNumMathThreads = 256;        // 2 warpgroups: wgmma + epilogue
+constexpr int kThreadsTC = kNumMathThreads + kNumProducerThreads + 32;   // + TMA warp = 544
 constexpr int kProdWarps = kNumProducerThreads / 32;
-constexpr int kEpiWarp0 = 0;                // warps 0..7 epilogue (warp % 4 = TMEM lane quarter)
-constexpr int kEpiWarps = kNumEpilogueThreads / 32;
-constexpr int kProdWarp0 = kEpiWarp0 + kEpiWarps;   // warps 8..15 converters
-constexpr int kMmaWarp = kProdWarp0 + kProdWarps;   // warp 16
-constexpr int kTmaWarp = kMmaWarp + 1;              // warp 17
+constexpr int kMathWarps = kNumMathThreads / 32;
+constexpr int kProdWarp0 = kMathWarps;               // warps 8..15 converters
+constexpr int kTmaWarp = kProdWarp0 + kProdWarps;    // warp 16
 constexpr int kAtomsOut = 16;                // N = 128 columns = 16 swizzle atoms of 8 rows
-constexpr int kNTile = 8 * kAtomsOut;
-constexpr int kMaxDK = 3;                    // K <= 384  (TMEM: K columns of taps + 128 of accumulators)
+constexpr int kMaxDK = 3;                    // K <= 384
 constexpr int kSplitBytesMax = (kAtomsOut + kMaxDK - 1) * 1024 * 2;   // per split: 2 K-chunks x 18 atoms
 constexpr int kStageBytes = 2 * kSplitBytesMax;                       // hi + lo = 72 KiB
-constexpr int kOutStageBytes = 16384;        // output staging: 16 blocks of 128 complex items (one bulk store), double-buffered
-constexpr int kOutStages = 2;
-constexpr int kTapsSmemBytes = 1040;         // <= 257 reversed taps staged once for the Toeplitz fill
-constexpr int kSmemTC = kStages * kStageBytes + kRawSlots * kRawSlotBytes + kOutStages * kOutStageBytes + 1024 /*align*/ +
-                        256 /*barriers*/ + kTapsSmemBytes;
+constexpr int kACores = kMaxDK * 16 + 15;    // core matrices of the aliased Toeplitz strip (K/8 + 128/8 - 1)
+constexpr int kABytes = kACores * 128;       // per precision (hi, lo)
+constexpr int kSmemTC = kStages * kStageBytes + kRawSlots * kRawSlotBytes + 2 * kABytes + 1024 /*align*/ + 256 /*barriers*/;
 static_assert(kSmemTC <= 227 * 1024, "tensor FIR shared memory exceeds the 227 KiB per-CTA limit");
 
 // ---- PTX helpers ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// Optional per-role cycle accounting (build with -DB2S_TC_TIMING, run with B2S_TC_TIMING_DUMP=1): every role's
-// lane 0 accumulates clock64() laps into 16 counters per CTA; scripts/build_variant.sh builds the variant.
-// epilogue store flavour: plain (default) or streaming (st.global.cs, -DB2S_TC_ST_CS) -- A/B switch
-#ifdef B2S_TC_ST_CS
-#define B2S_TC_STORE(ptr, val) __stcs((ptr), (val))
-#else
-#define B2S_TC_STORE(ptr, val) (*(ptr) = (val))
-#endif
-#ifdef B2S_TC_TIMING
-__device__ long long g_tc_timing[256 * 16];
-#define TCT_DECL(n) long long tct_[n] = {}; long long tct_t0_ = clock64();
-#define TCT_LAP(i) { const long long t_ = clock64(); tct_[i] += t_ - tct_t0_; tct_t0_ = t_; }
-#define TCT_DUMP(base, n) { for (int i_ = 0; i_ < (n); i_++) g_tc_timing[blockIdx.x * 16 + (base) + i_] = tct_[i_]; }
-#define TCT_START const long long tct_k0_ = clock64();
-#define TCT_MARK(i) { g_tc_timing[blockIdx.x * 16 + (i)] = clock64() - tct_k0_; }
-#else
-#define TCT_START
-#define TCT_MARK(i) {}
-#define TCT_DECL(n)
-#define TCT_LAP(i) {}
-#define TCT_DUMP(base, n) {}
-#endif
 
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
@@ -112,122 +84,63 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {}
 }
 // one thread of a converged warp; unlike `lane == 0` the compiler knows exactly one thread is active, so
-// uniform-datapath instructions (UTCHMMA, UBLKCP) are emitted bare instead of inside an ELECT retry loop
+// uniform-datapath instructions (UBLKCP) are emitted bare instead of inside an ELECT retry loop
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
-#ifdef B2S_TC_NO_ELECT
-    pred = (threadIdx.x & 31) == 0;             // A/B switch: the plain lane-0 guard
-#else
     asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-#endif
     return pred != 0;
 }
-// shared -> global bulk copy (TMA store, SASS UBLKCP.G.S) in the issuing thread's bulk async-group
-__device__ __forceinline__ void bulk_store(void *gdst, uint32_t ssrc, uint32_t bytes) {
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(ssrc), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kNumEpilogueThreads) : "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]   (kind::f16: bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                        uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// d[64] (+)= A[smem desc] * B[smem desc]   (m64n128k16, bf16 inputs, fp32 accumulate, both operands K-major)
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+        "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+        "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"r"(taddr),
-                 "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// f32 pair -> packed bf16x2 {lo16 = a, hi16 = b}, round-to-nearest-even, on the INTEGER pipes.
-// (cvt.rn.bf16x2.f32 is an XU-pipe instruction, 16 lanes/clk/SM: with 4 conversions per loaded
-// float4 it was the busiest unit of the kernel -- ncu: sm__inst_executed_pipe_xu 91 %.)
-// RNE on the bit pattern: r = u + 0x7FFF + ((u >> 16) & 1); bf16 = r >> 16.  Identical to
-// cvt.rn for every finite input (inf stays inf; NaN payloads may change, samples are finite).
-__device__ __forceinline__ uint32_t rne_bias(float x) {
-    const uint32_t u = __float_as_uint(x);
-    return u + 0x7FFFu + ((u >> 16) & 1u);
-}
-// f32 pair -> packed bf16x2 on the XU pipe (one instruction)
+// f32 pair -> packed bf16x2 {lo16 = a, hi16 = b}, round-to-nearest-even (one XU instruction)
 __device__ __forceinline__ uint32_t cvt_bf16x2(float a, float b) {
     uint32_t r;
     asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));
     return r;
 }
 // split (a, b) into bf16 hi pair and bf16 lo pair:  x ~= hi + lo.
-// B2S_SPLIT_MODE 0: integer pipes only; 1: hi on the XU (cvt), lo on the integer pipes; 2: both on the XU.
-// The producer warps are issue-limited, so trading 7 ALU instructions for 1 XU instruction pays
-// as long as the XU (16 lanes/clk/SM) keeps up: 2 cvt per float4 = ~530 XU cycles per 8192-sample tile.
-#ifndef B2S_SPLIT_MODE
-#define B2S_SPLIT_MODE 2
-#endif
 __device__ __forceinline__ void split2(float a, float b, uint32_t &hi, uint32_t &lo) {
-#if B2S_SPLIT_MODE == 0
-    const uint32_t ra = rne_bias(a), rb = rne_bias(b);
-    hi = __byte_perm(ra, rb, 0x7632);                               // {rb.hi16, ra.hi16}
-    const float ah = __uint_as_float(ra & 0xffff0000u), bh = __uint_as_float(rb & 0xffff0000u);
-    lo = __byte_perm(rne_bias(a - ah), rne_bias(b - bh), 0x7632);
-#else
     hi = cvt_bf16x2(a, b);
     const float ah = __uint_as_float(hi << 16), bh = __uint_as_float(hi & 0xffff0000u);
-#if B2S_SPLIT_MODE == 1
-    lo = __byte_perm(rne_bias(a - ah), rne_bias(b - bh), 0x7632);
-#else
     lo = cvt_bf16x2(a - ah, b - bh);
-#endif
-#endif
 }
 
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row atoms 1024 B apart
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-//  layout_type [61,64) = 2)
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)1 << 16;                 // LBO (unused for swizzled K-major) = 16 B
-    d |= (uint64_t)(1024 >> 4) << 32;       // SBO = 1024 B between 8-row atoms
-    d |= (uint64_t)1 << 46;                 // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                 // SWIZZLE_128B
-    return d;
+// wgmma shared-memory matrix descriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), layout [62,64)
+// (0 = no swizzle, 1 = 128-byte swizzle)
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo, uint32_t layout) {
+    return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
+           ((uint64_t)layout << 62);
 }
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): D=f32, A=B=bf16, K-major both, M=128, N=64
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// samples: K-major, SWIZZLE_128B, 8-row atoms 1024 B apart (LBO unused)
+__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) { return make_desc(smem_addr, 16, 1024, 1); }
+// aliased Toeplitz taps: no swizzle, the next core matrix along K and along M is the same 128 bytes further
+__device__ __forceinline__ uint64_t make_a_desc(uint32_t smem_addr) { return make_desc(smem_addr, 128, 128, 0); }
 
 struct TcParams {
     const float *in;      // samples (float2 when COMPLEX)
@@ -238,8 +151,7 @@ struct TcParams {
     int ntaps;
     int DK;               // K blocks of 128
     int num_tiles;
-    int flags;            // bit0: swap bf16 halves of the TMEM A words (bring-up switch)
-    int out_bulk;         // out is 16-byte aligned: interior tiles leave through bulk (TMA) stores
+    int flags;            // tuning switches: bit1 skip the stores, bit2 skip the MMAs, bit3 skip the conversion
     int decim;            // D | 128: only the output phases p == D-1 (mod D) are stored (decimating FIR)
     // ---- misaligned / detached history (b2s_fir_exec_hist) -------------------------------------------------
     // The kernel's item coordinate i is:  [0, lead) dummy items that only exist to keep every bulk copy 16-byte
@@ -260,39 +172,30 @@ struct TcParams {
 };
 
 // ---------------------------------------------------------------------------------------------
-// Tile = N_TILE = 128 columns = 16 swizzle atoms of 8 rows.
+// Tile = 128 columns = 16 swizzle atoms of 8 rows.
 // COMPLEX: rows are (stream ri, block b); 64 blocks x 128 complex samples per tile, column
 //          c = 8*gamma + 2*jb + ri  <->  block b0 + gamma + 16*jb   (gamma < 16, jb < 4)
 // REAL   : 128 blocks x 128 samples per tile, column c = 8*gamma + j <-> block b0 + gamma + 16*j.
-// Why N = 128: a tcgen05.mma (M=128, K=16) never takes less than 48 cycles on B200, whatever N
-// (measured, scripts/mma_rate.cu: N<=64 -> 48 cyc, N=128 -> 64, N=256 -> 128), so N = 64 tiles
-// ran the tensor pipe at 2/3 efficiency.  TMEM holds K columns of taps (hi+lo) + accumulators
-// of 128 columns: two accumulators when K <= 256 (ntaps <= 129), one when K = 384.
+// In the wgmma accumulator layout a thread holds columns 8*gamma + 2*(lane%4) + {0,1}: the (re, im) pair of
+// one complex output, or two real outputs 16 blocks apart.
 // ---------------------------------------------------------------------------------------------
 template <bool COMPLEX>
 __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams prm) {
     extern __shared__ unsigned char smem_raw[];
-    TCT_START
     // 1024-byte alignment for the 128B-swizzle atoms
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     unsigned char *gen_base = smem_raw + (base - raw);
     const uint32_t raw_base = base + kStages * kStageBytes;           // raw f32 ring
     unsigned char *raw_gen = gen_base + kStages * kStageBytes;
-    const uint32_t ost_base = raw_base + kRawSlots * kRawSlotBytes;   // output staging (epilogue -> bulk stores)
-    unsigned char *ost_gen = raw_gen + kRawSlots * kRawSlotBytes;
-    const uint32_t bar_base = ost_base + kOutStages * kOutStageBytes;
-    // barriers: full[kStages], empty[kStages], tfull[2], tempty[2], rfull[kRawSlots], rempty[kRawSlots], tmem slot
+    const uint32_t a_base = raw_base + kRawSlots * kRawSlotBytes;     // Toeplitz strip: hi, then lo
+    __nv_bfloat16 *a_gen = reinterpret_cast<__nv_bfloat16 *>(raw_gen + kRawSlots * kRawSlotBytes);
+    const uint32_t bar_base = a_base + 2 * kABytes;
+    // barriers: full[kStages], empty[kStages], rfull[kRawSlots], rempty[kRawSlots]
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-    auto tfull_bar = [&](int a) { return bar_base + 8u * (2 * kStages + a); };
-    auto tempty_bar = [&](int a) { return bar_base + 8u * (2 * kStages + 2 + a); };
-    auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * kStages + 4 + r); };
-    auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * kStages + 4 + kRawSlots + r); };
-    constexpr int kNumBars = 2 * kStages + 4 + 2 * kRawSlots;
-    const uint32_t tmem_slot = bar_base + 8u * kNumBars;
-    volatile uint32_t *tmem_slot_gen = reinterpret_cast<volatile uint32_t *>(
-        gen_base + kStages * kStageBytes + kRawSlots * kRawSlotBytes + kOutStages * kOutStageBytes + 8 * kNumBars);
+    auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * kStages + r); };
+    auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * kStages + kRawSlots + r); };
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (prm.pub_flag && blockIdx.x == 0 && threadIdx.x == 0) {
@@ -300,7 +203,6 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(prm.pub_flag), "r"(prm.pub_value) : "memory");
     }
     const int DK = prm.DK, K = 128 * DK;
-    const int nacc = (512 - K) / kNTile;             // accumulators that fit next to the taps (1 or 2)
     const int atoms = kAtomsOut + DK - 1;            // physical 8-row atoms per K-chunk
     const int chunk_bytes = atoms * 1024;            // one K-chunk (64 elements) of all rows
     const int split_bytes = 2 * chunk_bytes;
@@ -308,52 +210,25 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
     constexpr int TILE_BLOCKS = kAtomsOut * NSEQ;    // 64 / 128 blocks of 128 samples
     constexpr long long TILE_ITEMS = (long long)TILE_BLOCKS * 128;
 
-    if (warp == kMmaWarp) {
-        if (lane == 0) {
-            for (int s = 0; s < kStages; s++) { mbar_init(full_bar(s), kProdWarps); mbar_init(empty_bar(s), 1); }
-            for (int a = 0; a < 2; a++) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), kEpiWarps); }
-            for (int r = 0; r < kRawSlots; r++) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), kProdWarps); }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc(tmem_slot, 512);
+    if (warp == kTmaWarp && lane == 0) {
+        for (int s = 0; s < kStages; s++) { mbar_init(full_bar(s), kProdWarps); mbar_init(empty_bar(s), kMathWarps); }
+        for (int r = 0; r < kRawSlots; r++) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), kProdWarps); }
+        fence_barrier_init();
     }
-    // reversed taps -> shared memory (one coalesced pass; the Toeplitz fill below reads them 48 times per lane)
-    float *gs = reinterpret_cast<float *>(gen_base + kStages * kStageBytes + kRawSlots * kRawSlotBytes +
-                                          kOutStages * kOutStageBytes + 256);
-    for (int i = threadIdx.x; i < prm.ntaps; i += kThreadsTC) gs[i] = __ldg(prm.g + i);
-    tc_fence_before();
+    // ---- one-time: the aliased Toeplitz strip.  Core matrix s, row r, element e (byte 128*s + 16*r + 2*e) holds
+    // A[p'][kappa] for every p' = 8a + r, kappa = 8j + e with a + j = s:  g[kappa - p - lead], p = 127 - p'
+    // (`lead` zero taps in front meet the dummy items).
+    const int a_elems = (K / 8 + 15) * 64;
+    for (int i = threadIdx.x; i < a_elems; i += kThreadsTC) {
+        const int s = i >> 6, r = (i >> 3) & 7, e = i & 7;
+        const int t = 8 * s + r + e - 127 - prm.lead;
+        const float gv = (t >= 0 && t < prm.ntaps) ? __ldg(prm.g + t) : 0.0f;
+        const __nv_bfloat16 hi = __float2bfloat16_rn(gv);
+        a_gen[i] = hi;
+        a_gen[kABytes / 2 + i] = __float2bfloat16_rn(gv - __bfloat162float(hi));
+    }
+    fence_proxy_async();                             // generic-proxy stores -> visible to wgmma (async proxy)
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot_gen;
-    const uint32_t tmem_acc = tmem + (uint32_t)K;    // columns [K, 512): accumulators
-
-    // ---- one-time: Toeplitz taps into TMEM (epilogue warps 0..3 own lanes 32*warp..).  Only the MMA warp
-    // depends on it, so it alone waits (named barrier 2: 4 filler warps + the MMA warp); the TMA loader and
-    // the converters start streaming the first tiles while the table is being written.
-    if (warp >= kEpiWarp0 && warp < kEpiWarp0 + 4) {
-        const int q = warp - kEpiWarp0, p = 32 * q + lane;   // TMEM lane = output phase p
-        const uint32_t lane_addr = tmem + ((uint32_t)(32 * q) << 16);
-        for (int c0 = 0; c0 < K / 2; c0 += 8) {
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const int k0 = 2 * (c0 + i) - p - prm.lead, k1 = k0 + 1;   // `lead` zero taps in front (dummy items)
-                const float g0 = (k0 >= 0 && k0 < prm.ntaps) ? gs[k0] : 0.0f;
-                const float g1 = (k1 >= 0 && k1 < prm.ntaps) ? gs[k1] : 0.0f;
-                if (prm.flags & 1) split2(g1, g0, hi[i], lo[i]);
-                else split2(g0, g1, hi[i], lo[i]);
-            }
-            tmem_st8(lane_addr + (uint32_t)c0, hi);
-            tmem_st8(lane_addr + (uint32_t)(K / 2 + c0), lo);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        asm volatile("bar.sync 2, 160;" ::: "memory");
-    } else if (warp == kMmaWarp) {
-        asm volatile("bar.sync 2, 160;" ::: "memory");
-        tc_fence_after();
-    }
 
     // A tile's contiguous input span (TILE_BLOCKS + DK - 1 blocks of 128 items) travels through the raw
     // ring in slots of 8 KiB = 512 float4 (8 complex blocks / 16 real blocks); 9 slots per tile.
@@ -365,16 +240,12 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
 
     if (warp == kTmaWarp) {
         // ================================ TMA LOADER ===========================================
-        // One thread streams the input with bulk async copies (cp.async.bulk, UBLKCP): the copies
-        // complete on the slot's mbarrier (complete_tx), so HBM latency is absorbed by the 64 KiB
-        // ring and never by a converter warp's registers.
+        // One thread streams the input with bulk async copies (cp.async.bulk): the copies complete on the
+        // slot's mbarrier (complete_tx), so HBM latency is absorbed by the 48 KiB ring and never by a
+        // converter warp's registers.
         if (elect_one()) {
             int rs = 0;
             uint32_t rphase = 0;
-            TCT_DECL(2)
-            // (A whole-tile cp.async.bulk.prefetch.L2 two tiles ahead was tried: 63 % L2 read hit rate, but
-            // 1.3 % SLOWER -- the ring already covers HBM latency and the kernel runs power-capped, so the
-            // extra L2 traffic only costs clock.)
             for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
                 const long long item0 = (long long)tile * TILE_ITEMS;
 #pragma unroll 1
@@ -386,9 +257,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
                     long long items = (long long)nblk * 128;
                     if (it0 + items > prm.n_in) items = prm.n_in - it0;
                     long long bytes = items > 0 ? ((items * ITEM_BYTES) & ~15ll) : 0;    // whole 16-byte units
-                    TCT_LAP(1)
                     mbar_wait(rempty_bar(rs), rphase ^ 1);
-                    TCT_LAP(0)
                     if (tile == 0 && s == 0 && prm.hist_items > 0) {
                         // detached history: items [0, hist_items) come from `hist` (the left neighbour's tail over
                         // NVLink when it is peer memory), the rest of the slot from the caller's slice.
@@ -425,18 +294,15 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
                     if (++rs == kRawSlots) { rs = 0; rphase ^= 1; }
                 }
             }
-            TCT_DUMP(9, 2)
         }
         __syncwarp();
-    } else if (warp >= kProdWarp0 && warp < kMmaWarp) {
+    } else if (warp >= kProdWarp0) {
         // ================================ CONVERTERS ===========================================
         // 256 threads; thread t owns float4 #t and #(t+256) of every raw slot.  Its position inside a
         // 128-item block (fo) and its row inside a slot (rowsel) never change, and the slot / float4
         // loops are fully unrolled, so every shared-memory address is
         //     stage base + per-thread constant + compile-time constant + one of 8 precomputed swizzle offsets.
         // Per float4: one LDS.128, two XU conversions per value pair, 4 (8 for aliased rows) 32-bit stores.
-        // (The first version of this loop spent ~120 instructions per float4 on address arithmetic and
-        // bounds predicates and was the busiest part of the SM; interior tiles now take a check-free path.)
         const int tid = threadIdx.x - 32 * kProdWarp0;                   // 0..255
         const int fo = tid % F4_PER_BLOCK, rowsel = tid / F4_PER_BLOCK;  // rowsel 0..3 (complex) / 0..7 (real)
         const int kc = COMPLEX ? (fo >> 5) : (fo >> 4);
@@ -448,7 +314,6 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         for (int j = 0; j < 8; j++) xj[j] = (uint32_t)(j * 128 + ((c16 ^ j) << 4));
         const bool alias_thread = rowsel < DK - 1;                        // this thread's rows alias into atoms 16, 17
         const uint32_t sb = (uint32_t)split_bytes;
-        TCT_DECL(3)
 
         // compile-time geometry of (slot s, float4 i): block bl = BLOCKS_PER_SLOT*s + rowsel + ROWS*i = gamma + 16*seq
         //   complex: gamma = 8*(s&1) + 4*i + rowsel, seq = s>>1 ;  real: gamma = 8*i + rowsel, seq = s
@@ -458,9 +323,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
 #pragma unroll
             for (int s = 0; s < SLOTS_PER_TILE; s++) {
                 if (s * BLOCKS_PER_SLOT >= in_blocks) break;
-                TCT_LAP(1)
                 mbar_wait(rfull_bar(rs), rphase);
-                TCT_LAP(2)
                 const float4 *raw = reinterpret_cast<const float4 *>(raw_gen + rs * kRawSlotBytes);
                 float4 v[2];
                 v[0] = raw[tid];
@@ -542,9 +405,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
             const long long item0 = (long long)tile * TILE_ITEMS;
             const bool interior = item0 + (long long)in_blocks * 128 <= prm.n_in &&
                                   !(tile == 0 && (prm.lead | prm.hist_items) != 0);   // tile 0 zeroes the dummy items
-            TCT_LAP(1)
             mbar_wait(empty_bar(stage), phase ^ 1);
-            TCT_LAP(0)
             unsigned char *stage_ptr = gen_base + stage * kStageBytes;
             if (interior) convert_tile(std::true_type{}, stage_ptr, item0, rs, rphase);
             else convert_tile(std::false_type{}, stage_ptr, item0, rs, rphase);
@@ -553,158 +414,79 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
             if (lane == 0) mbar_arrive(full_bar(stage));
             if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
-        if (tid == 0) TCT_DUMP(6, 3)
-    } else if (warp == kMmaWarp) {
-        // ================================ MMA ISSUER ===========================================
-        if (elect_one()) {
-            const uint32_t idesc = make_idesc(128, kNTile);
-            int stage = 0, acc = 0;
-            uint32_t phase = 0, accphase = 0;
-            TCT_DECL(3)
-            TCT_MARK(11)
-            for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
-                TCT_LAP(2)
-                mbar_wait(full_bar(stage), phase);
-                TCT_LAP(0)
-                mbar_wait(tempty_bar(acc), accphase ^ 1);
-                TCT_LAP(1)
-                tc_fence_after();
-                const uint32_t sbase = base + stage * kStageBytes;
-                const uint32_t d_tmem = tmem_acc + (uint32_t)(kNTile * acc);
-                uint32_t accum = 0;
-                for (int d = 0; d < ((prm.flags & 4) ? 0 : DK); d++) {   // flags bit2: tuning switch, skip the MMAs
+    } else {
+        // ================================ MATH WARPGROUPS ======================================
+        // Warpgroup wg computes the accumulator rows p' = 64*wg .. 64*wg+63 (output phases p = 127 - p') of
+        // all 128 columns.  Thread (warp w, lane) holds rows 16*(w%4) + lane/4 + {0, 8} of its warpgroup and
+        // columns 8*gamma + 2*(lane%4) + {0, 1}: acc[4*gamma + 2*h + e].
+        const int wg = warp >> 2, wl = warp & 3, q4 = lane & 3;
+        // Decimation (decimating_fir.rs:80-92: o[k] = y[D-1 + k*D] of the full-rate FIR y): the MMAs still
+        // produce every phase -- the kernel is HBM-bound below ~130 taps -- and the epilogue keeps the phases
+        // p == D-1 (mod D).  D divides 128, so the kept phases are the same in every block and block b
+        // contributes the 128/D outputs  k = b*(128/D) + (p-(D-1))/D.
+        const int D = prm.decim, per_blk = 128 / D;
+        const uint32_t a_hi = a_base + 1024u * wg, a_lo = a_hi + kABytes;   // row group a = 8*wg + a_local
+        float acc[64];
 #pragma unroll
-                    for (int kc = 0; kc < 2; kc++) {
+        for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+            mbar_wait(full_bar(stage), phase);
+            wgmma_fence();                           // the previous tile's register reads precede the async writes
+            const uint32_t sbase = base + stage * kStageBytes;
+            uint32_t accum = 0;
+            for (int d = 0; d < ((prm.flags & 4) ? 0 : DK); d++) {   // flags bit2: tuning switch, skip the MMAs
 #pragma unroll
-                        for (int ks = 0; ks < 4; ks++) {
-                            // Toeplitz columns kappa >= ntaps + 127 hold no tap: skip those K-steps
-                            if (d * 128 + kc * 64 + ks * 16 >= prm.ntaps + prm.lead + 127) continue;
-                            const uint32_t kcol = (uint32_t)(d * 64 + kc * 32 + ks * 8);       // A column (2 bf16 / column)
-                            const uint32_t boff = (uint32_t)(kc * chunk_bytes + d * 1024 + ks * 32);
-                            const uint64_t bh = make_b_desc(sbase + boff);
-                            const uint64_t bl = make_b_desc(sbase + split_bytes + boff);
-                            umma_ts(d_tmem, tmem + kcol, bh, idesc, accum);                     // g_hi * x_hi
-                            umma_ts(d_tmem, tmem + kcol, bl, idesc, 1u);                        // g_hi * x_lo
-                            umma_ts(d_tmem, tmem + (uint32_t)(K / 2) + kcol, bh, idesc, 1u);    // g_lo * x_hi
-                            accum = 1u;
-                        }
+                for (int kc = 0; kc < 2; kc++) {
+#pragma unroll
+                    for (int ks = 0; ks < 4; ks++) {
+                        // Toeplitz columns kappa >= ntaps + 127 hold no tap: skip those K-steps
+                        const int kappa0 = d * 128 + kc * 64 + ks * 16;
+                        if (kappa0 >= prm.ntaps + prm.lead + 127) continue;
+                        const uint32_t aoff = (uint32_t)(kappa0 / 8) * 128u;                // core matrix a + j
+                        const uint32_t boff = (uint32_t)(kc * chunk_bytes + d * 1024 + ks * 32);
+                        const uint64_t bh = make_b_desc(sbase + boff);
+                        const uint64_t bl = make_b_desc(sbase + split_bytes + boff);
+                        const uint64_t ah = make_a_desc(a_hi + aoff);
+                        wgmma_m64n128(acc, ah, bh, accum);                           // g_hi * x_hi
+                        wgmma_m64n128(acc, ah, bl, 1u);                              // g_hi * x_lo
+                        wgmma_m64n128(acc, make_a_desc(a_lo + aoff), bh, 1u);        // g_lo * x_hi
+                        accum = 1u;
                     }
                 }
-                umma_commit(empty_bar(stage));       // smem stage may be refilled once the MMAs read it
-                umma_commit(tfull_bar(acc));         // accumulator complete
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                if (++acc == nacc) { acc = 0; accphase ^= 1; }
             }
-            TCT_DUMP(0, 3)
-            TCT_MARK(12)
-        }
-        __syncwarp();
-    } else {
-        // ================================ EPILOGUE =============================================
-        // 8 warps: warp w serves TMEM lanes 32*(w%4).. and column half (w-8)/4.  Each warp pulls its
-        // 64 columns with two back-to-back tcgen05.ld and releases the accumulator as soon as they
-        // have landed (the single-accumulator K=384 case stalls the MMA warp until then).
-        // Lane p holds y[128*b + p]; columns sharing jb (the sub-sequence index) belong to 16 consecutive
-        // blocks, i.e. ONE contiguous 16 KiB (complex) / 8 KiB (real) span of the output.  Interior tiles
-        // therefore leave in NSEQ rounds: the 8 warps lay the span out in a staging buffer (every store
-        // instruction writes a contiguous row segment, conflict-free), one thread hands it to the
-        // TMA as a single bulk store, and the next round fills the other buffer meanwhile.  Per-lane
-        // 8-byte global stores (the previous epilogue, still used for the ragged last tile and for
-        // unaligned outputs) kept the warps stalled on the LSU for ~40 % of a tile period.
-        const int ew = warp - kEpiWarp0, q = ew & 3, half = ew >> 2, p = 32 * q + lane;
-        const bool store_thread = threadIdx.x == 32 * kEpiWarp0;
-        // Decimation (decimating_fir.rs:80-92: o[k] = y[D-1 + k*D] of the full-rate FIR y): the MMAs still
-        // produce every phase -- the tensor pipe has the room, the kernel is HBM-bound below ~130 taps -- and
-        // the epilogue keeps the lanes p == D-1 (mod D).  D divides 128, so the kept lanes are the same in
-        // every block and block b contributes the 128/D outputs  k = b*(128/D) + (p-(D-1))/D.
-        const int D = prm.decim, per_blk = 128 / D;
-        const bool lane_on = (p % D) == D - 1;
-        const int pk = (p - (D - 1)) / D;
-        const uint32_t round_bytes = (uint32_t)(kAtomsOut * per_blk * ITEM_BYTES);   // 16 blocks' worth of outputs
-        int acc = 0, obuf = 0;
-        uint32_t accphase = 0;
-        TCT_DECL(3)
-        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
-            TCT_LAP(2)
-            mbar_wait(tfull_bar(acc), accphase);
-            TCT_LAP(0)
-            tc_fence_after();
-            const uint32_t taddr = tmem_acc + (uint32_t)(kNTile * acc + 64 * half) + ((uint32_t)(32 * q) << 16);
-            uint32_t v[2][32];
-            tmem_ld32(taddr, v[0]);
-            tmem_ld32(taddr + 32, v[1]);
-            tmem_wait_ld();
-            tc_fence_before();
+            wgmma_commit();
+            wgmma_wait_all();
             __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));     // accumulator drained -> MMA may reuse it
-            TCT_LAP(1)
+            if (lane == 0) mbar_arrive(empty_bar(stage));   // operand stage read: the converters may refill it
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
+            if (prm.flags & 2) continue;                    // tuning switch: skip the global stores
+
+            // ---- epilogue: for each (h, gamma) a warp writes 4 runs of 8 consecutive outputs (one per lane%4)
             const long long blk0 = (long long)tile * TILE_BLOCKS;
             const bool interior = (blk0 + TILE_BLOCKS) * per_blk <= prm.n_out;
-            if (prm.flags & 2) goto epi_next;           // tuning switch: skip the global stores
-            if (interior && prm.out_bulk) {
 #pragma unroll
-                for (int r = 0; r < NSEQ; r++) {          // r = jb (complex) / j (real)
-                    if (store_thread) bulk_wait_read<kOutStages - 1>();   // the bulk store that last read this buffer is done with it
-                    epi_bar_sync();
-                    unsigned char *buf = ost_gen + obuf * kOutStageBytes;
+            for (int h = 0; h < 2; h++) {
+                const int p = 127 - (64 * wg + 16 * wl + (lane >> 2) + 8 * h);
+                if ((p % D) != D - 1) continue;
+                const int pk = (p - (D - 1)) / D;
 #pragma unroll
-                    for (int c = 0; c < 2; c++) {
-#pragma unroll
-                        for (int gl = 0; gl < 4; gl++) {
-                            const int gam = half * 8 + c * 4 + gl;
-                            if (!lane_on) continue;
-                            if constexpr (COMPLEX) {
-                                reinterpret_cast<float2 *>(buf)[gam * per_blk + pk] =
-                                    make_float2(__uint_as_float(v[c][8 * gl + 2 * r]), __uint_as_float(v[c][8 * gl + 2 * r + 1]));
-                            } else {
-                                reinterpret_cast<float *>(buf)[gam * per_blk + pk] = __uint_as_float(v[c][8 * gl + r]);
-                            }
-                        }
-                    }
-                    fence_proxy_async();                  // generic-proxy writes -> visible to the bulk copy
-                    epi_bar_sync();
-                    if (store_thread)
-                        bulk_store(prm.out + ((blk0 + (long long)kAtomsOut * r) * per_blk) * (COMPLEX ? 2 : 1),
-                                   ost_base + obuf * kOutStageBytes, round_bytes);
-                    obuf ^= 1;
-                }
-                goto epi_next;
-            }
-#pragma unroll
-            for (int c = 0; c < 2; c++) {
-#pragma unroll
-                for (int gl = 0; gl < 4; gl++) {
-                    const int gam = half * 8 + c * 4 + gl;
-                    if (!lane_on) continue;
+                for (int gam = 0; gam < 16; gam++) {
+                    const float v0 = acc[4 * gam + 2 * h], v1 = acc[4 * gam + 2 * h + 1];
                     if constexpr (COMPLEX) {
-                        float2 *o = reinterpret_cast<float2 *>(prm.out) + (blk0 + gam) * per_blk + pk;
-#pragma unroll
-                        for (int jb = 0; jb < 4; jb++) {
-                            const float2 val = make_float2(__uint_as_float(v[c][8 * gl + 2 * jb]),
-                                                           __uint_as_float(v[c][8 * gl + 2 * jb + 1]));
-                            if (interior || (blk0 + gam + kAtomsOut * jb) * per_blk + pk < prm.n_out)
-                                B2S_TC_STORE(o + (long long)kAtomsOut * jb * per_blk, val);
-                        }
+                        const long long k = (blk0 + gam + kAtomsOut * q4) * per_blk + pk;
+                        if (interior || k < prm.n_out) reinterpret_cast<float2 *>(prm.out)[k] = make_float2(v0, v1);
                     } else {
-                        float *o = prm.out + (blk0 + gam) * per_blk + pk;
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            if (interior || (blk0 + gam + kAtomsOut * j) * per_blk + pk < prm.n_out)
-                                B2S_TC_STORE(o + (long long)kAtomsOut * j * per_blk, __uint_as_float(v[c][8 * gl + j]));
-                        }
+                        const long long k0 = (blk0 + gam + kAtomsOut * (2 * q4)) * per_blk + pk;
+                        const long long k1 = k0 + (long long)kAtomsOut * per_blk;
+                        if (interior || k0 < prm.n_out) prm.out[k0] = v0;
+                        if (interior || k1 < prm.n_out) prm.out[k1] = v1;
                     }
                 }
             }
-        epi_next:
-            if (++acc == nacc) { acc = 0; accphase ^= 1; }
         }
-        if (store_thread) bulk_wait_all();               // staging buffers must outlive the bulk stores
-        if (ew == 0 && lane == 0) TCT_DUMP(3, 3)
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kMmaWarp) tmem_dealloc(tmem, 512);
 }
 
 }  // namespace
@@ -782,32 +564,11 @@ int32_t fir_tc_launch_hist(b2s_fir *f, const FirHist *h, const void *d_in, size_
     const long long tile_items = cplx ? 64 * 128 : 128 * 128;
     prm.num_tiles = (int)ceil_div(n_out * f->decim, (size_t)tile_items);   // tiles over the full-rate index space
     prm.flags = f->tc_flags;
-    prm.out_bulk = (a_out & 15) == 0 && !(f->tc_flags & 16);   // flags bit4: force per-lane stores
     const int grid = std::min(prm.num_tiles, ctx->sm_count);
     if (prm.wait_flag) ctx->flag_ops++;
     if (cplx) fir_tc_kernel<true><<<grid, kThreadsTC, kSmemTC, stream>>>(prm);
     else fir_tc_kernel<false><<<grid, kThreadsTC, kSmemTC, stream>>>(prm);
     B2S_CHECK_LAUNCH(ctx);
-#ifdef B2S_TC_TIMING
-    if (getenv("B2S_TC_TIMING_DUMP")) {
-        static int calls = 0;
-        if (++calls == 8) {                       // a warm launch
-            cudaStreamSynchronize(stream);
-            static long long h[256 * 16];
-            cudaMemcpyFromSymbol(h, g_tc_timing, sizeof(h));
-            const char *names[13] = {"mma.wait_full", "mma.wait_tempty", "mma.issue", "epi.wait_tfull", "epi.tmem_ld",
-                                     "epi.stores", "cvt.wait_empty", "cvt.work", "cvt.wait_rfull", "tma.wait_rempty", "tma.issue",
-                                     "mma.loop_start", "mma.loop_end"};
-            const double tiles = (double)prm.num_tiles / grid;
-            for (int i = 0; i < 13; i++) {
-                double sum = 0;
-                for (int b = 0; b < grid; b++) sum += (double)h[b * 16 + i];
-                if (i < 11) fprintf(stderr, "TCT %-16s %9.0f cycles/tile\n", names[i], sum / grid / tiles);
-                else fprintf(stderr, "TCT %-16s %9.0f cycles after kernel entry (mean over CTAs)\n", names[i], sum / grid);
-            }
-        }
-    }
-#endif
     return B2S_OK;
 }
 

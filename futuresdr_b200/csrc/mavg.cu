@@ -26,8 +26,8 @@ namespace {
 // (warp 0), which cannot keep HBM busy on its own, so all 8 warps stream blocks of 64 chunks (64 rows of
 // 128 bytes) into a 4-deep shared-memory ring with cp.async (LDGSTS: no registers held across the wait),
 // three blocks ahead of the one warp 0 is walking.  Operations and their order are the reference's
-// (un-fused IEEE mul/add).  (A register double buffer, one block ahead, spent 4 us per block waiting for
-// a single DRAM round trip: 66 ns per chunk.)
+// (un-fused IEEE mul/add).  (A register double buffer, one block ahead, waits a whole DRAM round trip
+// per block.)
 constexpr int kMaBins = 32, kMaFrames = 64, kMaWarps = 8, kMaStages = 4;
 
 __device__ __forceinline__ void ma_cp_async4(float *dst_smem, const float *src, bool valid) {

@@ -158,12 +158,11 @@ __global__ void __launch_bounds__(kPaThreads) pfb_kernel(const PaParams P) {
     const long long o_end = sb1 == P.nsub ? P.nout : pfb_sub_start(P, sb1).o_start;
     const long long s_lo = max(first.s_beg, 0ll);                // first sample of the CTA (call coordinates)
     const long long s_hi = pfb_sub_start(P, sb1 - 1).s_end;
-    // arm pairs in shared memory with an ODD row stride: the threads of a warp read different arms at the same tap
-    // index, and with a stride of 16 all 32 of them hit two banks (ncu: 176 M bank conflicts, 16 % issue utilisation)
+    // arm rows in shared memory with an ODD row stride: the threads of a warp read different arms at the same tap
+    // index, and with a stride of 16 all 32 of them would hit two banks.
     // In shared memory the table is PLANAR (one float row per arm, arm b+1 is the second row a thread reads) with an odd
     // row stride: a 4-byte access has 32 banks for the 32 lanes, so any set of arms is conflict-free at a given tap index
-    // -- the 8-byte pair rows had 16 bank pairs for 32 arms and every load took two passes (ncu, profiles/r2_pfbarb.txt:
-    // 6.46 M wavefronts where 3.24 M are ideal, the LSU pipe 84 % busy).
+    // -- 8-byte pair rows would have 16 bank pairs for 32 arms and take two passes per load.
     const int TS = P.arms_in_smem ? (T | 1) : T;
     float *s_tap = reinterpret_cast<float *>(s_arms);
     if (P.arms_in_smem)

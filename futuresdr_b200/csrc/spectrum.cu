@@ -19,7 +19,7 @@
 // so parity with the oracle is a tolerance (1e-5 of the largest average, tests/test_gpu_spectrum.py), not bit
 // equality -- the unfused bit-exact blocks (fft.cu, apply.cu, mavg.cu) remain.  Why not one exact pass: a bin's chain
 // is 2 dependent f32 operations per frame (~8 cycles), i.e. at most ~240 M frames/s per bin however many SMs there
-// are -- for N = 2048 that alone caps a bit-exact pipe at ~59 % of this roofline.
+// are.
 #include <cmath>
 
 #include "common.cuh"
@@ -62,7 +62,7 @@ __device__ __forceinline__ void sp_cp_async16(void *dst_smem, const void *src) {
 // The next frame of a group is fetched with cp.async into a raw staging row while the current one is being
 // transformed: the first FFT pass reads the staging row, and from the barrier that ends it the row is free again, so
 // the fetch of frame c+1 overlaps passes 2.. and the averaging of frame c.  (The first version read the frame with
-// plain loads at the top of every round: 2 CTAs per SM x serialized load / compute phases = 40 % of HBM.)
+// plain loads at the top of every round, which serialized the load and compute phases.)
 template <int LOG2N>
 __global__ void __launch_bounds__(kSpThreads, (LOG2N <= 12 ? 3 : 1)) spectrum_kernel(const SpArgs p) {
     constexpr int N = 1 << LOG2N;

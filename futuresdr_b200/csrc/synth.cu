@@ -140,9 +140,9 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
     float2 *Sb = Vf + (size_t)OB * NP;                       // [TPAD-1+OB][N]  spun vectors, oldest row first
     const int tid = threadIdx.x;
     const int w = tid % N, run = tid / N;
-    unsigned long long tap[TPAD];            // (t, t) pairs: one FFMA2 per complex x real MAC (common.cuh cmac2)
+    float tap[TPAD];
 #pragma unroll
-    for (int j = 0; j < TPAD; j++) tap[j] = dup2(__ldg(arms_pad + (size_t)j * N + w));
+    for (int j = 0; j < TPAD; j++) tap[j] = __ldg(arms_pad + (size_t)j * N + w);
 
     const int t0 = blockIdx.x * tiles_per_cta, t1 = min(t0 + tiles_per_cta, ntiles);
     for (int t = t0 - WARM; t < t1; t++) {                   // t < t0: warm-up tiles (fill the ring, emit nothing)
@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
 #pragma unroll
                 for (int u = 0; u < RL; u++) {
                     const int j = u + TPAD - 1 - k;          // output u sees this row as its j-th newest spun sample
-                    if (j >= 0 && j < TPAD) cmac2(acc[u], x, tap[j]);
+                    if (j >= 0 && j < TPAD) mac(acc[u], x, tap[j]);
                 }
             }
 #pragma unroll

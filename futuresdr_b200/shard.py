@@ -94,7 +94,7 @@ class ShardedFir:
             self._filter = DecimatingFirFilter(self.decim, self.taps, sample_dtype, ctx=ctx, algo=algo)
             compute = self._filter.filter
             # the split/D outputs behind the exchange are a few hundred items: the CUDA-core kernel has no
-            # TMEM / tap-table prologue, so that second launch costs ~half of a tensor-kernel launch
+            # tap-table prologue, so that second launch costs ~half of a tensor-kernel launch
             self._head_filter = DecimatingFirFilter(self.decim, self.taps, sample_dtype, ctx=ctx, algo=_lib.ALGO_DIRECT)
             head_compute = self._head_filter.filter
         else:

@@ -1,5 +1,5 @@
 /*
- * b200sdr.h -- C ABI of the B200-native streaming-DSP backend for FutureSDR's
+ * b200sdr.h -- C ABI of the H100-native streaming-DSP backend for FutureSDR's
  * FIR / decimator / resampler / FFT / Apply / PfbArbResampler hot path.
  *
  * The reference (FutureSDR, Rust) has no FFI for this path: its boundary is a set of Rust
@@ -60,15 +60,15 @@ typedef enum {
 typedef enum {
     B2S_ALGO_AUTO   = 0,
     B2S_ALGO_DIRECT = 1, /* CUDA-core register-blocked direct form (any kind, any decimation) */
-    B2S_ALGO_TENSOR = 2, /* tcgen05 block-Toeplitz GEMM, split-bf16 (real taps, 16..257, decim divides 128).
+    B2S_ALGO_TENSOR = 2, /* wgmma block-Toeplitz GEMM, split-bf16 (real taps, 16..257, decim divides 128).
                           * Numerics: operands are split into bf16 hi + lo and three of the four partial products are
                           * summed in FP32: ~2^-18 rms per product, worst case ~3e-5 of ||taps||_1 max|x| when EVERY
                           * product errs the same way (constant taps on constant input -- AUTO keeps constant tap
                           * vectors on DIRECT).  Non-finite input: a NaN/Inf sample at index i makes every output of
                           * the 128-sample blocks whose K-range contains it non-finite (inside [i-K, i+131],
                           * K = 128*ceil((ntaps+127)/128), a superset of the reference's [i-ntaps+1, i]); all other
-                          * outputs are unaffected and no finite output is ever wrong.  f32 DENORMAL samples count as
-                          * zero (tensor-core operands are flush-to-zero).  Streams that may carry
+                          * outputs are unaffected and no finite output is ever wrong.  f32 DENORMAL samples may count as
+                          * zero (tensor-core operands may be flushed to zero).  Streams that may carry
                           * non-finite samples and need the reference's exact propagation: use B2S_ALGO_DIRECT. */
     B2S_ALGO_FFT    = 3  /* overlap-save FFT convolution (c32 samples, 64..2049 taps, decim == 1)  */
 } b2s_algo;

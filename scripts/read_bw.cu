@@ -1,7 +1,7 @@
 // read_bw.cu -- micro-benchmark: achievable HBM READ bandwidth with one persistent CTA per SM for
 //   (A) LDG.128 streaming with U loads in flight per thread, (B) cp.async.bulk (TMA) into a smem ring
 // of NS slots of SLOT bytes.  Used to size the tensor FIR's input path.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o read_bw read_bw.cu && ./read_bw
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o read_bw read_bw.cu && ./read_bw
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -102,19 +102,23 @@ int main() {
     cudaMemset(buf, 1, bytes);
     const size_t n4 = bytes / 16;
     auto rep = [&](const char *name, float ms) { printf("%-44s %8.3f ms  %7.1f GB/s\n", name, ms, bytes / ms / 1e6); };
-    for (int g : {148, 296, 592}) {
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    for (int g : {sms, 2 * sms, 4 * sms}) {
         char nm[96];
         snprintf(nm, 96, "LDG.128 grid-stride U=4 grid=%d", g); rep(nm, time_ms([&] { ldg_kernel<4><<<g, 512>>>((const float4 *)buf, n4, sink); }));
         snprintf(nm, 96, "LDG.128 grid-stride U=8 grid=%d", g); rep(nm, time_ms([&] { ldg_kernel<8><<<g, 512>>>((const float4 *)buf, n4, sink); }));
     }
-    rep("LDG.128 tile-ordered U=8 grid=148", time_ms([&] { ldg_tile_kernel<8><<<148, 512>>>((const float4 *)buf, n4, sink); }));
-    rep("LDG.128 tile-ordered U=8 grid=296", time_ms([&] { ldg_tile_kernel<8><<<296, 512>>>((const float4 *)buf, n4, sink); }));
+    for (int g : {sms, 2 * sms}) {
+        char nm[96];
+        snprintf(nm, 96, "LDG.128 tile-ordered U=8 grid=%d", g); rep(nm, time_ms([&] { ldg_tile_kernel<8><<<g, 512>>>((const float4 *)buf, n4, sink); }));
+    }
 #define BULK(SLOT, NS)                                                                                      \
     {                                                                                                       \
         auto k = bulk_kernel<SLOT, NS>;                                                                     \
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SLOT * NS);                    \
-        char nm[96]; snprintf(nm, 96, "cp.async.bulk slot=%dK x %d (%dK ring) grid=148", SLOT / 1024, NS, SLOT * NS / 1024); \
-        rep(nm, time_ms([&] { k<<<148, 64, SLOT * NS>>>(buf, bytes, sink); }));                             \
+        char nm[96]; snprintf(nm, 96, "cp.async.bulk slot=%dK x %d (%dK ring) grid=%d", SLOT / 1024, NS, SLOT * NS / 1024, sms); \
+        rep(nm, time_ms([&] { k<<<sms, 64, SLOT * NS>>>(buf, bytes, sink); }));                             \
     }
     BULK(4096, 16) BULK(8192, 8) BULK(8192, 16) BULK(8192, 24) BULK(16384, 4) BULK(16384, 8) BULK(16384, 12) BULK(32768, 4) BULK(32768, 6)
     cudaError_t e = cudaDeviceSynchronize();

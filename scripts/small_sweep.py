@@ -1,5 +1,5 @@
 """Tensor vs CUDA-core FIR on SMALL slices (the perf/fir regime: 1 M samples per call): where does the tensor kernel's
-fixed cost (TMEM allocation, Toeplitz fill, 148 persistent CTAs) stop paying?  Prints microseconds per call."""
+fixed cost (Toeplitz fill, one persistent CTA per SM) stop paying?  Prints microseconds per call."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

@@ -1,6 +1,6 @@
 // test_host.cpp -- the reference's known-answer tests replayed through the C++ host layer
 // (include/b200sdr.hpp) on a GPU.  Each CHECK names the reference test it restates.
-// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs a B200).
+// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <random>

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 (tensor-core, split-bf16) FIR against the oracle, through the C ABI.
+"""Parity of the wgmma (tensor-core, split-bf16) FIR against the oracle, through the C ABI.
 Same tolerance as the direct path: |y - y_ref| <= 1e-5 * ||taps||_1 * max|x|."""
 import numpy as np
 import pytest
@@ -54,7 +54,7 @@ def test_tensor_fir_ragged(fb, rng):
 
 
 def test_tensor_fir_many_tiles_multiwave(fb, rng):
-    # > 148 SMs x 4 stages of tiles: exercises the stage / accumulator ring wrap-around
+    # > 132 SMs x 4 stages of tiles: exercises the stage / accumulator ring wrap-around
     _check(fb, rng, 256, 4096 * 1500 + 255 + 17, True)
     _check(fb, rng, 100, 8192 * 700 + 99 + 5, False)
 
@@ -87,7 +87,7 @@ def test_tensor_unsupported_shapes_are_refused(fb):
         fb.FirFilter(np.ones(64, np.complex64), algo=fb.ALGO_TENSOR)
     with pytest.raises(fb.B200SdrError):       # < 16 taps: split-bf16 error bound too loose, refused
         fb.FirFilter(np.ones(5, np.float32), algo=fb.ALGO_TENSOR)
-    with pytest.raises(fb.B200SdrError):       # > 257 taps: Toeplitz operand no longer fits TMEM
+    with pytest.raises(fb.B200SdrError):       # > 257 taps: Toeplitz operand no longer fits K <= 384
         fb.FirFilter(np.ones(300, np.float32), algo=fb.ALGO_TENSOR)
     # AUTO falls back to the CUDA-core kernel for those shapes
     assert fb.FirFilter(np.ones(300, np.float32)).algo == fb.ALGO_FFT          # long filter: overlap-save

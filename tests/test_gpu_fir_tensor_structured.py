@@ -97,7 +97,7 @@ def test_boxcar_on_dc_documented_worst_case():
 
 def test_denormal_samples_are_flushed_to_zero():
     """Contract (include/b200sdr.h): the tensor path treats f32 DENORMAL samples as zero (the bf16 operands of
-    tcgen05.mma are flush-to-zero), where the reference's scalar loop keeps them.  The difference is bounded by
+    the tensor-core MMA may be flushed to zero), where the reference's scalar loop keeps them.  The difference is bounded by
     ||taps||_1 * 1.18e-38 (the largest denormal) -- 280 dB below full scale -- and normal samples are unaffected."""
     rng = np.random.default_rng(7)
     n = 20000
