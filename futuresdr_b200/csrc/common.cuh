@@ -45,11 +45,23 @@ struct PerDeviceOnce {
 };
 
 #ifdef __CUDACC__
+__device__ __forceinline__ void mac(float &acc, float x, float t) { acc = fmaf(x, t, acc); }
 // acc += x * t for a Complex<f32> sample and a REAL tap: two IEEE fused multiply-adds (sm_90 has no packed FFMA2).
 __device__ __forceinline__ void mac(float2 &acc, float2 x, float t) {
     acc.x = fmaf(x.x, t, acc.x);
     acc.y = fmaf(x.y, t, acc.y);
 }
+// Complex tap: re = xr*tr - xi*ti, im = xr*ti + xi*tr (fir.rs:257-276)
+__device__ __forceinline__ void mac(float2 &acc, float2 x, float2 t) {
+    acc.x = fmaf(x.x, t.x, acc.x);
+    acc.x = fmaf(-x.y, t.y, acc.x);
+    acc.y = fmaf(x.x, t.y, acc.y);
+    acc.y = fmaf(x.y, t.x, acc.y);
+}
+
+template <typename S> __device__ __forceinline__ S zero_of();
+template <> __device__ __forceinline__ float zero_of<float>() { return 0.0f; }
+template <> __device__ __forceinline__ float2 zero_of<float2>() { return make_float2(0.f, 0.f); }
 #endif
 
 extern thread_local std::string g_b2s_last_error;

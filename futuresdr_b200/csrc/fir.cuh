@@ -10,9 +10,9 @@ struct b2s_fir {
     b2s_algo algo_req = B2S_ALGO_AUTO, algo = B2S_ALGO_DIRECT;
 
     // ---- direct form (fir_direct.cu): per-phase, time-reversed, zero-padded taps in HBM.
-    // G[q][u] = g[D*u + q - (D-1)], g[t] = taps[N-1-t]   (see DESIGN.md "direct FIR")
+    // G[q][u] = g[D*u + q - (D-1)] (u < Upad), then g[t] = taps[N-1-t]   (see DESIGN.md "direct FIR")
     float *d_ptaps = nullptr;
-    int U = 0, Upad = 0;
+    int Upad = 0;
 
     // ---- tensor-core form (fir_tc.cu): split-bf16 Toeplitz blocks, built lazily
     void *d_toeplitz = nullptr;
@@ -32,10 +32,9 @@ struct b2s_fir {
 int32_t fir_direct_prepare(b2s_fir *f);
 int32_t fir_direct_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out,
                           cudaStream_t stream);
-// fir_direct.cu: rational resampler on the sliding-window machinery (called from resamp.cu)
-int     resamp_slide_upad(size_t M, size_t T);
+// fir_direct.cu: rational resampler on the same kernel (called from resamp.cu)
+std::vector<float> slide_table(const float *taps, size_t tf, size_t L, size_t M, size_t T, size_t lead);
 bool    resamp_slide_supported(size_t L, size_t M, size_t T, size_t item_bytes);
-void    resamp_slide_table(const float *taps, size_t L, size_t M, size_t T, std::vector<float> &g);
 int32_t resamp_slide_launch(b2s_ctx *ctx, b2s_kind kind, const float *d_gtab, size_t L, size_t M, size_t T,
                             const void *d_in, size_t n_in, void *d_out, size_t n_out, cudaStream_t stream);
 // detached history of b2s_fir_exec_hist: n_hist items that logically precede the slice, plus the optional

@@ -3,7 +3,9 @@
 //
 //   o[k] = sum_{t<T} i[floor(k*M/L) + t] * taps[L*(T-1-t) + (k*M mod L)],   T = ntaps / L
 //
-// The host rearranges the taps once into bank-major, time-reversed rows  G[b][t] =
+// Plans whose per-phase tap tables stay small (small L*M, resamp_slide_supported) run on the sliding-window kernel
+// of the direct FIR (fir_direct.cu), the resampler being L decimate-by-M FIRs over one staged tile.  All others run
+// resamp_kernel below: the host rearranges the taps once into bank-major, time-reversed rows  G[b][t] =
 // taps[L*(T-1-t) + b]  (row pitch odd so lanes on different banks hit different smem banks).
 // A CTA produces TK consecutive outputs: it stages the contiguous input span those outputs
 // touch plus the bank table in shared memory, then each thread walks its outputs' T taps.
@@ -23,12 +25,6 @@ namespace {
 
 constexpr int kRsThreads = 256;
 constexpr int kRsR = 4;          // outputs per thread that share one polyphase bank (tap reuse)
-
-template <typename S> __device__ __forceinline__ S rs_zero();
-template <> __device__ __forceinline__ float rs_zero<float>() { return 0.f; }
-template <> __device__ __forceinline__ float2 rs_zero<float2>() { return make_float2(0.f, 0.f); }
-__device__ __forceinline__ void rs_mac(float &a, float x, float t) { a = fmaf(x, t, a); }
-__device__ __forceinline__ void rs_mac(float2 &a, float2 x, float t) { a.x = fmaf(x.x, t, a.x); a.y = fmaf(x.y, t, a.y); }
 
 // A CTA produces R*S consecutive outputs, S = L*G >= 256 a multiple of L.  Thread slot tt < S owns
 // the R outputs  k = kb + tt + r*S:  they share the bank (k*M mod L) and their input windows are
@@ -60,21 +56,21 @@ resamp_kernel(const S *__restrict__ in, S *__restrict__ out, const float *__rest
         const float *gb = g + bank * pitch;
         S acc[kRsR];
 #pragma unroll
-        for (int r = 0; r < kRsR; r++) acc[r] = rs_zero<S>();
+        for (int r = 0; r < kRsR; r++) acc[r] = zero_of<S>();
         int nr = kRsR;                                          // outputs of this thread inside n_out
         while (nr > 1 && k0 + (long long)(nr - 1) * Sg > klast) nr--;
         if (nr == kRsR) {
             for (int t = 0; t < T; t++) {
                 const float tap = gb[t];
 #pragma unroll
-                for (int r = 0; r < kRsR; r++) rs_mac(acc[r], xs[i0 + r * step + t], tap);
+                for (int r = 0; r < kRsR; r++) mac(acc[r], xs[i0 + r * step + t], tap);
             }
         } else {
             for (int t = 0; t < T; t++) {
                 const float tap = gb[t];
 #pragma unroll
                 for (int r = 0; r < kRsR; r++)
-                    if (r < nr) rs_mac(acc[r], xs[i0 + r * step + t], tap);
+                    if (r < nr) mac(acc[r], xs[i0 + r * step + t], tap);
             }
         }
 #pragma unroll
@@ -108,8 +104,8 @@ int32_t b2s_resamp_plan(b2s_ctx *ctx, b2s_kind kind, const float *taps, size_t n
     if (e != cudaSuccess) { delete r; return b2s_fail(ctx, B2S_ENOMEM, "resampler taps"); }
     B2S_CUDA(ctx, cudaMemcpyAsync(r->d_banks, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     std::vector<float> gt;
-    if (resamp_slide_supported(interp, decim, r->T, kind_in_bytes(kind)) && !getenv("B2S_RESAMP_NO_SLIDE")) {
-        resamp_slide_table(taps, interp, decim, r->T, gt);
+    if (resamp_slide_supported(interp, decim, r->T, kind_in_bytes(kind))) {
+        gt = slide_table(taps, 1, interp, decim, r->T, 0);
         e = cudaMalloc((void **)&r->d_gtab, gt.size() * sizeof(float));
         if (e != cudaSuccess) { cudaFree(r->d_banks); delete r; return b2s_fail(ctx, B2S_ENOMEM, "resampler phase taps"); }
         B2S_CUDA(ctx, cudaMemcpyAsync(r->d_gtab, gt.data(), gt.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));

@@ -4,14 +4,7 @@
 set -e
 cd "$(dirname "$0")/../futuresdr_b200/csrc"
 NAME=$1; EXTRA=$2
-mkdir -p ../variants build_$NAME
-FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -ffp-contract=off -ccbin /usr/bin/g++ -I../../include -I. --expt-relaxed-constexpr $EXTRA"
-OBJS=""
-for f in abi fir_direct fir_tc fir_fft firdes fft apply resamp pfbarb rotator chan synth mavg ring peer; do
-  /usr/local/cuda/bin/nvcc $FLAGS -c $f.cu -o build_$NAME/$f.o &
-  OBJS="$OBJS build_$NAME/$f.o"
-done
-wait
-/usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../variants/libb200sdr_$NAME.so $OBJS -lcudart_static -ldl -lrt -lpthread
+mkdir -p ../variants
+make -j8 OUT=../variants/libb200sdr_$NAME.so BUILD=build_$NAME EXTRA="$EXTRA"
 rm -rf build_$NAME
 echo built ../variants/libb200sdr_$NAME.so
