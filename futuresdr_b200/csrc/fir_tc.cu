@@ -23,16 +23,20 @@
 //    is a whole 8-row swizzle atom: physical atom gamma holds blocks {gamma + 16*jb}; the view
 //    for shift d starts at atom d (descriptor base + 1024*d bytes).  Atoms 16, 17 duplicate the
 //    rows they alias (12 % extra conversion work, no extra HBM traffic).
-//  * 17 warps, one persistent CTA per SM, everything handed over with mbarriers:
-//      warp 16    TMA loader : cp.async.bulk of the raw f32 samples into a 6 x 8 KiB ring
+//  * 5 warpgroups, one persistent CTA per SM, everything handed over with mbarriers; setmaxnreg moves registers
+//    from the converters and the loader to the math warpgroups:
+//      warp 16    TMA loader : cp.async.bulk of the raw f32 samples into a 6 x 8 KiB ring (warps 17-19 only
+//                              complete the loader warpgroup and exit)
 //      warps 8-15 converters : LDS.128 -> bf16 hi/lo split (cvt.rn.bf16x2) -> swizzled st.shared
 //                              into one of two 72 KiB operand stages
-//      warps 0-7  two math warpgroups, 64 output phases (M rows) each: 72 wgmma.m64n128k16 per tile
-//                 (DK x 8 K-steps x 3 products) into 64 FP32 accumulator registers per thread, then the
-//                 stores of those outputs straight from the registers.
+//      warps 0-7  two math warpgroups, 64 output phases (M rows) each: 3 wgmma.m64n128k16 per K-step, only over
+//                 the K-steps whose Toeplitz slice holds a tap for the warpgroup's phases (20 of 24 at 256 taps),
+//                 into one of two sets of 64 FP32 accumulator registers per thread; while tile t's MMAs run, the
+//                 outputs of tile t-1 are stored from the other set straight from the registers.
 #include <cuda_bf16.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstdlib>
 #include <type_traits>
 
@@ -48,11 +52,22 @@ constexpr int kRawSlots = B2S_RAW_SLOTS;    // raw f32 staging ring, 8 KiB per s
 constexpr int kRawSlotBytes = 8192;
 constexpr int kNumProducerThreads = 256;    // 8 converter warps
 constexpr int kNumMathThreads = 256;        // 2 warpgroups: wgmma + epilogue
-constexpr int kThreadsTC = kNumMathThreads + kNumProducerThreads + 32;   // + TMA warp = 544
+constexpr int kNumLoaderThreads = 128;      // loader warpgroup: one TMA warp, three that exit (setmaxnreg is per warpgroup)
+constexpr int kThreadsTC = kNumMathThreads + kNumProducerThreads + kNumLoaderThreads;   // 640
 constexpr int kProdWarps = kNumProducerThreads / 32;
 constexpr int kMathWarps = kNumMathThreads / 32;
 constexpr int kProdWarp0 = kMathWarps;               // warps 8..15 converters
 constexpr int kTmaWarp = kProdWarp0 + kProdWarps;    // warp 16
+// Registers per thread: __launch_bounds__(640, 1) gives every thread 96 (65536 / 640, in units of 8).  The math
+// warpgroups hold two 64-register accumulator sets plus descriptors and epilogue addresses (the f32 epilogue spills
+// at 168), so they take what the converters (48 suffice) and the loader give back; the CTA's allocation must cover
+// the sum or setmaxnreg.inc never returns.  kRegsAtLaunch assumes ptxas gives the kernel exactly that count at entry
+// (-Xptxas -v: "Used 96 registers"); a lower entry count would shrink the pool below the budget, so fir_tc_prepare
+// refuses the plan if the built kernel reports any other count.
+constexpr int kRegsAtLaunch = 65536 / kThreadsTC / 8 * 8;
+constexpr int kMathRegs = 176, kProdRegs = 48, kLoaderRegs = 24;
+static_assert(kNumMathThreads * kMathRegs + kNumProducerThreads * kProdRegs + kNumLoaderThreads * kLoaderRegs <=
+              kThreadsTC * kRegsAtLaunch, "setmaxnreg budget exceeds the CTA's register allocation");
 constexpr int kAtomsOut = 16;                // N = 128 columns = 16 swizzle atoms of 8 rows
 constexpr int kMaxDK = 3;                    // K <= 384
 constexpr int kSplitBytesMax = (kAtomsOut + kMaxDK - 1) * 1024 * 2;   // per split: 2 K-chunks x 18 atoms
@@ -96,6 +111,20 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Predicated global stores, branch-free in PTX: the epilogue runs while wgmma.mma_async writes the other accumulator
+// set, and ptxas serialises every wgmma of a kernel when registers are read on a path it must assume divergent
+// between an mma_async and its wait_group.
+__device__ __forceinline__ void st_global_if(float2 *p, float a, float b, bool pred) {
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q st.global.v2.f32 [%0], {%1, %2};\n\t}"
+                 ::"l"(p), "f"(a), "f"(b), "r"((int)pred) : "memory");
+}
+__device__ __forceinline__ void st_global_if(float *p, float a, bool pred) {
+    asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q st.global.f32 [%0], %1;\n\t}"
+                 ::"l"(p), "f"(a), "r"((int)pred) : "memory");
+}
+// per-thread register limit of the executing warpgroup (every warp of the warpgroup must execute the same one)
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 // d[64] (+)= A[smem desc] * B[smem desc]   (m64n128k16, bf16 inputs, fp32 accumulate, both operands K-major)
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
     asm volatile(
@@ -238,11 +267,13 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
     constexpr int ITEM_BYTES = COMPLEX ? 8 : 4;
     const int in_blocks = TILE_BLOCKS + DK - 1;
 
-    if (warp == kTmaWarp) {
+    if (warp >= kTmaWarp) {
         // ================================ TMA LOADER ===========================================
         // One thread streams the input with bulk async copies (cp.async.bulk): the copies complete on the
         // slot's mbarrier (complete_tx), so HBM latency is absorbed by the 48 KiB ring and never by a
         // converter warp's registers.
+        setmaxnreg_dec<kLoaderRegs>();
+        if (warp != kTmaWarp) return;
         if (elect_one()) {
             int rs = 0;
             uint32_t rphase = 0;
@@ -303,6 +334,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         // loops are fully unrolled, so every shared-memory address is
         //     stage base + per-thread constant + compile-time constant + one of 8 precomputed swizzle offsets.
         // Per float4: one LDS.128, two XU conversions per value pair, 4 (8 for aliased rows) 32-bit stores.
+        setmaxnreg_dec<kProdRegs>();
         const int tid = threadIdx.x - 32 * kProdWarp0;                   // 0..255
         const int fo = tid % F4_PER_BLOCK, rowsel = tid / F4_PER_BLOCK;  // rowsel 0..3 (complex) / 0..7 (real)
         const int kc = COMPLEX ? (fo >> 5) : (fo >> 4);
@@ -419,72 +451,101 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         // Warpgroup wg computes the accumulator rows p' = 64*wg .. 64*wg+63 (output phases p = 127 - p') of
         // all 128 columns.  Thread (warp w, lane) holds rows 16*(w%4) + lane/4 + {0, 8} of its warpgroup and
         // columns 8*gamma + 2*(lane%4) + {0, 1}: acc[4*gamma + 2*h + e].
-        const int wg = warp >> 2, wl = warp & 3, q4 = lane & 3;
+        setmaxnreg_inc<kMathRegs>();
+        // warp-uniform by construction (a broadcast): the K-step loop below branches on it, and wgmma.mma_async in a
+        // loop the compiler must assume divergent is serialised
+        const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
+        const int wl = warp & 3, q4 = lane & 3;
         // Decimation (decimating_fir.rs:80-92: o[k] = y[D-1 + k*D] of the full-rate FIR y): the MMAs still
         // produce every phase -- the kernel is HBM-bound below ~130 taps -- and the epilogue keeps the phases
         // p == D-1 (mod D).  D divides 128, so the kept phases are the same in every block and block b
         // contributes the 128/D outputs  k = b*(128/D) + (p-(D-1))/D.
         const int D = prm.decim, per_blk = 128 / D;
         const uint32_t a_hi = a_base + 1024u * wg, a_lo = a_hi + kABytes;   // row group a = 8*wg + a_local
-        float acc[64];
-#pragma unroll
-        for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+        // The warpgroup's phases p in [p0, p0 + 63] meet taps only in the Toeplitz columns
+        // kappa in [p0 + lead, p0 + 63 + lead + ntaps - 1]: K-steps j (kappa = 16j .. 16j+15) outside [j0, j1] would
+        // add only zero products and are not issued.  flags bit2 (tuning switch): no MMAs at all.
+        const int p0 = 64 * (1 - wg);
+        const int j0 = (p0 + prm.lead) / 16;
+        const int j1 = (prm.flags & 4) ? j0 - 1 : min((p0 + 63 + prm.lead + prm.ntaps - 1) / 16, 8 * DK - 1);
+
         int stage = 0;
         uint32_t phase = 0;
-        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+        // wait for the stage, issue its MMAs into acc and commit them (they run while the caller stores)
+        auto mma_tile = [&](float (&acc)[64]) {
             mbar_wait(full_bar(stage), phase);
-            wgmma_fence();                           // the previous tile's register reads precede the async writes
+            wgmma_fence();                           // earlier register reads of acc precede the async writes
             const uint32_t sbase = base + stage * kStageBytes;
-            uint32_t accum = 0;
-            for (int d = 0; d < ((prm.flags & 4) ? 0 : DK); d++) {   // flags bit2: tuning switch, skip the MMAs
-#pragma unroll
-                for (int kc = 0; kc < 2; kc++) {
-#pragma unroll
-                    for (int ks = 0; ks < 4; ks++) {
-                        // Toeplitz columns kappa >= ntaps + 127 hold no tap: skip those K-steps
-                        const int kappa0 = d * 128 + kc * 64 + ks * 16;
-                        if (kappa0 >= prm.ntaps + prm.lead + 127) continue;
-                        const uint32_t aoff = (uint32_t)(kappa0 / 8) * 128u;                // core matrix a + j
-                        const uint32_t boff = (uint32_t)(kc * chunk_bytes + d * 1024 + ks * 32);
-                        const uint64_t bh = make_b_desc(sbase + boff);
-                        const uint64_t bl = make_b_desc(sbase + split_bytes + boff);
-                        const uint64_t ah = make_a_desc(a_hi + aoff);
-                        wgmma_m64n128(acc, ah, bh, accum);                           // g_hi * x_hi
-                        wgmma_m64n128(acc, ah, bl, 1u);                              // g_hi * x_lo
-                        wgmma_m64n128(acc, make_a_desc(a_lo + aoff), bh, 1u);        // g_lo * x_hi
-                        accum = 1u;
-                    }
-                }
+#pragma unroll 1
+            for (int j = j0; j <= j1; j++) {
+                const int d = j >> 3, kc = (j >> 2) & 1, ks = j & 3;
+                const int kappa0 = d * 128 + kc * 64 + ks * 16;
+                const uint32_t aoff = (uint32_t)(kappa0 / 8) * 128u;                // core matrix a + j
+                const uint32_t boff = (uint32_t)(kc * chunk_bytes + d * 1024 + ks * 32);
+                const uint64_t bh = make_b_desc(sbase + boff);
+                const uint64_t bl = make_b_desc(sbase + split_bytes + boff);
+                const uint64_t ah = make_a_desc(a_hi + aoff);
+                wgmma_m64n128(acc, ah, bh, j != j0);                         // g_hi * x_hi
+                wgmma_m64n128(acc, ah, bl, 1u);                              // g_hi * x_lo
+                wgmma_m64n128(acc, make_a_desc(a_lo + aoff), bh, 1u);        // g_lo * x_hi
             }
             wgmma_commit();
+        };
+        // wait for the MMAs, then hand the operand stage back to the converters (they may refill it)
+        auto release_stage = [&]() {
             wgmma_wait_all();
             __syncwarp();
-            if (lane == 0) mbar_arrive(empty_bar(stage));   // operand stage read: the converters may refill it
+            if (lane == 0) mbar_arrive(empty_bar(stage));
             if (++stage == kStages) { stage = 0; phase ^= 1; }
-            if (prm.flags & 2) continue;                    // tuning switch: skip the global stores
-
-            // ---- epilogue: for each (h, gamma) a warp writes 4 runs of 8 consecutive outputs (one per lane%4)
-            const long long blk0 = (long long)tile * TILE_BLOCKS;
-            const bool interior = (blk0 + TILE_BLOCKS) * per_blk <= prm.n_out;
+        };
+        // ---- epilogue: for each (h, gamma) a warp writes 4 runs of 8 consecutive outputs (one per lane%4).  The
+        // output of column gamma is kb + gamma * per_blk (+ 16 * per_blk for the second real value); it is written when
+        // its phase is kept and k < n_out, i.e. gamma * per_blk < room.  D is a power of two (D | 128).
+        const int log2D = __ffs(D) - 1;
+        auto store_tile = [&](const float (&acc)[64], int tile) {
+            if (prm.flags & 2) return;                      // tuning switch: skip the global stores
 #pragma unroll
             for (int h = 0; h < 2; h++) {
                 const int p = 127 - (64 * wg + 16 * wl + (lane >> 2) + 8 * h);
-                if ((p % D) != D - 1) continue;
-                const int pk = (p - (D - 1)) / D;
+                const int keep = (p & (D - 1)) == D - 1;
+                const long long kb = ((long long)tile * TILE_BLOCKS + kAtomsOut * q4 * (COMPLEX ? 1 : 2)) * per_blk +
+                                     (p >> log2D);
+                const int room = (int)max(min(prm.n_out - kb, (long long)INT_MAX), 0ll) & -keep;
 #pragma unroll
                 for (int gam = 0; gam < 16; gam++) {
                     const float v0 = acc[4 * gam + 2 * h], v1 = acc[4 * gam + 2 * h + 1];
+                    const int kg = gam * per_blk;
                     if constexpr (COMPLEX) {
-                        const long long k = (blk0 + gam + kAtomsOut * q4) * per_blk + pk;
-                        if (interior || k < prm.n_out) reinterpret_cast<float2 *>(prm.out)[k] = make_float2(v0, v1);
+                        st_global_if(reinterpret_cast<float2 *>(prm.out) + kb + kg, v0, v1, kg < room);
                     } else {
-                        const long long k0 = (blk0 + gam + kAtomsOut * (2 * q4)) * per_blk + pk;
-                        const long long k1 = k0 + (long long)kAtomsOut * per_blk;
-                        if (interior || k0 < prm.n_out) prm.out[k0] = v0;
-                        if (interior || k1 < prm.n_out) prm.out[k1] = v1;
+                        const int kg1 = kg + kAtomsOut * per_blk;
+                        st_global_if(prm.out + (kb + kg), v0, kg < room);
+                        st_global_if(prm.out + (kb + kg1), v1, kg1 < room);
                     }
                 }
             }
+        };
+
+        // Two accumulator sets: tile t's MMAs go to one while tile t-1 is stored from the other.  Unrolled by two so
+        // that every register index is static; at the top of the loop the MMAs of `tile` have completed into acc0.
+        float acc0[64], acc1[64];
+#pragma unroll
+        for (int i = 0; i < 64; i++) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+        int tile = blockIdx.x;
+        if (tile < prm.num_tiles) {
+            mma_tile(acc0);
+            release_stage();
+        }
+        for (; tile < prm.num_tiles; tile += 2 * gridDim.x) {
+            const int next = tile + gridDim.x;
+            if (next >= prm.num_tiles) { store_tile(acc0, tile); break; }
+            mma_tile(acc1);
+            store_tile(acc0, tile);
+            release_stage();
+            if (next + (int)gridDim.x >= prm.num_tiles) { store_tile(acc1, next); break; }
+            mma_tile(acc0);
+            store_tile(acc1, next);
+            release_stage();
         }
     }
 }
@@ -507,6 +568,14 @@ int32_t fir_tc_prepare(b2s_fir *f) {
     f->tc_kblocks = (int)ceil_div(f->ntaps + 127, 128);
     B2S_CUDA(ctx, cudaFuncSetAttribute(fir_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTC));
     B2S_CUDA(ctx, cudaFuncSetAttribute(fir_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTC));
+    // the setmaxnreg budget holds only for the entry register count it was sized for; any other would hang the kernel
+    for (const void *k : {(const void *)fir_tc_kernel<true>, (const void *)fir_tc_kernel<false>}) {
+        cudaFuncAttributes attr;
+        B2S_CUDA(ctx, cudaFuncGetAttributes(&attr, k));
+        if (attr.numRegs != kRegsAtLaunch)
+            return b2s_fail(ctx, B2S_EUNSUPPORTED, "tensor FIR: kernel built with %d registers per thread, its setmaxnreg "
+                            "budget assumes %d", attr.numRegs, kRegsAtLaunch);
+    }
     if (const char *e = getenv("B2S_TC_FLAGS")) f->tc_flags = atoi(e);
     f->tc_ready = true;
     return B2S_OK;

@@ -64,8 +64,8 @@ typedef enum {
                           * Numerics: operands are split into bf16 hi + lo and three of the four partial products are
                           * summed in FP32: ~2^-18 rms per product, worst case ~3e-5 of ||taps||_1 max|x| when EVERY
                           * product errs the same way (constant taps on constant input -- AUTO keeps constant tap
-                          * vectors on DIRECT).  Non-finite input: a NaN/Inf sample at index i makes every output of
-                          * the 128-sample blocks whose K-range contains it non-finite (inside [i-K, i+131],
+                          * vectors on DIRECT).  Non-finite input: a NaN/Inf sample at index i makes outputs of the
+                          * 128-sample blocks whose issued K-range contains it non-finite (all inside [i-K, i+131],
                           * K = 128*ceil((ntaps+127)/128), a superset of the reference's [i-ntaps+1, i]); all other
                           * outputs are unaffected and no finite output is ever wrong.  f32 DENORMAL samples may count as
                           * zero (tensor-core operands may be flushed to zero).  Streams that may carry
