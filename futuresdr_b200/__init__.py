@@ -10,11 +10,11 @@ Importing this package loads libb200sdr.so and raises if it is missing: no CPU f
 from ._lib import (  # noqa: F401
     B200SdrError,
     INSUFFICIENT_INPUT, INSUFFICIENT_OUTPUT, BOTH_SUFFICIENT,
-    ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT,
+    ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN,
 )
 from .context import Context, default_context  # noqa: F401
 from .filters import (  # noqa: F401
-    ComputationStatus, FirFilter, DecimatingFirFilter, PolyphaseResamplingFir,
+    ComputationStatus, FirFilter, DecimatingFirFilter, PolyphaseResamplingFir, IirFilter,
 )
 from . import firdes  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain): futuresdr_b200.edges

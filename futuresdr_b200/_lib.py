@@ -16,7 +16,7 @@ SO_PATH = os.environ.get("B2S_LIB") or os.path.join(_HERE, "libb200sdr.so")
 OK, EINVAL, ECUDA, ENOMEM, EAGAIN, EUNSUPPORTED, ESTATE, ETIMEOUT = 0, -1, -2, -3, -4, -5, -6, -7
 INSUFFICIENT_INPUT, INSUFFICIENT_OUTPUT, BOTH_SUFFICIENT = 0, 1, 2
 F32_F32, C32_F32, C32_C32, F64_F64 = 0, 1, 2, 3
-ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT = 0, 1, 2, 3
+ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
  OP_MAG_C32, OP_LOG10_F32) = range(8)
 
@@ -84,6 +84,13 @@ SIGNATURES = {
     "b2s_mavg_create": (_i32, [_vp, _sz, _f32, _sz, _vpp]),
     "b2s_mavg_destroy": (None, [_vp]),
     "b2s_mavg_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp]),
+    "b2s_iir_plan_f32": (_i32, [_vp, _f32p, _sz, _f32p, _sz, _vpp]),
+    "b2s_iir_plan_f64": (_i32, [_vp, C.POINTER(C.c_double), _sz, C.POINTER(C.c_double), _sz, _vpp]),
+    "b2s_iir_destroy": (None, [_vp]),
+    "b2s_iir_length": (_sz, [_vp]),
+    "b2s_iir_set_algo": (_i32, [_vp, C.c_int]),
+    "b2s_iir_get_algo": (_i32, [_vp]),
+    "b2s_iir_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp, _i32p]),
     "b2s_spectrum_plan": (_i32, [_vp, _sz, _i32, _f32, _sz, _f32, _vpp]),
     "b2s_spectrum_destroy": (None, [_vp]),
     "b2s_spectrum_reset": (_i32, [_vp]),

@@ -2,6 +2,7 @@
 
 Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``Fir`` / ``FirBuilder``      src/blocks/fir.rs:13-95, :126-233
+  * ``Iir`` / ``IirBuilder``      src/blocks/iir.rs:8-176
   * ``Fft`` / ``FftDirection``    src/blocks/fft.rs:30-221
   * ``Apply``                     src/blocks/apply.rs:100-131 (closed catalogue of closures)
   * ``PfbArbResampler``           src/blocks/pfb/arb_resampler.rs:72-231
@@ -25,7 +26,7 @@ import torch
 from . import _lib, firdes
 from ._lib import lib, check
 from .context import Context, default_context
-from .filters import (ComputationStatus, DecimatingFirFilter, FirFilter, PolyphaseResamplingFir,
+from .filters import (ComputationStatus, DecimatingFirFilter, FirFilter, IirFilter, PolyphaseResamplingFir,
                       _FilterBase)
 
 
@@ -37,7 +38,8 @@ class WorkIo:
 
 
 def _tdtype(np_dtype):
-    return torch.complex64 if np.dtype(np_dtype) == np.complex64 else torch.float32
+    return {np.dtype(np.complex64): torch.complex64, np.dtype(np.float64): torch.float64}.get(np.dtype(np_dtype),
+                                                                                             torch.float32)
 
 
 def _ctx_device(ctx) -> torch.device:
@@ -169,6 +171,44 @@ class FirBuilder:
     @staticmethod
     def resampling_with_taps(interp: int, decim: int, taps, sample_dtype=np.complex64, ctx=None) -> Fir:
         return Fir(PolyphaseResamplingFir(interp, decim, taps, sample_dtype, ctx))
+
+
+class Iir(Block):
+    """blocks::Iir (src/blocks/iir.rs:8-176): generic over a ``StatefulFilter`` core (an ``IirFilter``)."""
+
+    def __init__(self, core: IirFilter):
+        self.filter = core
+        self.in_dtype = self.out_dtype = core.sample_dtype
+        self._ports()
+        self.input.set_min_items(core.length())              # iir.rs:133
+
+    @classmethod
+    def new(cls, a_taps, b_taps, sample_dtype=np.float32, ctx: Optional[Context] = None) -> "Iir":
+        return cls(IirFilter(a_taps, b_taps, sample_dtype, ctx))
+
+    @classmethod
+    def with_core(cls, core: IirFilter) -> "Iir":
+        return cls(core)
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()        # iir.rs:162-163
+        consumed, produced, status = self.filter.filter(i, o)
+        self.input.consume(consumed)
+        self.output.produce(produced)
+        if self.input.finished() and status != ComputationStatus.InsufficientOutput:   # iir.rs:170-172
+            io.finished = True
+
+
+class IirBuilder:
+    """blocks::IirBuilder (src/blocks/iir.rs:32-64)."""
+
+    @staticmethod
+    def iir(a_taps, b_taps, sample_dtype=np.float32, ctx: Optional[Context] = None) -> Iir:
+        return Iir(IirFilter(a_taps, b_taps, sample_dtype, ctx))
+
+    @staticmethod
+    def same_type(a_taps, b_taps, sample_dtype=np.float32, ctx: Optional[Context] = None) -> Iir:
+        return IirBuilder.iir(a_taps, b_taps, sample_dtype, ctx)
 
 
 class FftDirection(enum.Enum):

@@ -89,7 +89,9 @@ int32_t b2s_ctx_sync(b2s_ctx *ctx) {
         ctx->flag_ops = 0;
         if (st) {
             cudaMemset(ctx->d_status, 0, sizeof(st));
-            return b2s_fail(ctx, B2S_ETIMEOUT, "a cross-GPU flag wait timed out (status 0x%x): the peer never published its chunk", st);
+            if (st & 1u)
+                return b2s_fail(ctx, B2S_ETIMEOUT, "a cross-GPU flag wait timed out (status 0x%x): the peer never published its chunk", st);
+            return b2s_fail(ctx, B2S_ETIMEOUT, "an IIR scan look-back wait timed out (status 0x%x)", st);
         }
     }
     return B2S_OK;
@@ -238,6 +240,8 @@ size_t b2s_fir_length(const b2s_fir *f) { return f ? f->ntaps : 0; }
 
 int32_t b2s_fir_set_algo(b2s_fir *f, b2s_algo algo) {
     if (!f) return b2s_fail(nullptr, B2S_EINVAL, "fir is NULL");
+    if (algo < B2S_ALGO_AUTO || algo > B2S_ALGO_FFT)      // B2S_ALGO_SCAN is an IIR algorithm
+        return b2s_fail(f->ctx, B2S_EUNSUPPORTED, "FIR filters have the AUTO, DIRECT, TENSOR and FFT algorithms (got %d)", (int)algo);
     if (f->kind == B2S_F64_F64)
         return algo == B2S_ALGO_AUTO || algo == B2S_ALGO_DIRECT ? B2S_OK
                : b2s_fail(f->ctx, B2S_EUNSUPPORTED, "f64 filters only have the CUDA-core form");

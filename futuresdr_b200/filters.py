@@ -155,6 +155,43 @@ class FirFilter(DecimatingFirFilter):
         super().__init__(1, taps, sample_dtype, ctx, algo)
 
 
+class IirFilter(_FilterBase):
+    """futuredsp::IirFilter (crates/futuredsp/src/iir.rs:33-178), a ``StatefulFilter``: ``memory`` (the last n_a
+    outputs, first filled with the stream's first n_a input samples) and the fill count live in the plan, so
+    consecutive ``filter`` calls continue one stream.  f32 and f64 samples (the only impls, :56-76); device slices
+    only.  ``algo``: ALGO_AUTO, ALGO_DIRECT (bit-exact sequential kernel) or ALGO_SCAN (chained scan, f32 stable
+    filters; numerics in include/b200sdr.h)."""
+    _exec = lib.b2s_iir_exec
+    _host = None
+    _destroy = lib.b2s_iir_destroy
+    _length = lib.b2s_iir_length
+
+    def __init__(self, a_taps, b_taps, sample_dtype=np.float32, ctx: Context | None = None,
+                 algo: int = _lib.ALGO_AUTO):
+        super().__init__(ctx)
+        self.sample_dtype = np.dtype(sample_dtype)
+        if self.sample_dtype == np.float64:
+            ct, plan = C.c_double, lib.b2s_iir_plan_f64
+        elif self.sample_dtype == np.float32:
+            ct, plan = C.c_float, lib.b2s_iir_plan_f32
+        else:
+            raise TypeError("IirFilter has f32 x f32 and f64 x f64 impls only (iir.rs:56-76)")
+        a = np.ascontiguousarray(np.asarray(a_taps, dtype=self.sample_dtype).reshape(-1))
+        b = np.ascontiguousarray(np.asarray(b_taps, dtype=self.sample_dtype).reshape(-1))
+        self.a_taps, self.b_taps = a, b
+        check(plan(self.ctx.handle, a.ctypes.data_as(C.POINTER(ct)), a.size, b.ctypes.data_as(C.POINTER(ct)), b.size,
+                   C.byref(self._h)), self.ctx.handle)
+        if algo != _lib.ALGO_AUTO:
+            self.set_algo(algo)
+
+    def set_algo(self, algo: int):
+        check(lib.b2s_iir_set_algo(self._h, algo), self.ctx.handle)
+
+    @property
+    def algo(self) -> int:
+        return lib.b2s_iir_get_algo(self._h)
+
+
 class PolyphaseResamplingFir(_FilterBase):
     """futuredsp::PolyphaseResamplingFir (crates/futuredsp/src/polyphase_resampling_fir.rs:42-124)."""
     _exec = lib.b2s_resamp_exec

@@ -70,7 +70,9 @@ typedef enum {
                           * outputs are unaffected and no finite output is ever wrong.  f32 DENORMAL samples may count as
                           * zero (tensor-core operands may be flushed to zero).  Streams that may carry
                           * non-finite samples and need the reference's exact propagation: use B2S_ALGO_DIRECT. */
-    B2S_ALGO_FFT    = 3  /* overlap-save FFT convolution (c32 samples, 64..2049 taps, decim == 1)  */
+    B2S_ALGO_FFT    = 3, /* overlap-save FFT convolution (c32 samples, 64..2049 taps, decim == 1)  */
+    B2S_ALGO_SCAN   = 4  /* IIR only (b2s_iir_set_algo): single-pass chained scan, see b2s_iir below;
+                          * b2s_fir_set_algo rejects it */
 } b2s_algo;
 
 typedef struct b2s_ctx    b2s_ctx;
@@ -254,6 +256,45 @@ int32_t b2s_mavg_create(b2s_ctx *ctx, size_t width, float decay_factor, size_t h
 void    b2s_mavg_destroy(b2s_mavg *m);
 int32_t b2s_mavg_exec(b2s_mavg *m, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
                       size_t *consumed, size_t *produced);
+
+/* ---- IirFilter (≙ crates/futuredsp/src/iir.rs:33-178, the core of src/blocks/iir.rs): StatefulFilter::filter.
+ * y = sum_j b[j] * x[k + n_b - 1 - j] + sum_j a[j] * memory[j] (PLUS sign on the a-term, b[0] multiplies the newest
+ * sample), then memory shifts and memory[0] = y.  Before the first output `memory` is filled with the stream's first
+ * n_a INPUT samples (memory[0] = x[0]); those are not consumed and a call that fills memory returns (0, 0).  Each call
+ * produces n = min(n_in - n_b + 1, n_out_cap) outputs and consumes as many; the status is the reference's (:166-177).
+ * memory and the fill count live in the plan (on the device): calls are stream-ordered and never synchronise.
+ * n_b == 0 is B2S_EINVAL (the reference asserts, :132); n_a and n_b are each limited to 2048.  Input and output
+ * slices must not overlap.
+ * Algorithms:
+ *   B2S_ALGO_DIRECT  one thread runs the recurrence with un-fused IEEE multiply/add in the reference's order:
+ *                    bit-identical to the reference for f32 and f64, denormals and non-finite values included (NaN
+ *                    payloads aside).  About 5-12 Msamples/s (one GPU thread walks the recurrence).
+ *   B2S_ALGO_SCAN    f32 only; 1 <= n_a <= 8, n_b <= 64 and a stable filter: ||A^(2^20)|| < 1e-3 in f64 (A: the
+ *                    companion matrix of a), i.e. max|pole| < 1 - 6.6e-6.  Blocked scan of the state recurrence with
+ *                    decoupled look-back across 4096-output tiles, 8 B/sample of HBM traffic.
+ *                    Numerics: each run of 16 outputs is re-computed with the reference's operations from a start
+ *                    state that the scan evaluates in a different order (f32 FMA, matrix powers rounded from f64),
+ *                    so outputs are not bit-identical to the reference.  With G = ||h||_1 + sum_j ||g_j||_1 (h: the
+ *                    impulse response, g_j: the zero-input response to memory e_j), the error against the exact
+ *                    (f64) recurrence is within max(1e-5 G max|x|, 2 x the reference's own f32 error), and the
+ *                    distance to the reference within 1e-5 G max|x| + the reference's own f32 error.  Near the unit
+ *                    circle on DC input the f32 reference itself drifts by ~eps/(1-r); the scan stays closer to the
+ *                    exact value there.  A NaN/Inf input at index i makes every output from i - n_b + 1 on
+ *                    non-finite, exactly the reference's set (0 * NaN = NaN carries it through the state).
+ *                    A look-back wait that exceeds 4 s gives up and b2s_ctx_sync reports B2S_ETIMEOUT.
+ *   B2S_ALGO_AUTO    SCAN when the plan is admitted, otherwise DIRECT; a pure-FIR plan (n_a == 0) runs on a FIR plan
+ *                    with taps = b (the same sum, added oldest sample first) and b2s_iir_get_algo reports the FIR's
+ *                    algorithm.  The choice depends on the plan only, never on the call size. */
+typedef struct b2s_iir b2s_iir;
+int32_t b2s_iir_plan_f32(b2s_ctx *ctx, const float *a_taps, size_t n_a, const float *b_taps, size_t n_b, b2s_iir **out);
+int32_t b2s_iir_plan_f64(b2s_ctx *ctx, const double *a_taps, size_t n_a, const double *b_taps, size_t n_b,
+                         b2s_iir **out);
+void    b2s_iir_destroy(b2s_iir *f);
+size_t  b2s_iir_length(const b2s_iir *f);            /* ≙ StatefulFilter::length: n_b */
+int32_t b2s_iir_set_algo(b2s_iir *f, b2s_algo algo); /* AUTO, DIRECT or SCAN; SCAN on a plan it does not admit: EUNSUPPORTED */
+int32_t b2s_iir_get_algo(const b2s_iir *f);          /* the algorithm AUTO resolved to */
+int32_t b2s_iir_exec(b2s_iir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
+                     size_t *consumed, size_t *produced, int32_t *status);
 
 /* ---- fused spectrum pipe (SURVEY §8f-3): Fft::with_options(n, Forward, fft_shift, None) -> Apply(|x|^2) ->
  * MovingAvg<n>::new(decay_factor, history_size) [-> log10_scale * log10(.) when log10_scale != 0] of

@@ -3,8 +3,8 @@
 //
 //   futuredsp::Filter::filter(&self, &[In], &mut [Out]) -> (usize, usize, ComputationStatus)
 //                                     (crates/futuredsp/src/lib.rs:48-68)
-//   futuredsp::{FirFilter, DecimatingFirFilter, PolyphaseResamplingFir}
-//   futuresdr::blocks::{Fir, FirBuilder, Fft, Apply, PfbArbResampler}   (src/blocks/*.rs)
+//   futuredsp::{FirFilter, DecimatingFirFilter, PolyphaseResamplingFir, IirFilter}
+//   futuresdr::blocks::{Fir, FirBuilder, Iir, IirBuilder, Fft, Apply, PfbArbResampler}   (src/blocks/*.rs)
 //   futuresdr::runtime::{WorkIo, mocker::Mocker}                        (work_io.rs, mocker.rs)
 //
 // The reference is Rust; no Rust toolchain exists in this image, so this header is the
@@ -160,6 +160,48 @@ private:
     b2s_resamp *plan_ = nullptr;
 };
 
+// ≙ futuredsp::IirFilter (crates/futuredsp/src/iir.rs:33-178), a StatefulFilter: memory and its fill count live in the
+// plan, so filter() is non-const and consecutive calls continue one stream.  Sample = float or double (:56-76).
+template <typename Sample> class IirFilter {
+    static_assert(std::is_same_v<Sample, float> || std::is_same_v<Sample, double>, "IirFilter: f32 or f64 only");
+public:
+    IirFilter(const Instance &inst, const std::vector<Sample> &a_taps, const std::vector<Sample> &b_taps,
+              b2s_algo algo = B2S_ALGO_AUTO)
+        : inst_(inst) {
+        if constexpr (std::is_same_v<Sample, float>)
+            check(b2s_iir_plan_f32(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), &plan_), inst.get());
+        else
+            check(b2s_iir_plan_f64(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), &plan_), inst.get());
+        if (algo != B2S_ALGO_AUTO) set_algo(algo);
+    }
+    ~IirFilter() { b2s_iir_destroy(plan_); }
+    IirFilter(const IirFilter &) = delete;
+    IirFilter &operator=(const IirFilter &) = delete;
+    void set_algo(b2s_algo algo) { check(b2s_iir_set_algo(plan_, algo), inst_.get()); }
+    int algo() const { return b2s_iir_get_algo(plan_); }
+    size_t length() const { return b2s_iir_length(plan_); }
+    // device slices (asynchronous on the instance's stream)
+    FilterResult filter_device(const Sample *i, size_t n_in, Sample *o, size_t n_out) {
+        size_t c = 0, p = 0; int32_t st = 0;
+        check(b2s_iir_exec(plan_, i, n_in, o, n_out, &c, &p, &st), inst_.get());
+        return {c, p, static_cast<ComputationStatus>(st)};
+    }
+    // host slices: staged through device memory
+    FilterResult filter(const Sample *i, size_t n_in, Sample *o, size_t n_out) {
+        Sample *di = inst_.device_alloc<Sample>(n_in + 1), *dout = inst_.device_alloc<Sample>(n_out + 1);
+        inst_.upload(di, i, n_in);
+        auto r = filter_device(di, n_in, dout, n_out);
+        inst_.download(o, dout, std::get<1>(r));
+        inst_.device_free(di); inst_.device_free(dout);
+        return r;
+    }
+    FilterResult filter(const std::vector<Sample> &i, std::vector<Sample> &o) { return filter(i.data(), i.size(), o.data(), o.size()); }
+
+private:
+    const Instance &inst_;
+    b2s_iir *plan_ = nullptr;
+};
+
 // ---- firdes (futuredsp::firdes::kaiser, firdes/basic.rs:310-459) ---------------------------------
 namespace firdes::kaiser {
 inline std::vector<float> lowpass(double cutoff, double transition_bw, double max_ripple) {
@@ -249,6 +291,35 @@ struct FirBuilder {
     static Fir<Sample> resampling_with_taps(const Instance &i, size_t interp, size_t decim, const std::vector<float> &taps) {
         if (taps.size() % interp) throw Error(B2S_EINVAL, "taps.num_taps().is_multiple_of(interp)");   // :56
         return Fir<Sample>(i, std::make_unique<PolyphaseResamplingFir<Sample>>(i, interp, decim, taps));
+    }
+};
+
+// ≙ blocks::Iir (src/blocks/iir.rs:8-176)
+template <typename Sample> class Iir {
+public:
+    Iir(const Instance &inst, std::unique_ptr<IirFilter<Sample>> core) : input(inst), output(inst), core_(std::move(core)) {}
+    size_t length() const { return core_->length(); }                                  // set_min_items(n_b), :133
+    void work(WorkIo &io) {                                                        // iir.rs:156-175
+        auto [consumed, produced, status] = core_->filter_device(input.slice(), input.len(), output.slice(), output.capacity());
+        input.consume(consumed);
+        output.produce(produced);
+        if (input.finished() && status != ComputationStatus::InsufficientOutput) io.finished = true;
+    }
+    Reader<Sample> input;
+    Writer<Sample> output;
+private:
+    std::unique_ptr<IirFilter<Sample>> core_;
+};
+
+// ≙ blocks::IirBuilder (src/blocks/iir.rs:32-64)
+struct IirBuilder {
+    template <typename Sample>
+    static Iir<Sample> iir(const Instance &i, const std::vector<Sample> &a_taps, const std::vector<Sample> &b_taps) {
+        return Iir<Sample>(i, std::make_unique<IirFilter<Sample>>(i, a_taps, b_taps));
+    }
+    template <typename Sample>
+    static Iir<Sample> same_type(const Instance &i, const std::vector<Sample> &a_taps, const std::vector<Sample> &b_taps) {
+        return iir<Sample>(i, a_taps, b_taps);
     }
 };
 

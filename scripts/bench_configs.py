@@ -44,11 +44,50 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 
 def want(section):
-    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, scale)."""
+    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
     return True
+
+
+def iir_section(quick):
+    """IirFilter: SCAN on 64 Mi samples per call, DIRECT (sequential, bit-exact) on 1 Mi, and the oracle's one-thread
+    rate (the recurrence cannot be split across host threads).  8 B/sample of HBM traffic (4 in, 4 out)."""
+    from scipy import signal
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import iir_oracle as orc
+    n = (16 if quick else 64) << 20
+    bb, aa = signal.butter(2, 0.1)
+    b6, a6 = signal.butter(6, 0.1)
+    poles = 0.9 * np.exp(1j * np.linspace(0.3, 2.8, 3))
+    a7 = -np.real(np.poly(np.concatenate([poles, poles.conj(), [0.5]])))[1:]
+    shapes = {"biquad": (-aa[1:], bb), "dc_blocker": ([0.995], [1.0, -1.0]), "butter6": (-a6[1:], b6),
+              "na7_nb1": (a7, [1.0])}
+    g = torch.Generator(device="cuda").manual_seed(3)
+    x = torch.randn(n + 64, generator=g, device="cuda")
+    y = torch.empty(n + 64, device="cuda")
+    for name, (a, b) in shapes.items():
+        f = fb.IirFilter(np.float32(a), np.float32(b), np.float32, algo=fb.ALGO_SCAN)
+        sec = timeit(lambda: f.filter(x[: n + len(b) - 1], y[:n]), iters=10, warm=3)
+        report(f"iir_scan_{name}", n, 8 * n, sec, extra=f"Gsamples_s={n / sec / 1e9:.2f}")
+    nd = 1 << 20
+    for name, (a, b) in shapes.items():
+        f = fb.IirFilter(np.float32(a), np.float32(b), np.float32, algo=fb.ALGO_DIRECT)
+        sec = timeit(lambda: f.filter(x[: nd + len(b) - 1], y[:nd]), iters=3, warm=1)
+        report(f"iir_direct_{name}", nd, 8 * nd, sec, extra=f"Gsamples_s={nd / sec / 1e9:.4f}")
+    x64 = torch.randn(nd + 64, dtype=torch.float64, generator=g, device="cuda")
+    y64 = torch.empty(nd + 64, dtype=torch.float64, device="cuda")
+    f = fb.IirFilter(-aa[1:], bb, np.float64)
+    sec = timeit(lambda: f.filter(x64[: nd + 2], y64[:nd]), iters=3, warm=1)
+    report("iir64_direct_biquad", nd, 16 * nd, sec, extra=f"Gsamples_s={nd / sec / 1e9:.4f}")
+    xc = x[:nd].cpu().numpy()
+    orc.lib()                                   # compile the oracle outside the timed window
+    for name, (a, b) in shapes.items():
+        t0 = time.perf_counter()
+        orc.iir(np.float32(a), np.float32(b), xc)
+        sec = time.perf_counter() - t0
+        report(f"iir_oracle_1thread_{name}", nd, 8 * nd, sec, extra=f"CPU, one thread; Gsamples_s={nd / sec / 1e9:.4f}")
 
 
 def main():
@@ -228,6 +267,8 @@ def main():
             keep.work(B.WorkIo())
         sec = timeit(run_spec, iters=5, warm=1)
         report("spectrum_pipe_fft2048_normsqr_mavg", n, 8 * n + 4 * (n // 3), sec, extra="unfused: 3 kernels, 32 B/sample of HBM traffic")
+    if want("iir"):
+        iir_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
