@@ -3,7 +3,8 @@ FFT / Apply / PfbArbResampler hot path.
 
 Python host layer above the C ABI (include/b200sdr.h).  Class and method names mirror the
 reference's Rust API for this path (futuredsp::{FirFilter, DecimatingFirFilter,
-PolyphaseResamplingFir}, futuresdr::blocks::{Fir, FirBuilder, Fft, Apply, PfbArbResampler},
+PolyphaseResamplingFir}, futuresdr::blocks::{Fir, FirBuilder, Fft, Apply, PfbArbResampler,
+SignalSource, SignalSourceBuilder, FixedPointPhase, Head},
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -15,6 +16,9 @@ from ._lib import (  # noqa: F401
 from .context import Context, default_context  # noqa: F401
 from .filters import (  # noqa: F401
     ComputationStatus, FirFilter, DecimatingFirFilter, PolyphaseResamplingFir, IirFilter,
+)
+from .blocks import (  # noqa: F401
+    FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
 )
 from . import firdes  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain): futuresdr_b200.edges

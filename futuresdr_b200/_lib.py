@@ -19,6 +19,7 @@ F32_F32, C32_F32, C32_C32, F64_F64 = 0, 1, 2, 3
 ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
  OP_MAG_C32, OP_LOG10_F32) = range(8)
+WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
 
 _vp, _sz, _i32, _f32 = C.c_void_p, C.c_size_t, C.c_int32, C.c_float
 _szp, _i32p, _vpp, _f32p = C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_float)
@@ -91,7 +92,14 @@ SIGNATURES = {
     "b2s_iir_set_algo": (_i32, [_vp, C.c_int]),
     "b2s_iir_get_algo": (_i32, [_vp]),
     "b2s_iir_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp, _i32p]),
-    "b2s_spectrum_plan": (_i32, [_vp, _sz, _i32, _f32, _sz, _f32, _vpp]),
+    "b2s_sigsrc_create": (_i32, [_vp, C.c_int, _i32, _f32, _f32, _f32, _f32, _vpp]),
+    "b2s_sigsrc_destroy": (None, [_vp]),
+    "b2s_sigsrc_set_amplitude": (_i32, [_vp, _f32]),
+    "b2s_sigsrc_phase": (_i32, [_vp, _i32p, _i32p]),
+    "b2s_sigsrc_exec": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_fxpt_phase_new": (_i32, [_f32, _i32p]),
+    "b2s_fxpt_sin_cos": (_i32, [_i32, _f32p, _f32p]),
+    "b2s_spectrum_plan":(_i32, [_vp, _sz, _i32, _f32, _sz, _f32, _vpp]),
     "b2s_spectrum_destroy": (None, [_vp]),
     "b2s_spectrum_reset": (_i32, [_vp]),
     "b2s_spectrum_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp]),

@@ -3,6 +3,8 @@
 Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``Fir`` / ``FirBuilder``      src/blocks/fir.rs:13-95, :126-233
   * ``Iir`` / ``IirBuilder``      src/blocks/iir.rs:8-176
+  * ``SignalSource`` / ``SignalSourceBuilder`` / ``FixedPointPhase``   src/blocks/signal_source/{mod,fxpt_phase}.rs
+  * ``Head``                      src/blocks/head.rs:22-84
   * ``Fft`` / ``FftDirection``    src/blocks/fft.rs:30-221
   * ``Apply``                     src/blocks/apply.rs:100-131 (closed catalogue of closures)
   * ``PfbArbResampler``           src/blocks/pfb/arb_resampler.rs:72-231
@@ -209,6 +211,128 @@ class IirBuilder:
     @staticmethod
     def same_type(a_taps, b_taps, sample_dtype=np.float32, ctx: Optional[Context] = None) -> Iir:
         return IirBuilder.iir(a_taps, b_taps, sample_dtype, ctx)
+
+
+class FixedPointPhase:
+    """blocks::FixedPointPhase (src/blocks/signal_source/fxpt_phase.rs:8-99): a phase as a wrapping i32, -2^31 = -pi.
+    ``new``, ``sin`` and ``cos`` run on the host through the library (b2s_fxpt_phase_new / b2s_fxpt_sin_cos)."""
+
+    def __init__(self, value: int):
+        v = int(value) & 0xFFFFFFFF
+        self.value = v - (1 << 32) if v >= 1 << 31 else v
+
+    @classmethod
+    def new(cls, x: float) -> "FixedPointPhase":
+        v = C.c_int32(0)
+        check(lib.b2s_fxpt_phase_new(float(np.float32(x)), C.byref(v)))
+        return cls(v.value)
+
+    def _sin_cos(self):
+        s, c = C.c_float(0.0), C.c_float(0.0)
+        check(lib.b2s_fxpt_sin_cos(self.value, C.byref(s), C.byref(c)))
+        return np.float32(s.value), np.float32(c.value)
+
+    def sin(self) -> np.float32:
+        return self._sin_cos()[0]
+
+    def cos(self) -> np.float32:
+        return self._sin_cos()[1]
+
+
+class SignalWave(enum.IntEnum):
+    """The phase-to-amplitude closures of SignalSourceBuilder (b2s_wave)."""
+    Cos = _lib.WAVE_COS
+    Sin = _lib.WAVE_SIN
+    Square = _lib.WAVE_SQUARE
+
+
+class SignalSource(Block):
+    """blocks::SignalSource (src/blocks/signal_source/mod.rs:29-108): a source without an input port.  Each ``work``
+    fills the whole output slice and the block never finishes; the samples are bit-identical to the reference's."""
+    in_dtype = None
+
+    def __init__(self, wave: SignalWave, frequency: float, sample_rate: float, amplitude: float,
+                 initial_phase: float, dtype=np.float32, ctx: Optional[Context] = None):
+        self.out_dtype = np.dtype(dtype)
+        if self.out_dtype not in (np.dtype(np.float32), np.dtype(np.complex64)):
+            raise ValueError(f"SignalSource: f32 or Complex32 items, not {self.out_dtype}")
+        self.ctx = ctx or default_context()
+        self.wave = SignalWave(wave)
+        self._h = C.c_void_p()
+        check(lib.b2s_sigsrc_create(self.ctx.handle, int(self.wave), int(self.out_dtype == np.complex64),
+                                    float(np.float32(frequency)), float(np.float32(sample_rate)),
+                                    float(np.float32(amplitude)), float(np.float32(initial_phase)), C.byref(self._h)),
+              self.ctx.handle)
+        self.input = None
+        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
+
+    def set_amplitude(self, amplitude: float):
+        """SignalSource::set_amplitude (mod.rs:71-73): applies from the next call."""
+        check(lib.b2s_sigsrc_set_amplitude(self._h, float(np.float32(amplitude))), self.ctx.handle)
+
+    def phase(self) -> tuple[FixedPointPhase, FixedPointPhase]:
+        """(the next sample's phase, the per-sample increment) of the NCO."""
+        v, inc = C.c_int32(0), C.c_int32(0)
+        check(lib.b2s_sigsrc_phase(self._h, C.byref(v), C.byref(inc)), self.ctx.handle)
+        return FixedPointPhase(v.value), FixedPointPhase(inc.value)
+
+    def generate(self, o: torch.Tensor) -> int:
+        """Fill the device slice ``o`` (asynchronous on the context's stream); returns the items written."""
+        p = C.c_size_t(0)
+        check(lib.b2s_sigsrc_exec(self._h, C.c_void_p(o.data_ptr()), o.numel(), C.byref(p)), self.ctx.handle)
+        return p.value
+
+    def work(self, io: WorkIo):
+        o = self.output.slice()                                                 # mod.rs:94-104
+        self.output.produce(self.generate(o))
+
+    def __del__(self):
+        try:                                   # (module globals may already be gone at interpreter shutdown)
+            if getattr(self, "_h", None):
+                lib.b2s_sigsrc_destroy(self._h)
+                self._h = None
+        except Exception:  # noqa: BLE001
+            pass
+
+
+class SignalSourceBuilder:
+    """blocks::SignalSourceBuilder (src/blocks/signal_source/mod.rs:110-227); ``dtype`` picks the item type (the
+    reference's type parameter): np.float32 or np.complex64."""
+
+    @staticmethod
+    def cos(frequency, sample_rate, amplitude, initial_phase, dtype=np.float32, ctx=None) -> SignalSource:
+        return SignalSource(SignalWave.Cos, frequency, sample_rate, amplitude, initial_phase, dtype, ctx)
+
+    @staticmethod
+    def sin(frequency, sample_rate, amplitude, initial_phase, dtype=np.float32, ctx=None) -> SignalSource:
+        return SignalSource(SignalWave.Sin, frequency, sample_rate, amplitude, initial_phase, dtype, ctx)
+
+    @staticmethod
+    def square(frequency, sample_rate, amplitude, initial_phase, dtype=np.float32, ctx=None) -> SignalSource:
+        return SignalSource(SignalWave.Square, frequency, sample_rate, amplitude, initial_phase, dtype, ctx)
+
+
+class Head(Block):
+    """blocks::Head (src/blocks/head.rs:22-84): copies the first ``n_items`` input items and finishes once it has
+    copied them all -- not when its input finishes."""
+
+    def __init__(self, dtype, n_items: int, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.in_dtype = self.out_dtype = np.dtype(dtype)
+        self.n_items = int(n_items)
+        self._ports()
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()                          # head.rs:63-83
+        m = min(self.n_items, i.numel(), o.numel())
+        if m > 0:
+            check(lib.b2s_memcpy_d2d(self.ctx.handle, C.c_void_p(o.data_ptr()), C.c_void_p(i.data_ptr()),
+                                     m * self.in_dtype.itemsize), self.ctx.handle)
+            self.n_items -= m
+            if self.n_items == 0:
+                io.finished = True
+            self.input.consume(m)
+            self.output.produce(m)
 
 
 class FftDirection(enum.Enum):

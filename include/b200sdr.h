@@ -296,6 +296,36 @@ int32_t b2s_iir_get_algo(const b2s_iir *f);          /* the algorithm AUTO resol
 int32_t b2s_iir_exec(b2s_iir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
                      size_t *consumed, size_t *produced, int32_t *status);
 
+/* ---- SignalSource (≙ src/blocks/signal_source/mod.rs:29-227, SignalSourceBuilder :110-227) with its fixed-point NCO
+ * (fxpt_nco.rs:3-43) and FixedPointPhase (fxpt_phase.rs:8-99).  A source: no input, each exec fills the WHOLE output
+ * slice (mod.rs:94-104) and the block never finishes.  The phase is a wrapping 32-bit integer, so output k of a call
+ * is f(phase0 + k inc) * amplitude with nothing carried between samples: the device output is bit-identical to the
+ * reference at any stream length, signed zeros from a zero or negative amplitude included.  NaN outputs (NaN amplitude,
+ * or 0 * inf) carry the bit patterns of the reference's f32 multiply on x86-64: the amplitude's NaN quieted, or the
+ * default NaN 0xFFC00000.
+ *   create: phase0 = FixedPointPhase::new(initial_phase), inc = FixedPointPhase::new(((2 PI) frequency) / sample_rate),
+ *           all in f32 (mod.rs:130-133).  Like the reference nothing is validated: sample_rate == 0, NaN or inf give
+ *           whatever FixedPointPhase::new makes of them (Rust's saturating `as i32`, NaN -> 0).
+ *   waves:  f32       COS cos(phase), SIN sin(phase), SQUARE (value < 0 ? 1 : 0)
+ *           Complex32 COS and SIN both (cos, sin) (mod.rs:175-199); SQUARE maps value >> 30 as -2 -> (1,0),
+ *           -1 -> (1,1), 0 -> (0,1), 1 -> (0,0) (:213-221); each times amplitude.
+ *   exec:   writes n_out_cap items at d_out (4-byte aligned; no other alignment needed), *produced = n_out_cap, then
+ *           advances the phase by n_out_cap steps.  Phase and increment live in the plan on the host: calls are
+ *           stream-ordered and never synchronise.  set_amplitude applies from the next exec. */
+typedef enum { B2S_WAVE_COS = 0, B2S_WAVE_SIN = 1, B2S_WAVE_SQUARE = 2 } b2s_wave;
+typedef struct b2s_sigsrc b2s_sigsrc;
+int32_t b2s_sigsrc_create(b2s_ctx *ctx, b2s_wave wave, int32_t complex_items, float frequency, float sample_rate,
+                          float amplitude, float initial_phase, b2s_sigsrc **out);
+void    b2s_sigsrc_destroy(b2s_sigsrc *s);
+int32_t b2s_sigsrc_set_amplitude(b2s_sigsrc *s, float amplitude);      /* ≙ SignalSource::set_amplitude (:71-73) */
+/* the NCO's current phase (the next sample's FixedPointPhase::value) and its increment */
+int32_t b2s_sigsrc_phase(const b2s_sigsrc *s, int32_t *value, int32_t *inc);
+int32_t b2s_sigsrc_exec(b2s_sigsrc *s, void *d_out, size_t n_out_cap, size_t *produced);
+/* Host-only mirrors of the public FixedPointPhase (need no device): new(x) (fxpt_phase.rs:75-82) and sin() / cos()
+ * (:85-98) of a phase value, from the same sine table the kernel uses. */
+int32_t b2s_fxpt_phase_new(float x, int32_t *value);
+int32_t b2s_fxpt_sin_cos(int32_t value, float *sin_out, float *cos_out);
+
 /* ---- fused spectrum pipe (SURVEY §8f-3): Fft::with_options(n, Forward, fft_shift, None) -> Apply(|x|^2) ->
  * MovingAvg<n>::new(decay_factor, history_size) [-> log10_scale * log10(.) when log10_scale != 0] of
  * examples/spectrum/src/bin/cpu.rs:21-28 in ONE pass over the samples: 8 B/sample in, n floats per `history_size`

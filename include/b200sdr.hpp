@@ -4,7 +4,8 @@
 //   futuredsp::Filter::filter(&self, &[In], &mut [Out]) -> (usize, usize, ComputationStatus)
 //                                     (crates/futuredsp/src/lib.rs:48-68)
 //   futuredsp::{FirFilter, DecimatingFirFilter, PolyphaseResamplingFir, IirFilter}
-//   futuresdr::blocks::{Fir, FirBuilder, Iir, IirBuilder, Fft, Apply, PfbArbResampler}   (src/blocks/*.rs)
+//   futuresdr::blocks::{Fir, FirBuilder, Iir, IirBuilder, Fft, Apply, PfbArbResampler, SignalSource,
+//                       SignalSourceBuilder, FixedPointPhase, Head}                       (src/blocks/*.rs)
 //   futuresdr::runtime::{WorkIo, mocker::Mocker}                        (work_io.rs, mocker.rs)
 //
 // The reference is Rust; no Rust toolchain exists in this image, so this header is the
@@ -12,6 +13,7 @@
 // C++17, links against libb200sdr.so.  Errors the reference panics/asserts on throw b2s::Error.
 #pragma once
 
+#include <algorithm>
 #include <complex>
 #include <cstdint>
 #include <cstring>
@@ -20,6 +22,7 @@
 #include <string>
 #include <tuple>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "b200sdr.h"
@@ -321,6 +324,79 @@ struct IirBuilder {
     static Iir<Sample> same_type(const Instance &i, const std::vector<Sample> &a_taps, const std::vector<Sample> &b_taps) {
         return iir<Sample>(i, a_taps, b_taps);
     }
+};
+
+// ≙ blocks::FixedPointPhase (src/blocks/signal_source/fxpt_phase.rs:8-99), evaluated on the host by the library
+struct FixedPointPhase {
+    int32_t value = 0;
+    static FixedPointPhase make(float x) { FixedPointPhase p; check(b2s_fxpt_phase_new(x, &p.value)); return p; }   // ::new
+    float sin() const { float s, c; check(b2s_fxpt_sin_cos(value, &s, &c)); return s; }
+    float cos() const { float s, c; check(b2s_fxpt_sin_cos(value, &s, &c)); return c; }
+};
+
+// ≙ blocks::SignalSource (src/blocks/signal_source/mod.rs:29-108): no input; work() fills the whole output slice and
+// never finishes.  T = float or Complex32.
+template <typename T> class SignalSource {
+    static_assert(std::is_same_v<T, float> || std::is_same_v<T, Complex32>, "SignalSource: f32 or Complex32 items");
+public:
+    SignalSource(const Instance &inst, b2s_wave wave, float frequency, float sample_rate, float amplitude,
+                 float initial_phase)
+        : output(inst), inst_(inst) {
+        check(b2s_sigsrc_create(inst.get(), wave, std::is_same_v<T, Complex32> ? 1 : 0, frequency, sample_rate,
+                                amplitude, initial_phase, &h_), inst.get());
+    }
+    ~SignalSource() { b2s_sigsrc_destroy(h_); }
+    SignalSource(const SignalSource &) = delete;
+    SignalSource &operator=(const SignalSource &) = delete;
+    void set_amplitude(float amplitude) { check(b2s_sigsrc_set_amplitude(h_, amplitude), inst_.get()); }   // :71-73
+    // (the next sample's phase, the increment)
+    std::pair<FixedPointPhase, FixedPointPhase> phase() const {
+        FixedPointPhase v, inc;
+        check(b2s_sigsrc_phase(h_, &v.value, &inc.value), inst_.get());
+        return {v, inc};
+    }
+    void work(WorkIo &) {                                                           // mod.rs:88-107
+        size_t p = 0;
+        check(b2s_sigsrc_exec(h_, output.slice(), output.capacity(), &p), inst_.get());
+        output.produce(p);
+    }
+    Writer<T> output;
+private:
+    const Instance &inst_; b2s_sigsrc *h_ = nullptr;
+};
+
+// ≙ blocks::SignalSourceBuilder (src/blocks/signal_source/mod.rs:110-227)
+template <typename T> struct SignalSourceBuilder {
+    static SignalSource<T> cos(const Instance &i, float frequency, float sample_rate, float amplitude, float initial_phase) {
+        return SignalSource<T>(i, B2S_WAVE_COS, frequency, sample_rate, amplitude, initial_phase);
+    }
+    static SignalSource<T> sin(const Instance &i, float frequency, float sample_rate, float amplitude, float initial_phase) {
+        return SignalSource<T>(i, B2S_WAVE_SIN, frequency, sample_rate, amplitude, initial_phase);
+    }
+    static SignalSource<T> square(const Instance &i, float frequency, float sample_rate, float amplitude, float initial_phase) {
+        return SignalSource<T>(i, B2S_WAVE_SQUARE, frequency, sample_rate, amplitude, initial_phase);
+    }
+};
+
+// ≙ blocks::Head (src/blocks/head.rs:22-84): copies the first n_items items, finishes when n_items reaches 0
+template <typename T> class Head {
+public:
+    Head(const Instance &inst, uint64_t n_items) : input(inst), output(inst), inst_(inst), n_items_(n_items) {}
+    uint64_t n_items() const { return n_items_; }
+    void work(WorkIo &io) {                                                        // head.rs:57-83
+        const size_t m = (size_t)std::min<uint64_t>(n_items_, std::min(input.len(), output.capacity()));
+        if (m > 0) {
+            check(b2s_memcpy_d2d(inst_.get(), output.slice(), input.slice(), m * sizeof(T)), inst_.get());
+            n_items_ -= m;
+            if (n_items_ == 0) io.finished = true;
+            input.consume(m);
+            output.produce(m);
+        }
+    }
+    Reader<T> input;
+    Writer<T> output;
+private:
+    const Instance &inst_; uint64_t n_items_;
 };
 
 // ≙ blocks::Fft (src/blocks/fft.rs:30-221)

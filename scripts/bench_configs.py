@@ -44,7 +44,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 
 def want(section):
-    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, scale)."""
+    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -88,6 +88,44 @@ def iir_section(quick):
         orc.iir(np.float32(a), np.float32(b), xc)
         sec = time.perf_counter() - t0
         report(f"iir_oracle_1thread_{name}", nd, 8 * nd, sec, extra=f"CPU, one thread; Gsamples_s={nd / sec / 1e9:.4f}")
+
+
+def sigsrc_section(quick):
+    """SignalSource: 64 Mi items per call, write-only traffic (4 B/sample f32, 8 B/sample Complex32) against the
+    3.35 TB/s data-sheet figure.  fs/64 is in the set because its increment (2^26) puts neighbouring samples 16 table
+    entries apart, the stride that would collapse an unpadded shared-memory table onto one bank; fs/4 makes every
+    lane of a warp read the same entry.  The oracle's one-thread CPU rate is given for context."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import sigsrc_oracle as orc
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({"kernel": "sigsrc_device", "gpu": q[torch.cuda.current_device()] if q else "unknown"}), flush=True)
+    n = (16 if quick else 64) << 20
+    fs = 48000.0
+    freqs = {"1k": 1000.0, "48k": 48000.0, "fs4": fs / 4, "fs64": fs / 64}
+    cases = [("f32_sin", fb.SignalWave.Sin, np.float32), ("c32_sin", fb.SignalWave.Sin, np.complex64),
+             ("c32_square", fb.SignalWave.Square, np.complex64)]
+    out = {np.float32: torch.empty(n, dtype=torch.float32, device="cuda"),
+           np.complex64: torch.empty(n, dtype=torch.complex64, device="cuda")}
+    for name, wave, dt in cases:
+        bps = np.dtype(dt).itemsize
+        for fname, f in freqs.items():
+            src = fb.SignalSource(wave, f, fs, 0.5, 0.0, dt)
+            sec = timeit(lambda: src.generate(out[dt]), iters=20, warm=3)
+            gbs = bps * n / sec / 1e9
+            print(json.dumps({"kernel": f"sigsrc_{name}_{fname}", "items": n, "ms": round(sec * 1e3, 4),
+                              "Gsamples_s": round(n / sec / 1e9, 2), "bytes_written": bps * n,
+                              "write_GBs": round(gbs, 1), "frac_3350GBs": round(gbs / 3350.0, 4)}), flush=True)
+    nc = 4 << 20
+    for name, wave, dt in cases:
+        ref = orc.Source(int(wave), 1000.0, fs, 0.5, 0.0, dt)
+        ref.work(1024)                              # compile the oracle outside the timed window
+        t0 = time.perf_counter()
+        ref.work(nc)
+        sec = time.perf_counter() - t0
+        print(json.dumps({"kernel": f"sigsrc_oracle_1thread_{name}", "items": nc,
+                          "Gsamples_s": round(nc / sec / 1e9, 4), "note": "CPU, one thread"}), flush=True)
 
 
 def main():
@@ -269,6 +307,8 @@ def main():
         report("spectrum_pipe_fft2048_normsqr_mavg", n, 8 * n + 4 * (n // 3), sec, extra="unfused: 3 kernels, 32 B/sample of HBM traffic")
     if want("iir"):
         iir_section(quick)
+    if want("sigsrc"):
+        sigsrc_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
