@@ -8,7 +8,9 @@
 // resamp_kernel below: the host rearranges the taps once into bank-major, time-reversed rows  G[b][t] =
 // taps[L*(T-1-t) + b]  (row pitch odd so lanes on different banks hit different smem banks).
 // A CTA produces TK consecutive outputs: it stages the contiguous input span those outputs
-// touch plus the bank table in shared memory, then each thread walks its outputs' T taps.
+// touch plus the bank table in shared memory, then each thread walks its outputs' T taps.  Plans whose span does not
+// fit that tile (200 KiB) run resamp_naive_kernel, one thread per output reading global memory, so every plan that
+// b2s_resamp_plan accepts executes.
 // The (consumed, produced, status) triple follows :92-106 exactly (produced is a multiple of L).
 #include "fir.cuh"
 
@@ -77,6 +79,21 @@ resamp_kernel(const S *__restrict__ in, S *__restrict__ out, const float *__rest
         for (int r = 0; r < kRsR; r++)
             if (r < nr) out[k0 + (long long)r * Sg] = acc[r];
     }
+}
+
+// Plans whose input span does not fit resamp_kernel's tile (large M/L, e.g. 1/100 or 4/125): one thread per output
+// straight from global memory (L1/L2 cached), the same tap order as resamp_kernel.
+template <typename S>
+__global__ void resamp_naive_kernel(const S *__restrict__ in, S *__restrict__ out, const float *__restrict__ banks,
+                                    int L, int M, int T, int pitch, long long n_out) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_out) return;
+    const long long km = k * M;
+    const S *x = in + km / L;
+    const float *g = banks + (km % L) * pitch;
+    S acc = zero_of<S>();
+    for (int t = 0; t < T; t++) mac(acc, x[t], g[t]);
+    out[k] = acc;
 }
 
 }  // namespace
@@ -152,7 +169,17 @@ int32_t b2s_resamp_exec(b2s_resamp *r, const void *d_in, size_t n_in, void *d_ou
     const size_t xs_bytes = round_up((size_t)span_max * isz, 16);
     const bool taps_smem = xs_bytes + taps_bytes <= 160 * 1024;
     const size_t smem = xs_bytes + (taps_smem ? taps_bytes : 0);
-    if (xs_bytes > 200 * 1024) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_resamp_exec: decimation too large for one tile");
+    if (xs_bytes > 200 * 1024) {   // the span does not fit one tile in shared memory
+        const unsigned nb = (unsigned)ceil_div(p, (size_t)kRsThreads);
+        if (r->kind == B2S_F32_F32)
+            resamp_naive_kernel<float><<<nb, kRsThreads, 0, ctx->stream>>>((const float *)d_in, (float *)d_out, r->d_banks,
+                                                                           (int)L, (int)M, (int)T, r->pitch, (long long)p);
+        else
+            resamp_naive_kernel<float2><<<nb, kRsThreads, 0, ctx->stream>>>((const float2 *)d_in, (float2 *)d_out, r->d_banks,
+                                                                             (int)L, (int)M, (int)T, r->pitch, (long long)p);
+        B2S_CHECK_LAUNCH(ctx);
+        return B2S_OK;
+    }
     const unsigned grid = (unsigned)ceil_div(p, tile_out);
 #define RS_LAUNCH(S, TS)                                                                                     \
     do {                                                                                                     \

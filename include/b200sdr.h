@@ -155,7 +155,8 @@ int32_t b2s_fir_filter_host(b2s_fir *f, const void *h_in, size_t n_in, void *h_o
                             size_t *consumed, size_t *produced, int32_t *status);
 
 /* ---- rational polyphase resampler (≙ PolyphaseResamplingFir, polyphase_resampling_fir.rs:42-124)
- * kinds B2S_F32_F32 and B2S_C32_F32 (the only impls, :126-167); ntaps % interp == 0 (:56). */
+ * kinds B2S_F32_F32 and B2S_C32_F32 (the only impls, :126-167); ntaps % interp == 0 (:56).  interp > 4096,
+ * decim > 65536 or ntaps > 2^20 is refused at plan time (B2S_EUNSUPPORTED); every plan that is accepted executes. */
 int32_t b2s_resamp_plan(b2s_ctx *ctx, b2s_kind kind, const float *taps, size_t ntaps, size_t interp,
                         size_t decim, b2s_resamp **out);
 void    b2s_resamp_destroy(b2s_resamp *r);
