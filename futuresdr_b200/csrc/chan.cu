@@ -223,11 +223,18 @@ __global__ void chan_transpose_kernel(const float2 *__restrict__ spec, float2 *_
 // Outputs whose windows still reach into the previous call's history (the first T-1 of a call) take the generic
 // three-kernel path.
 // ---------------------------------------------------------------------------------------------------------------
-// Row stride of the FFT buffers = the padded transform length.  (The exact, odd stride N + N/16 - 1 puts the 512/N
-// transforms a warp works on at distinct bank offsets, but its rows start 8 bytes off a 16-byte boundary, which cost
-// more than the bank conflicts it removes.  Also: at 68 the 64-channel kernel sits at EXACTLY two CTAs per SM,
-// 2 x (2 x 40448 + 64 x 68 x 8 + 1024 reserved) = 233472 bytes; one float2 more per row halves the occupancy.)
-__host__ __device__ constexpr int chan_row_stride(int n) { return n + n / 16; }
+// Row stride of the FFT buffers = the padded transform length fft_geom(..).np.  (The exact, odd stride N + N/16 - 1
+// puts the 512/N transforms a warp works on at distinct bank offsets, but its rows start 8 bytes off a 16-byte
+// boundary, which cost more than the bank conflicts it removes.  Also: at 68 the 64-channel kernel sits at EXACTLY two
+// CTAs per SM, 2 x (2 x 40448 + 64 x 68 x 8 + 1024 reserved) = 233472 bytes; one float2 more per row halves the
+// occupancy.)
+
+// items of one input tile: (OB + TPAD - 1) x N samples, reused as the transposed [OB][N+1] output staging
+constexpr size_t chan_xcap(int log2n, int tpad) {
+    const fftk::FftGeom g = fftk::fft_geom(log2n, 256);
+    const size_t rows = (size_t)(g.fpb + tpad - 1) * g.n, staging = (size_t)g.fpb * (g.n + 1);
+    return rows > staging ? rows : staging;
+}
 
 __device__ __forceinline__ void chan_cp_async16(void *dst_smem, const void *src, bool valid) {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
@@ -243,14 +250,13 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
                                                          const float2 *__restrict__ tw, float2 *__restrict__ out, int base0,
                                                          long long o_first, long long nprod, long long out_stride, int ntiles) {
     using namespace fftk;
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;            // threads per transform
-    constexpr int OB = 256 / TT;                             // output vectors per tile
+    constexpr FftGeom G = fft_geom(LOG2N, 256);
+    constexpr int N = G.n, TT = G.t, NP = G.np;              // TT threads per transform
+    constexpr int OB = G.fpb;                                // output vectors per tile
     constexpr int RUNS = 256 / N;                            // runs of outputs per window
     constexpr int RL = OB / RUNS;                            // outputs per run
     constexpr int ROWS = OB + TPAD - 1;
-    constexpr int NP = chan_row_stride(N);
-    constexpr size_t XCAP = ((size_t)ROWS * N > (size_t)OB * (N + 1)) ? (size_t)ROWS * N : (size_t)OB * (N + 1);
+    constexpr size_t XCAP = chan_xcap(LOG2N, TPAD);
     extern __shared__ __align__(16) unsigned char csm[];
     float2 *Xbuf = reinterpret_cast<float2 *>(csm);          // 2 x [ROWS][N] input tiles (each reused as the transposed staging [OB][N+1])
     float2 *V = Xbuf + 2 * XCAP;                             // [OB][NP]    FFT buffers
@@ -315,9 +321,9 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
         {
             const int ol = tid / TT, t = tid % TT;
             float2 *sm = V + (size_t)ol * NP;
-            fft_passes<LOG2N, TT>([&](int idx) { return sm[pad(idx)]; },
-                                  [&](int idx, float2 v) { X[(size_t)ol * (N + 1) + idx] = make_float2(v.x, -v.y); },
-                                  sm, tw, t, true);
+            fft_passes<LOG2N, TT, Tw::Ahead>([&](int idx) { return sm[pad(idx)]; },
+                                             [&](int idx, float2 v) { X[(size_t)ol * (N + 1) + idx] = make_float2(v.x, -v.y); },
+                                             sm, tw, t, true);
         }
         // (fft_passes ends with a CTA barrier)  ---- D: for each channel the OB outputs are contiguous
         for (int e = tid; e < OB * N; e += 256) {
@@ -329,20 +335,15 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
 }
 
 template <int LOG2N, int TPAD> constexpr size_t chan_fused_smem() {
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;
-    constexpr int OB = 256 / TT;
-    constexpr size_t xcap = ((size_t)(OB + TPAD - 1) * N > (size_t)OB * (N + 1)) ? (size_t)(OB + TPAD - 1) * N : (size_t)OB * (N + 1);
-    return (2 * xcap + (size_t)OB * chan_row_stride(N)) * sizeof(float2);
+    constexpr fftk::FftGeom G = fftk::fft_geom(LOG2N, 256);
+    return (2 * chan_xcap(LOG2N, TPAD) + (size_t)G.fpb * G.np) * sizeof(float2);
 }
 
 static inline bool ntiles_overflow(long long nprod, long long o_first, int ob) { return (nprod - o_first) / ob > 0x7fffff00ll; }
 
 template <int LOG2N, int TPAD>
 int32_t chan_fused_launch(b2s_chan *c, const float2 *in, float2 *out, long long o_first, long long nprod, long long out_stride) {
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;
-    constexpr int OB = 256 / TT;
+    constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = chan_fused_smem<LOG2N, TPAD>();
     auto kern = chan_fused_kernel<LOG2N, TPAD>;
     static PerDeviceOnce optin;
@@ -366,16 +367,8 @@ int32_t chan_fused_launch(b2s_chan *c, const float2 *in, float2 *out, long long 
 template <int TPAD>
 int32_t chan_fused_dispatch(b2s_chan *c, int log2n, const float2 *in, float2 *out, long long o_first, long long nprod,
                             long long out_stride) {
-    switch (log2n) {
-        case 2: return chan_fused_launch<2, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 3: return chan_fused_launch<3, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 4: return chan_fused_launch<4, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 5: return chan_fused_launch<5, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 6: return chan_fused_launch<6, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 7: return chan_fused_launch<7, TPAD>(c, in, out, o_first, nprod, out_stride);
-        case 8: return chan_fused_launch<8, TPAD>(c, in, out, o_first, nprod, out_stride);
-    }
-    return B2S_EAGAIN;
+    return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN,
+                                  [&](auto L) { return chan_fused_launch<L, TPAD>(c, in, out, o_first, nprod, out_stride); });
 }
 
 // TPAD (8 / 16 / 32) the fused kernel would use for this plan, 0 if the plan is outside its shapes

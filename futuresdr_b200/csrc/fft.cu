@@ -11,7 +11,8 @@
 // writes it, both fully coalesced (element j + r*N/R for consecutive j).  HBM traffic is the
 // algorithmic minimum, 8 B in + 8 B out per sample (the reference's WGSL/CubeCL prior art makes
 // one global pass per radix-2 stage, perf/burn/src/bin/fft-wgpu-hack.rs:270-397).
-// fftshift is an index rotation on the first-pass load / last-pass store, normalisation a
+// The passes are fftk::fft_passes (fft_common.cuh); this file supplies their first load and last
+// store.  fftshift is an index rotation on the first-pass load / last-pass store, normalisation a
 // multiply on the store; the inverse transform is conj(FFT(conj(x))) (conjugations are free on
 // load/store).  Twiddles come from a table W_N[k] evaluated in f64 on the host.
 #include <cmath>
@@ -52,113 +53,55 @@ struct FftArgs {
     float norm;
 };
 
-// One Stockham pass of radix R at sub-transform size NS (NS = product of the radices of the
-// earlier passes).  FIRST reads global, LAST writes global, otherwise shared memory `sm`.
-// A middle pass is in place in shared memory: every thread first pulls ALL its butterflies'
-// inputs into registers, the CTA synchronises, then results are scattered.
-template <int N, int R, int NS, bool FIRST, bool LAST, int T>
-__device__ __forceinline__ void fft_pass(const FftArgs &a, const float2 *gin, float2 *gout, float2 *sm, int t,
-                                         bool active) {
-    constexpr int NB = N / R;                      // butterflies per transform
-    constexpr int ITER = (NB + T - 1) / T;
-    static_assert(NB % T == 0 || ITER == 1, "butterflies must tile the threads");
-    float2 v[ITER][R];
-#pragma unroll
-    for (int it = 0; it < ITER; it++) {
-        const int j = t + it * T;
-#pragma unroll
-        for (int r = 0; r < R; r++) {
-            const int idx = j + r * NB;
-            if constexpr (FIRST) {
-                // inverse + shift: buff[k] = i[(k + N/2) % N]   (fft.rs:179-185)
-                const int src = (a.inverse && a.shift) ? ((idx + N / 2) & (N - 1)) : idx;
-                float2 x = (j < NB) ? __ldg(gin + src) : make_float2(0.f, 0.f);
-                if (a.inverse) x.y = -x.y;
-                v[it][r] = x;
-            } else {
-                v[it][r] = (j < NB) ? sm[pad(idx)] : make_float2(0.f, 0.f);
-            }
-        }
-    }
-    if constexpr (!FIRST && !LAST) __syncthreads();
-#pragma unroll
-    for (int it = 0; it < ITER; it++) {
-        const int j = t + it * T;
-        if constexpr (NS > 1) {
-            const int k = j & (NS - 1);
-            constexpr int STEP = N / (NS * R);
-            apply_twiddles<R>(v[it], __ldg(a.tw + k * STEP));
-        }
-        Dft<R>::run(v[it]);
-        const int j0 = (j / NS) * NS * R + (j & (NS - 1));
-#pragma unroll
-        for (int r = 0; r < R; r++) {
-            const int idx = j0 + r * NS;
-            if (j >= NB) continue;
-            if constexpr (LAST) {
-                float2 y = v[it][r];
-                if (a.inverse) y.y = -y.y;
-                if (a.has_norm) { y.x *= a.norm; y.y *= a.norm; }
-                // forward + shift: o[k] = X[(k + N/2) % N]   (fft.rs:196-204)
-                const int dst = (!a.inverse && a.shift) ? ((idx + N / 2) & (N - 1)) : idx;
-                if (active) gout[dst] = y;
-            } else {
-                sm[pad(idx)] = v[it][r];
-            }
-        }
-    }
-    if constexpr (!LAST) __syncthreads();
-}
-
 constexpr int kFftThreads = 256;
 
-// threads per CTA / CTAs per SM the register allocation must allow, per size.  8192: the unconstrained build takes
-// one 256-thread CTA per SM by registers although shared memory admits more -> cap at 128 registers, two CTAs.  16384: one transform fills 139 KiB of shared memory, so one CTA per SM whatever we do -- 512 threads halve
-// the butterflies (and registers) per thread and double the warps that hide latency.
-// (<= 4096: three CTAs per SM -- naming a minimum of 1 lets ptxas take more registers than three CTAs allow.)
-template <int LOG2N> struct FftCfg { static constexpr int THREADS = LOG2N >= 14 ? 512 : 256, MINB = LOG2N >= 14 ? 1 : (LOG2N == 13 ? 2 : 3); };
+// CTA size and CTAs per SM the register allocation must allow, per size.  <= 4096: three 256-thread CTAs per SM --
+// naming a minimum of 1 lets ptxas take more registers than three CTAs allow.  8192: the unconstrained build takes one
+// 256-thread CTA per SM by registers although shared memory admits more -> cap at 128 registers, two CTAs.  16384: one
+// transform = one CTA = one SM (139 KiB of shared memory); 1024 threads run ONE butterfly each per pass at 64 registers
+// and give the SM 32 warps to hide latency with.
+constexpr int fft_cta_threads(int log2n) { return log2n == 14 ? 1024 : kFftThreads; }
+constexpr int fft_min_blocks(int log2n) { return log2n == 14 ? 1 : (log2n == 13 ? 2 : 3); }
 
 template <int LOG2N, int TH, int MINB>
 __global__ void __launch_bounds__(TH, MINB) fft_kernel(const FftArgs a) {
-    constexpr int N = 1 << LOG2N;
-    using PL = Plan<LOG2N>;
-    constexpr int T = (N / 16 < 1) ? 1 : ((N / 16 > TH) ? TH : N / 16);                     // threads per transform
-    constexpr int FPB = TH / T;                                                             // transforms per CTA
-    constexpr int NP = N + N / 16;                                                          // padded length
+    constexpr FftGeom G = fft_geom(LOG2N, TH);
+    constexpr int N = G.n;
     extern __shared__ __align__(16) unsigned char fsm[];
-    const int t = threadIdx.x % T, fl = threadIdx.x / T;
-    const long long f = (long long)blockIdx.x * FPB + fl;
+    const int t = threadIdx.x % G.t, fl = threadIdx.x / G.t;
+    const long long f = (long long)blockIdx.x * G.fpb + fl;
     const bool active = f < a.nfft;
-    float2 *sm = reinterpret_cast<float2 *>(fsm) + (size_t)fl * NP;
+    float2 *sm = reinterpret_cast<float2 *>(fsm) + (size_t)fl * G.np;
     // idle transform slots of the last CTA recompute transform nfft-1 and skip the store
     const long long fc = active ? f : a.nfft - 1;
     const float2 *gin = a.in + fc * N;
     float2 *gout = a.out + fc * N;
-
-    if constexpr (PL::P == 1) {
-        fft_pass<N, PL::R0, 1, true, true, T>(a, gin, gout, sm, t, active);
-    } else if constexpr (PL::P == 2) {
-        fft_pass<N, PL::R0, 1, true, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R1, PL::R0, false, true, T>(a, gin, gout, sm, t, active);
-    } else if constexpr (PL::P == 3) {
-        fft_pass<N, PL::R0, 1, true, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R1, PL::R0, false, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R2, PL::R0 * PL::R1, false, true, T>(a, gin, gout, sm, t, active);
-    } else {
-        fft_pass<N, PL::R0, 1, true, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R1, PL::R0, false, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R2, PL::R0 * PL::R1, false, false, T>(a, gin, gout, sm, t, active);
-        fft_pass<N, PL::R3, PL::R0 * PL::R1 * PL::R2, false, true, T>(a, gin, gout, sm, t, active);
-    }
+    // twiddles from the table after each barrier: fetching them a pass ahead costs registers and spills at 8192/16384.
+    // The last pass stores to global memory and ends the kernel: it runs without barriers.
+    fft_passes<LOG2N, G.t, Tw::Table>(
+        [&](int idx) {
+            // inverse + shift: buff[k] = i[(k + N/2) % N]   (fft.rs:179-185)
+            const int src = (a.inverse && a.shift) ? ((idx + N / 2) & (N - 1)) : idx;
+            float2 x = __ldg(gin + src);
+            if (a.inverse) x.y = -x.y;
+            return x;
+        },
+        [&](int idx, float2 y) {
+            if (a.inverse) y.y = -y.y;
+            if (a.has_norm) { y.x *= a.norm; y.y *= a.norm; }
+            // forward + shift: o[k] = X[(k + N/2) % N]   (fft.rs:196-204)
+            const int dst = (!a.inverse && a.shift) ? ((idx + N / 2) & (N - 1)) : idx;
+            if (active) gout[dst] = y;
+        },
+        sm, a.tw, t, false, false);
 }
 
-template <int LOG2N, int TH, int MINB>
-int32_t launch_fft_cfg(b2s_fft *p, const FftArgs &a, cudaStream_t stream) {
-    constexpr int N = 1 << LOG2N;
-    constexpr int T = (N / 16 < 1) ? 1 : ((N / 16 > TH) ? TH : N / 16);
-    constexpr int FPB = TH / T;
-    constexpr size_t smem = (size_t)FPB * (N + N / 16) * sizeof(float2);
-    auto kern = fft_kernel<LOG2N, TH, MINB>;
+template <int LOG2N>
+int32_t launch_fft(b2s_fft *p, const FftArgs &a, cudaStream_t stream) {
+    constexpr int TH = fft_cta_threads(LOG2N);
+    constexpr FftGeom G = fft_geom(LOG2N, TH);
+    constexpr size_t smem = (size_t)G.fpb * G.np * sizeof(float2);
+    auto kern = fft_kernel<LOG2N, TH, fft_min_blocks(LOG2N)>;
     if (smem > 48 * 1024) {
         static PerDeviceOnce optin;              // per template instantiation, per device
         if (optin.need(p->ctx->device)) {
@@ -166,28 +109,10 @@ int32_t launch_fft_cfg(b2s_fft *p, const FftArgs &a, cudaStream_t stream) {
             optin.done(p->ctx->device);
         }
     }
-    const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)FPB);
+    const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)G.fpb);
     kern<<<grid, TH, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);
     return B2S_OK;
-}
-
-template <int LOG2N>
-int32_t launch_fft(b2s_fft *p, const FftArgs &a, cudaStream_t stream) {
-    if constexpr (LOG2N == 14) {
-        // one transform = one CTA = one SM (139 KiB of shared memory): 1024 threads run ONE butterfly each per pass at
-        // 64 registers (32 B of spills) and give the SM 32 warps to hide latency with; 512 threads (two butterflies,
-        // 128 registers) is the A/B alternative (B2S_FFT16K_THREADS=512)
-        static const int th = [] { const char *e = getenv("B2S_FFT16K_THREADS"); return e ? atoi(e) : 1024; }();
-        if (th == 512) return launch_fft_cfg<14, 512, 1>(p, a, stream);
-        return launch_fft_cfg<14, 1024, 1>(p, a, stream);
-    } else if constexpr (LOG2N == 13) {
-        static const int th = [] { const char *e = getenv("B2S_FFT8K_THREADS"); return e ? atoi(e) : 256; }();
-        if (th == 512) return launch_fft_cfg<13, 512, 2>(p, a, stream);      // A/B: one butterfly per thread and pass
-        return launch_fft_cfg<13, 256, 2>(p, a, stream);
-    } else {
-        return launch_fft_cfg<LOG2N, FftCfg<LOG2N>::THREADS, FftCfg<LOG2N>::MINB>(p, a, stream);
-    }
 }
 
 
@@ -205,22 +130,19 @@ struct BsArgs {
 
 template <int LOG2M>
 __global__ void __launch_bounds__(kFftThreads) bluestein_kernel(const BsArgs a) {
-    constexpr int M = 1 << LOG2M;
-    constexpr int T = (M / 16 < 1) ? 1 : ((M / 16 > kFftThreads) ? kFftThreads : M / 16);
-    constexpr int FPB = kFftThreads / T;
-    constexpr int MP = M + M / 16;
+    constexpr FftGeom G = fft_geom(LOG2M, kFftThreads);
     extern __shared__ __align__(16) unsigned char fsm[];
-    const int t = threadIdx.x % T, fl = threadIdx.x / T;
-    const long long f = (long long)blockIdx.x * FPB + fl;
+    const int t = threadIdx.x % G.t, fl = threadIdx.x / G.t;
+    const long long f = (long long)blockIdx.x * G.fpb + fl;
     const bool active = f < a.nfft;
     const long long fc = active ? f : a.nfft - 1;
-    float2 *sm = reinterpret_cast<float2 *>(fsm) + (size_t)fl * MP;
+    float2 *sm = reinterpret_cast<float2 *>(fsm) + (size_t)fl * G.np;
     const float2 *gin = a.in + fc * a.n;
     float2 *gout = a.out + fc * a.n;
     const int n = a.n, half = n / 2;
     auto st_sm = [&](int idx, float2 v) { sm[pad(idx)] = v; };
     // forward M-point FFT of a[j] = x'[j] * w[j]  (x' = conj / pre-shifted input for the inverse direction)
-    fft_passes<LOG2M, T>(
+    fft_passes<LOG2M, G.t, Tw::Ahead>(
         [&](int idx) {
             if (idx >= n) return make_float2(0.f, 0.f);
             const int src = (a.inverse && a.shift) ? (idx + half) % n : idx;        // fft.rs:179-185
@@ -230,7 +152,7 @@ __global__ void __launch_bounds__(kFftThreads) bluestein_kernel(const BsArgs a) 
         },
         st_sm, sm, a.tw, t, false);
     // inverse M-point FFT of A . Bhat as conj(FFT(conj(.))), then the post-chirp
-    fft_passes<LOG2M, T>(
+    fft_passes<LOG2M, G.t, Tw::Ahead>(
         [&](int idx) {
             const float2 y = cmul(sm[pad(idx)], __ldg(a.bhat + idx));
             return make_float2(y.x, -y.y);
@@ -248,10 +170,8 @@ __global__ void __launch_bounds__(kFftThreads) bluestein_kernel(const BsArgs a) 
 
 template <int LOG2M>
 int32_t launch_bluestein(b2s_fft *p, const BsArgs &a, cudaStream_t stream) {
-    constexpr int M = 1 << LOG2M;
-    constexpr int T = (M / 16 < 1) ? 1 : ((M / 16 > kFftThreads) ? kFftThreads : M / 16);
-    constexpr int FPB = kFftThreads / T;
-    constexpr size_t smem = (size_t)FPB * (M + M / 16) * sizeof(float2);
+    constexpr FftGeom G = fft_geom(LOG2M, kFftThreads);
+    constexpr size_t smem = (size_t)G.fpb * G.np * sizeof(float2);
     auto kern = bluestein_kernel<LOG2M>;
     if (smem > 48 * 1024) {
         static PerDeviceOnce optin;              // per template instantiation, per device
@@ -260,7 +180,7 @@ int32_t launch_bluestein(b2s_fft *p, const BsArgs &a, cudaStream_t stream) {
             optin.done(p->ctx->device);
         }
     }
-    const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)FPB);
+    const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)G.fpb);
     kern<<<grid, kFftThreads, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);
     return B2S_OK;
@@ -426,11 +346,7 @@ int32_t b2s_fft_plan_c32(b2s_ctx *ctx, size_t n, int32_t inverse, int32_t fft_sh
             cudaGetLastError(); b2s_fft_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "fft four-step scratch (%zu items)", (p->bluestein ? 4 : 2) * tw_n);
         }
     }
-    std::vector<float2> tw(big ? 1 : tw_n);
-    for (size_t k = 0; k < tw.size(); k++) {
-        const double ang = -2.0 * PI * (double)k / (double)tw_n;
-        tw[k] = make_float2((float)std::cos(ang), (float)std::sin(ang));
-    }
+    const std::vector<float2> tw = twiddle_table(big ? 1 : tw_n);   // four-step: W_1 = {1}, unused
     cudaError_t e = cudaMalloc((void **)&p->d_tw, tw.size() * sizeof(float2));
     if (e != cudaSuccess) { b2s_fft_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "fft twiddles"); }
     B2S_CUDA(ctx, cudaMemcpyAsync(p->d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
@@ -537,45 +453,14 @@ int32_t b2s_fft_exec(b2s_fft *p, const void *d_in, size_t n_in, void *d_out, siz
         b.in = (const float2 *)d_in; b.out = (float2 *)d_out; b.tw = p->d_tw; b.chirp = p->d_chirp; b.bhat = p->d_bhat;
         b.nfft = (long long)(m / p->n); b.n = (int)p->n;
         b.inverse = p->inverse; b.shift = p->shift; b.has_norm = p->has_norm; b.norm = p->norm;
-        cudaStream_t bs = p->ctx->stream;
-        switch (p->log2m) {
-            case 2: return launch_bluestein<2>(p, b, bs);
-            case 3: return launch_bluestein<3>(p, b, bs);
-            case 4: return launch_bluestein<4>(p, b, bs);
-            case 5: return launch_bluestein<5>(p, b, bs);
-            case 6: return launch_bluestein<6>(p, b, bs);
-            case 7: return launch_bluestein<7>(p, b, bs);
-            case 8: return launch_bluestein<8>(p, b, bs);
-            case 9: return launch_bluestein<9>(p, b, bs);
-            case 10: return launch_bluestein<10>(p, b, bs);
-            case 11: return launch_bluestein<11>(p, b, bs);
-            case 12: return launch_bluestein<12>(p, b, bs);
-            case 13: return launch_bluestein<13>(p, b, bs);
-            case 14: return launch_bluestein<14>(p, b, bs);
-        }
-        return b2s_fail(p->ctx, B2S_EUNSUPPORTED, "b2s_fft_exec: unsupported Bluestein size");
+        const int rc = with_log2n<2, 14>(p->log2m, B2S_EUNSUPPORTED, [&](auto L) { return launch_bluestein<L>(p, b, p->ctx->stream); });
+        return rc == B2S_EUNSUPPORTED ? b2s_fail(p->ctx, rc, "b2s_fft_exec: unsupported Bluestein size") : rc;
     }
     FftArgs a;
     a.in = (const float2 *)d_in; a.out = (float2 *)d_out; a.tw = p->d_tw; a.nfft = (long long)(m / p->n);
     a.inverse = p->inverse; a.shift = p->shift; a.has_norm = p->has_norm; a.norm = p->norm;
-    cudaStream_t s = p->ctx->stream;
-    switch (p->log2n) {
-        case 1: return launch_fft<1>(p, a, s);
-        case 2: return launch_fft<2>(p, a, s);
-        case 3: return launch_fft<3>(p, a, s);
-        case 4: return launch_fft<4>(p, a, s);
-        case 5: return launch_fft<5>(p, a, s);
-        case 6: return launch_fft<6>(p, a, s);
-        case 7: return launch_fft<7>(p, a, s);
-        case 8: return launch_fft<8>(p, a, s);
-        case 9: return launch_fft<9>(p, a, s);
-        case 10: return launch_fft<10>(p, a, s);
-        case 11: return launch_fft<11>(p, a, s);
-        case 12: return launch_fft<12>(p, a, s);
-        case 13: return launch_fft<13>(p, a, s);
-        case 14: return launch_fft<14>(p, a, s);
-    }
-    return b2s_fail(p->ctx, B2S_EUNSUPPORTED, "b2s_fft_exec: unsupported size");
+    const int rc = with_log2n<1, 14>(p->log2n, B2S_EUNSUPPORTED, [&](auto L) { return launch_fft<L>(p, a, p->ctx->stream); });
+    return rc == B2S_EUNSUPPORTED ? b2s_fail(p->ctx, rc, "b2s_fft_exec: unsupported size") : rc;
 }
 
 }  // extern "C"

@@ -1,7 +1,12 @@
-// fft_common.cuh -- in-register radix-2/4/8/16 forward DFTs and the padded shared-memory index
-// shared by fft.cu (Fft block) and fir_fft.cu (overlap-save FIR).
+// fft_common.cuh -- the shared-memory Stockham FFT core of every transform in the library (fft.cu, fir_fft.cu,
+// spectrum.cu, chan.cu, synth.cu): in-register radix-2/4/8/16 forward DFTs, the padded shared-memory index, the
+// batched CTA layout, the pass driver and the host-side twiddle table and size dispatch.
 #pragma once
 #include <cuda_runtime.h>
+
+#include <cmath>
+#include <type_traits>
+#include <vector>
 
 namespace fftk {
 
@@ -62,6 +67,37 @@ template <> struct Dft<16> {
 
 __device__ __forceinline__ int pad(int i) { return i + (i >> 4); }
 
+// Batched layout of 2^log2n-point transforms in a CTA of `cta_threads` threads: t threads per transform (one radix-16
+// butterfly each, at most the whole CTA), fpb transforms per CTA, each in a padded row of np = n + n/16 elements.
+// Kernels and their launchers both take it from here, so the shared-memory size always matches the kernel.
+struct FftGeom {
+    int n, t, fpb, np;
+};
+constexpr FftGeom fft_geom(int log2n, int cta_threads) {
+    const int n = 1 << log2n;
+    const int t = n / 16 < 1 ? 1 : (n / 16 > cta_threads ? cta_threads : n / 16);
+    return FftGeom{n, t, cta_threads / t, n + n / 16};
+}
+
+// W_n[k] = exp(-2 pi i k / n), k in [0, n), evaluated in f64 and rounded to f32
+inline std::vector<float2> twiddle_table(size_t n) {
+    const double PI = 3.14159265358979323846264338327950288;
+    std::vector<float2> tw(n);
+    for (size_t k = 0; k < n; k++) {
+        const double ang = -2.0 * PI * (double)k / (double)n;
+        tw[k] = make_float2((float)std::cos(ang), (float)std::sin(ang));
+    }
+    return tw;
+}
+
+// f(std::integral_constant<int, L>{}) for L = log2n if LO <= log2n <= HI, else `otherwise`: one switch over the sizes a
+// kernel template is instantiated for.
+template <int LO, int HI, typename F>
+int with_log2n(int log2n, int otherwise, F &&f) {
+    if constexpr (LO > HI) return otherwise;
+    else return log2n == LO ? f(std::integral_constant<int, LO>{}) : with_log2n<LO + 1, HI>(log2n, otherwise, f);
+}
+
 
 // v[r] *= w^r for r = 1..R-1, powers built by a log-depth product tree from ONE table load
 // (15 dependent-free complex multiplies instead of 15 scattered 8-byte loads per butterfly: the
@@ -103,22 +139,24 @@ template <> struct Plan<13> { static constexpr int P = 4, R0 = 16, R1 = 8,  R2 =
 template <> struct Plan<14> { static constexpr int P = 4, R0 = 16, R1 = 16, R2 = 8, R3 = 8; };
 
 
-// One Stockham pass: loads through `load`, optional CTA barrier (in-place passes), twiddles, DFT,
-// stores through `store`, CTA barrier.
-// The pass's base twiddle of butterfly j: a table lookup, or (TwPre) a value the caller fetched ahead of time -- with
-// one butterfly per thread the index depends on the thread alone, so a kernel that runs the same plan repeatedly loads
-// it once instead of waiting for a global load after every barrier.
+template <int LOG2N> constexpr int plan_radix(int p) {        // radix of pass p
+    using PL = Plan<LOG2N>;
+    return p == 0 ? PL::R0 : p == 1 ? PL::R1 : p == 2 ? PL::R2 : PL::R3;
+}
+template <int LOG2N> constexpr int plan_ns(int p) {           // sub-transform size before pass p
+    return p == 0 ? 1 : plan_ns<LOG2N>(p - 1) * plan_radix<LOG2N>(p - 1);
+}
+
+// The base twiddle of butterfly j of a pass: loaded from the table after the pass's barrier (TwTable), or held in
+// registers from a fetch before the PREVIOUS pass ran (TwAhead) -- with a fixed number of butterflies per thread the
+// index depends on the thread alone, so the load is in flight across the barrier instead of being waited for right
+// after it.  The held values cost registers, which is why the choice is per kernel (Tw below).
 struct TwTable {
     const float2 *__restrict__ tw;
     template <int N, int R, int NS> __device__ __forceinline__ float2 get(int j, int) const {
         return __ldg(tw + (j & (NS - 1)) * (N / (NS * R)));
     }
 };
-struct TwPre {
-    float2 w;
-    template <int N, int R, int NS> __device__ __forceinline__ float2 get(int, int) const { return w; }
-};
-// Base twiddles of one whole pass (ITER butterflies per thread), fetched before the PREVIOUS pass runs.
 template <int N, int R, int NS, int T> struct TwAhead {
     static constexpr int ITER = (N / R) / T > 0 ? (N / R) / T : 1;
     float2 w[ITER];
@@ -129,10 +167,16 @@ template <int N, int R, int NS, int T> struct TwAhead {
     template <int N_, int R_, int NS_> __device__ __forceinline__ float2 get(int, int it) const { return w[it]; }
 };
 
+// Where passes 1.. of fft_passes take their base twiddles from: Table = TwTable, Ahead = TwAhead.
+enum class Tw { Table, Ahead };
+
+// One Stockham pass: loads through `load`, optional CTA barrier (in-place passes), twiddles, DFT,
+// stores through `store`, optional CTA barrier.
 template <int N, int R, int NS, int T, typename LoadF, typename StoreF, typename TwF>
-__device__ __forceinline__ void ss_pass_tw(LoadF load, StoreF store, TwF twf, int t, bool sync_between) {
+__device__ __forceinline__ void ss_pass_tw(LoadF load, StoreF store, TwF twf, int t, bool sync_between,
+                                           bool sync_after = true) {
     constexpr int NB = N / R, ITER = NB / T;
-    static_assert(NB % T == 0 || NB < T, "butterflies must tile the threads");
+    static_assert(NB % T == 0, "butterflies must tile the threads");
     float2 v[ITER][R];
 #pragma unroll
     for (int it = 0; it < ITER; it++) {
@@ -150,75 +194,61 @@ __device__ __forceinline__ void ss_pass_tw(LoadF load, StoreF store, TwF twf, in
 #pragma unroll
         for (int r = 0; r < R; r++) store(j0 + r * NS, v[it][r]);
     }
-    __syncthreads();
+    if (sync_after) __syncthreads();
 }
 
-template <int N, int R, int NS, int T, typename LoadF, typename StoreF>
-__device__ __forceinline__ void ss_pass(LoadF load, StoreF store, const float2 *__restrict__ tw, int t,
-                                        bool sync_between) {
-    ss_pass_tw<N, R, NS, T>(load, store, TwTable{tw}, t, sync_between);
+template <Tw TW, int LOG2N, int P, int T>
+__device__ __forceinline__ auto pass_twiddles(const float2 *__restrict__ tw, int t) {
+    if constexpr (TW == Tw::Ahead) {
+        TwAhead<1 << LOG2N, plan_radix<LOG2N>(P), plan_ns<LOG2N>(P), T> w;
+        w.fetch(tw, t);
+        return w;
+    } else {
+        return TwTable{tw};
+    }
 }
 
+// Passes P.. of the plan, in place in `sm` except the last, which writes through `last_store`; `w` holds pass P's
+// base twiddles.  With Tw::Ahead the next pass's twiddles are fetched before this pass runs.
+template <int LOG2N, int T, Tw TW, int P, typename StoreF, typename TwF>
+__device__ __forceinline__ void fft_passes_from(StoreF last_store, float2 *sm, const float2 *__restrict__ tw, int t,
+                                                bool sync_last, const TwF &w) {
+    constexpr int N = 1 << LOG2N, R = plan_radix<LOG2N>(P), NS = plan_ns<LOG2N>(P);
+    auto ld_sm = [&](int idx) { return sm[pad(idx)]; };
+    if constexpr (P + 1 == Plan<LOG2N>::P) {
+        ss_pass_tw<N, R, NS, T>(ld_sm, last_store, w, t, sync_last, sync_last);
+    } else {
+        const auto wn = pass_twiddles<TW, LOG2N, P + 1, T>(tw, t);
+        ss_pass_tw<N, R, NS, T>(ld_sm, [&](int idx, float2 v) { sm[pad(idx)] = v; }, w, t, true);
+        fft_passes_from<LOG2N, T, TW, P + 1>(last_store, sm, tw, t, sync_last, wn);
+    }
+}
+
+struct NoHook {
+    __device__ __forceinline__ void operator()() const {}
+};
 
 // Runs a whole LOG2N-point forward FFT as Stockham passes through the padded smem buffer `sm`.
 // Pass 0 reads through `first_load(idx)`, the last pass writes through `last_store(idx, v)`, the
 // passes in between read and write `sm`.  first_reads_smem: pass 0's source is `sm` itself.
-template <int LOG2N, int T, typename LoadF, typename StoreF>
+// sync_last = false drops the barriers of the last pass (between its loads and stores, and after it) -- for a last
+// store that leaves shared memory at the end of the kernel.
+// `after_first` runs right after pass 0: from then on pass 0's source is free (spectrum.cu starts the asynchronous
+// fetch of the next transform's input there).  TW: where passes 1.. take their base twiddles (see TwTable).
+template <int LOG2N, int T, Tw TW, typename LoadF, typename StoreF, typename HookF = NoHook>
 __device__ __forceinline__ void fft_passes(LoadF first_load, StoreF last_store, float2 *sm,
-                                           const float2 *__restrict__ tw, int t, bool first_reads_smem) {
-    constexpr int N = 1 << LOG2N;
-    using PL = Plan<LOG2N>;
-    auto ld_sm = [&](int idx) { return sm[pad(idx)]; };
-    auto st_sm = [&](int idx, float2 v) { sm[pad(idx)] = v; };
-    // every pass's base twiddles are fetched one pass ahead: the load is in flight across the barrier
-    if constexpr (PL::P == 1) {
-        ss_pass<N, PL::R0, 1, T>(first_load, last_store, tw, t, first_reads_smem);
-    } else if constexpr (PL::P == 2) {
-        TwAhead<N, PL::R1, PL::R0, T> w1; w1.fetch(tw, t);
-        ss_pass<N, PL::R0, 1, T>(first_load, st_sm, tw, t, first_reads_smem);
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, last_store, w1, t, true);
-    } else if constexpr (PL::P == 3) {
-        TwAhead<N, PL::R1, PL::R0, T> w1; w1.fetch(tw, t);
-        ss_pass<N, PL::R0, 1, T>(first_load, st_sm, tw, t, first_reads_smem);
-        TwAhead<N, PL::R2, PL::R0 * PL::R1, T> w2; w2.fetch(tw, t);
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, st_sm, w1, t, true);
-        ss_pass_tw<N, PL::R2, PL::R0 * PL::R1, T>(ld_sm, last_store, w2, t, true);
+                                           const float2 *__restrict__ tw, int t, bool first_reads_smem,
+                                           bool sync_last = true, HookF after_first = {}) {
+    constexpr int N = 1 << LOG2N, R0 = Plan<LOG2N>::R0;
+    if constexpr (Plan<LOG2N>::P == 1) {
+        ss_pass_tw<N, R0, 1, T>(first_load, last_store, TwTable{tw}, t, first_reads_smem, sync_last);
+        after_first();
     } else {
-        TwAhead<N, PL::R1, PL::R0, T> w1; w1.fetch(tw, t);
-        ss_pass<N, PL::R0, 1, T>(first_load, st_sm, tw, t, first_reads_smem);
-        TwAhead<N, PL::R2, PL::R0 * PL::R1, T> w2; w2.fetch(tw, t);
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, st_sm, w1, t, true);
-        TwAhead<N, PL::R3, PL::R0 * PL::R1 * PL::R2, T> w3; w3.fetch(tw, t);
-        ss_pass_tw<N, PL::R2, PL::R0 * PL::R1, T>(ld_sm, st_sm, w2, t, true);
-        ss_pass_tw<N, PL::R3, PL::R0 * PL::R1 * PL::R2, T>(ld_sm, last_store, w3, t, true);
-    }
-}
-
-// Same, with a hook that runs right after the first pass (its source buffer is free from then on: the caller
-// starts the asynchronous fetch of the NEXT transform's input there).  Plans with at least two passes (N >= 32).
-template <int LOG2N, int T, typename LoadF, typename HookF, typename StoreF>
-__device__ __forceinline__ void fft_passes_hook(LoadF first_load, HookF after_first, StoreF last_store, float2 *sm,
-                                                const float2 *__restrict__ tw, int t) {
-    constexpr int N = 1 << LOG2N;
-    using PL = Plan<LOG2N>;
-    static_assert(PL::P >= 2, "fft_passes_hook needs a multi-pass plan");
-    auto ld_sm = [&](int idx) { return sm[pad(idx)]; };
-    auto st_sm = [&](int idx, float2 v) { sm[pad(idx)] = v; };
-    TwAhead<N, PL::R1, PL::R0, T> w1; w1.fetch(tw, t);
-    ss_pass<N, PL::R0, 1, T>(first_load, st_sm, tw, t, false);
-    after_first();
-    if constexpr (PL::P == 2) {
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, last_store, w1, t, true);
-    } else if constexpr (PL::P == 3) {
-        TwAhead<N, PL::R2, PL::R0 * PL::R1, T> w2; w2.fetch(tw, t);
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, st_sm, w1, t, true);
-        ss_pass_tw<N, PL::R2, PL::R0 * PL::R1, T>(ld_sm, last_store, w2, t, true);
-    } else {
-        TwAhead<N, PL::R2, PL::R0 * PL::R1, T> w2; w2.fetch(tw, t);
-        ss_pass_tw<N, PL::R1, PL::R0, T>(ld_sm, st_sm, w1, t, true);
-        TwAhead<N, PL::R3, PL::R0 * PL::R1 * PL::R2, T> w3; w3.fetch(tw, t);
-        ss_pass_tw<N, PL::R2, PL::R0 * PL::R1, T>(ld_sm, st_sm, w2, t, true);
-        ss_pass_tw<N, PL::R3, PL::R0 * PL::R1 * PL::R2, T>(ld_sm, last_store, w3, t, true);
+        const auto w1 = pass_twiddles<TW, LOG2N, 1, T>(tw, t);
+        ss_pass_tw<N, R0, 1, T>(first_load, [&](int idx, float2 v) { sm[pad(idx)] = v; }, TwTable{tw}, t,
+                                first_reads_smem);
+        after_first();
+        fft_passes_from<LOG2N, T, TW, 1>(last_store, sm, tw, t, sync_last, w1);
     }
 }
 

@@ -10,7 +10,6 @@
 // 4*N FLOP per sample of the direct form (4096 FLOP/sample at 1024 taps).  Radix-16 Stockham passes from fft_common.cuh; H is computed in f64 on the host.
 // Parity: |err| <~ 1e-6 * rms(y) * sqrt(log2 NF), far inside 1e-5 * ||taps||_1 * max|x|.
 #include <cmath>
-#include <cstdlib>
 
 #include "fft_common.cuh"
 #include "fir.cuh"
@@ -32,48 +31,36 @@ struct FftFirArgs {
     int V;              // valid outputs per block
 };
 
-// MINB = CTAs per SM the register allocation must allow: the unconstrained build takes ONE 256-thread CTA per SM by
-// registers; MINB = 2 caps it at 128 registers for two.
+// __launch_bounds__(256, 2): the unconstrained build takes ONE 256-thread CTA per SM by registers; a minimum of two
+// CTAs per SM caps it at 128 registers.  (A template, with this one instantiation, so that profiles name it
+// fir_fft_kernel<2>.)
 template <int MINB>
 __global__ void __launch_bounds__(kFfThreads, MINB) fir_fft_kernel(const FftFirArgs a) {
-    constexpr int N = kNF, T = kFfThreads;
     extern __shared__ __align__(16) unsigned char ffsm[];
     float2 *sm = reinterpret_cast<float2 *>(ffsm);
     const int t = threadIdx.x;
     const long long s = (long long)blockIdx.x * a.V;
     const float2 *in = a.in + s;
     const long long avail = a.n_in - s;                 // items readable from `in`
+    static_assert(fft_geom(kLog2NF, kFfThreads).t == kFfThreads, "one transform per CTA");
 
-    auto ld_sm = [&](int idx) { return sm[pad(idx)]; };
-    auto st_sm = [&](int idx, float2 v) { sm[pad(idx)] = v; };
-    // one butterfly per thread and pass: the base twiddle of a pass depends on the thread alone, so it is fetched one
-    // pass AHEAD (the load is in flight across the barrier instead of being waited for right after it)
-    static_assert(N / 16 == T, "one radix-16 butterfly per thread");
-    const float2 *tw2p = a.tw + (t & 15) * 16, *tw3p = a.tw + t;
-    float2 w = __ldg(tw2p);
-    // forward: 16 x 16 x 16
-    ss_pass<N, 16, 1, T>([&](int idx) { return idx < avail ? __ldg(in + idx) : make_float2(0.f, 0.f); }, st_sm, a.tw, t, false);
-    TwPre twa{w};
-    w = __ldg(tw3p);
-    ss_pass_tw<N, 16, 16, T>(ld_sm, st_sm, twa, t, true);
-    TwPre twb{w};
-    ss_pass_tw<N, 16, 256, T>(ld_sm, st_sm, twb, t, true);
-    // inverse = conj(FFT(conj(X . H))): spectrum product + conjugation fused into the first load
-    w = __ldg(tw2p);
-    ss_pass<N, 16, 1, T>([&](int idx) {
-        const float2 y = cmul(sm[pad(idx)], __ldg(a.H + idx));
-        return make_float2(y.x, -y.y);
-    }, st_sm, a.tw, t, true);
-    TwPre twc{w};
-    w = __ldg(tw3p);
-    ss_pass_tw<N, 16, 16, T>(ld_sm, st_sm, twc, t, true);
-    const TwPre tw3{w};
+    // forward: global -> sm.  Every pass's base twiddle is fetched one pass ahead (Tw::Ahead).
+    fft_passes<kLog2NF, kFfThreads, Tw::Ahead>([&](int idx) { return idx < avail ? __ldg(in + idx) : make_float2(0.f, 0.f); },
+                                              [&](int idx, float2 v) { sm[pad(idx)] = v; }, sm, a.tw, t, false);
+    // inverse = conj(FFT(conj(X . H))): spectrum product + conjugation fused into the first load, the final
+    // conjugation into the store of the V valid outputs
     const long long room = a.n_out - s;
     float2 *out = a.out + s;
     const int V = a.V;
-    ss_pass_tw<N, 16, 256, T>(ld_sm, [&](int idx, float2 v) {
-        if (idx < V && idx < room) out[idx] = make_float2(v.x, -v.y);
-    }, tw3, t, true);
+    fft_passes<kLog2NF, kFfThreads, Tw::Ahead>(
+        [&](int idx) {
+            const float2 y = cmul(sm[pad(idx)], __ldg(a.H + idx));
+            return make_float2(y.x, -y.y);
+        },
+        [&](int idx, float2 v) {
+            if (idx < V && idx < room) out[idx] = make_float2(v.x, -v.y);
+        },
+        sm, a.tw, t, true);
 }
 
 }  // namespace
@@ -91,13 +78,13 @@ int32_t fir_fft_prepare(b2s_fir *f) {
     const size_t N = f->ntaps;
     const bool ctap = f->kind == B2S_C32_C32;
     const double PI = 3.14159265358979323846264338327950288;
-    std::vector<float2> H(kNF), tw(kNF);
+    std::vector<float2> H(kNF);
+    const std::vector<float2> tw = twiddle_table(kNF);
     // H[f] = (1/NF) sum_t g[t] e^{+2 pi i f t / NF},  g[t] = taps[N-1-t]
     std::vector<double> cs(kNF), sn(kNF);
     for (int k = 0; k < kNF; k++) {
         const double ang = 2.0 * PI * (double)k / (double)kNF;
         cs[k] = std::cos(ang); sn[k] = std::sin(ang);
-        tw[k] = make_float2((float)cs[k], (float)-sn[k]);
     }
     for (int fr = 0; fr < kNF; fr++) {
         double re = 0.0, im = 0.0;
@@ -137,11 +124,8 @@ int32_t fir_fft_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, s
     a.n_in = (long long)n_in; a.n_out = (long long)n_out;
     a.V = kNF - (int)(f->ntaps - 1);
     const unsigned grid = (unsigned)ceil_div(n_out, (size_t)a.V);
-    const size_t smem = (size_t)(kNF + kNF / 16) * sizeof(float2);
-    static const int minb = [] { const char *e = getenv("B2S_FFTFIR_MINB"); const int v = e ? atoi(e) : 2; return v >= 1 && v <= 3 ? v : 2; }();
-    if (minb == 1) fir_fft_kernel<1><<<grid, kFfThreads, smem, stream>>>(a);
-    else if (minb == 3) fir_fft_kernel<3><<<grid, kFfThreads, smem, stream>>>(a);
-    else fir_fft_kernel<2><<<grid, kFfThreads, smem, stream>>>(a);
+    const size_t smem = (size_t)fft_geom(kLog2NF, kFfThreads).np * sizeof(float2);
+    fir_fft_kernel<2><<<grid, kFfThreads, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }

@@ -65,17 +65,15 @@ __device__ __forceinline__ void sp_cp_async16(void *dst_smem, const void *src) {
 // plain loads at the top of every round, which serialized the load and compute phases.)
 template <int LOG2N>
 __global__ void __launch_bounds__(kSpThreads, (LOG2N <= 12 ? 3 : 1)) spectrum_kernel(const SpArgs p) {
-    constexpr int N = 1 << LOG2N;
-    constexpr int T = (N / 16 < 1) ? 1 : ((N / 16 > kSpThreads) ? kSpThreads : N / 16);   // threads per transform
-    constexpr int FPB = kSpThreads / T;
-    constexpr int NP = N + N / 16;
+    constexpr FftGeom G = fft_geom(LOG2N, kSpThreads);
+    constexpr int N = G.n, T = G.t, FPB = G.fpb;
     constexpr int NB = N / T;                                                            // bins per thread
     extern __shared__ __align__(16) unsigned char ssm[];
     const int t = threadIdx.x % T, fl = threadIdx.x / T;
     const int g = blockIdx.x * FPB + fl;
     const bool live = g < p.groups;
-    float2 *sm = reinterpret_cast<float2 *>(ssm) + (size_t)fl * NP;           // padded FFT buffer of this group
-    float2 *raw = reinterpret_cast<float2 *>(ssm) + (size_t)FPB * NP + (size_t)fl * N;   // staging row (next frame)
+    float2 *sm = reinterpret_cast<float2 *>(ssm) + (size_t)fl * G.np;         // padded FFT buffer of this group
+    float2 *raw = reinterpret_cast<float2 *>(ssm) + (size_t)FPB * G.np + (size_t)fl * N;   // staging row (next frame)
     float *sP = reinterpret_cast<float *>(sm);              // |X|^2 of the current frame (aliases the FFT buffer)
     const long long f0 = (long long)(live ? g : p.groups - 1) * p.C;
     const long long nf = live ? min(p.C, p.nframes - f0) : 0;
@@ -92,10 +90,9 @@ __global__ void __launch_bounds__(kSpThreads, (LOG2N <= 12 ? 3 : 1)) spectrum_ke
         const bool act = c < nf;
         asm volatile("cp.async.wait_group 0;" ::: "memory");
         __syncthreads();                                     // raw holds frame c; everyone is done with sP of frame c-1
-        fft_passes_hook<LOG2N, T>([&](int idx) { return raw[idx]; },
-                                  [&]() { if (c + 1 < p.C) fetch(c + 1); },
-                                  [&](int idx, float2 v) { sP[idx] = fmaf(v.x, v.x, v.y * v.y); },   // norm_sqr
-                                  sm, p.tw, t);
+        fft_passes<LOG2N, T, Tw::Ahead>([&](int idx) { return raw[idx]; },
+                                        [&](int idx, float2 v) { sP[idx] = fmaf(v.x, v.x, v.y * v.y); },   // norm_sqr
+                                        sm, p.tw, t, false, true, [&]() { if (c + 1 < p.C) fetch(c + 1); });
         if (act) {
             const long long fs = f0 + c;                     // frame index within the call
             const bool emit = ((p.i0 + fs + 1) % p.history) == 0;
@@ -186,28 +183,28 @@ spectrum_fixup(float *out, const float *__restrict__ carry, const float *__restr
     *reinterpret_cast<float4 *>(out + row * n + b) = v;
 }
 
+constexpr size_t spectrum_smem(int log2n) {           // per transform slot: the padded FFT buffer and the staging row
+    const FftGeom g = fft_geom(log2n, kSpThreads);
+    return (size_t)g.fpb * (g.np + g.n) * sizeof(float2);
+}
+
 template <int LOG2N>
 int32_t launch_spectrum(b2s_spectrum *p, const SpArgs &a, cudaStream_t stream) {
-    constexpr int N = 1 << LOG2N;
-    constexpr int T = (N / 16 < 1) ? 1 : ((N / 16 > kSpThreads) ? kSpThreads : N / 16);
-    constexpr int FPB = kSpThreads / T;
-    constexpr size_t smem = (size_t)FPB * (N + N / 16 + N) * sizeof(float2);
+    constexpr size_t smem = spectrum_smem(LOG2N);
     auto kern = spectrum_kernel<LOG2N>;
     static PerDeviceOnce optin;                  // per template instantiation, per device
     if (smem > 48 * 1024 && optin.need(p->ctx->device)) {
         B2S_CUDA(p->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         optin.done(p->ctx->device);
     }
-    const unsigned grid = (unsigned)ceil_div((size_t)a.groups, (size_t)FPB);
+    const unsigned grid = (unsigned)ceil_div((size_t)a.groups, (size_t)fft_geom(LOG2N, kSpThreads).fpb);
     kern<<<grid, kSpThreads, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);
     return B2S_OK;
 }
 
 template <int LOG2N> int spectrum_resident() {         // CTAs of this instantiation that fit one SM
-    constexpr int N = 1 << LOG2N;
-    constexpr int T = (N / 16 < 1) ? 1 : ((N / 16 > kSpThreads) ? kSpThreads : N / 16);
-    constexpr size_t smem = (size_t)(kSpThreads / T) * (N + N / 16 + N) * sizeof(float2);
+    constexpr size_t smem = spectrum_smem(LOG2N);
     auto kern = spectrum_kernel<LOG2N>;
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     int nb = 1;
@@ -233,12 +230,7 @@ int32_t b2s_spectrum_plan(b2s_ctx *ctx, size_t n, int32_t fft_shift, float decay
     p->ctx = ctx; p->n = n; p->shift = fft_shift != 0; p->decay = decay_factor; p->history = history_size;
     p->log10_k = log10_scale;
     while (((size_t)1 << p->log2n) < n) p->log2n++;
-    std::vector<float2> tw(n);
-    const double PI = 3.14159265358979323846264338327950288;
-    for (size_t k = 0; k < n; k++) {
-        const double ang = -2.0 * PI * (double)k / (double)n;
-        tw[k] = make_float2((float)std::cos(ang), (float)std::sin(ang));
-    }
+    const std::vector<float2> tw = twiddle_table(n);
     if (cudaMalloc((void **)&p->d_tw, n * sizeof(float2)) != cudaSuccess || cudaMalloc((void **)&p->d_avg, n * sizeof(float)) != cudaSuccess) {
         cudaGetLastError(); b2s_spectrum_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "spectrum tables");
     }
@@ -292,20 +284,8 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     NvtxRange nvtx("b2s_spectrum_exec");
     cudaStream_t st = ctx->stream;
     // thread groups: one wave of resident CTAs when the call is long enough, never fewer than 4 frames per group
-    const int T = (int)std::min<size_t>(kSpThreads, N / 16), FPB = kSpThreads / T;
-    if (!p->resident) {
-        switch (p->log2n) {
-            case 5: p->resident = spectrum_resident<5>(); break;
-            case 6: p->resident = spectrum_resident<6>(); break;
-            case 7: p->resident = spectrum_resident<7>(); break;
-            case 8: p->resident = spectrum_resident<8>(); break;
-            case 9: p->resident = spectrum_resident<9>(); break;
-            case 10: p->resident = spectrum_resident<10>(); break;
-            case 11: p->resident = spectrum_resident<11>(); break;
-            case 12: p->resident = spectrum_resident<12>(); break;
-            case 13: p->resident = spectrum_resident<13>(); break;
-        }
-    }
+    const int FPB = fft_geom(p->log2n, kSpThreads).fpb;
+    if (!p->resident) p->resident = with_log2n<5, 13>(p->log2n, 0, [](auto L) { return spectrum_resident<L>(); });
     const size_t resident = (size_t)std::max(1, p->resident);
     const size_t g_target = (size_t)ctx->sm_count * resident * FPB;
     const size_t C = std::max<size_t>(4, ceil_div(frames, g_target));
@@ -335,18 +315,7 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     a.in = (const float2 *)d_in; a.out = (float *)d_out; a.fin = p->d_final; a.tw = p->d_tw;
     a.nframes = (long long)frames; a.C = (long long)C; a.groups = (int)groups; a.shift = p->shift;
     a.history = (int)h; a.i0 = (int)p->i; a.a = 1.0f - p->decay; a.d = p->decay;
-    int32_t rc = B2S_EUNSUPPORTED;
-    switch (p->log2n) {
-        case 5: rc = launch_spectrum<5>(p, a, st); break;
-        case 6: rc = launch_spectrum<6>(p, a, st); break;
-        case 7: rc = launch_spectrum<7>(p, a, st); break;
-        case 8: rc = launch_spectrum<8>(p, a, st); break;
-        case 9: rc = launch_spectrum<9>(p, a, st); break;
-        case 10: rc = launch_spectrum<10>(p, a, st); break;
-        case 11: rc = launch_spectrum<11>(p, a, st); break;
-        case 12: rc = launch_spectrum<12>(p, a, st); break;
-        case 13: rc = launch_spectrum<13>(p, a, st); break;
-    }
+    const int32_t rc = with_log2n<5, 13>(p->log2n, B2S_EUNSUPPORTED, [&](auto L) { return launch_spectrum<L>(p, a, st); });
     if (rc != B2S_OK) return rc == B2S_EUNSUPPORTED ? b2s_fail(ctx, rc, "b2s_spectrum_exec: unsupported size") : rc;
     const double ad = (double)(1.0f - p->decay);
     const size_t c_last = frames - (groups - 1) * C;

@@ -127,11 +127,10 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
                                                           float2 *__restrict__ out, float2 *__restrict__ hist, int T,
                                                           long long k2, int ntiles, int tiles_per_cta) {
     using namespace fftk;
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;            // threads per transform
-    constexpr int OB = 256 / TT;                             // vectors per tile
+    constexpr FftGeom G = fft_geom(LOG2N, 256);
+    constexpr int N = G.n, TT = G.t, NP = G.np;              // TT threads per transform
+    constexpr int OB = G.fpb;                                // vectors per tile
     constexpr int RUNS = 256 / N, RL = OB / RUNS;
-    constexpr int NP = N + N / 16;
     constexpr int XP = OB + 1;                               // odd pitch of the gather staging
     constexpr int WARM = (TPAD - 1 + OB - 1) / OB;           // warm-up tiles that fill TPAD-1 rows of history (1 unless OB < TPAD-1)
     extern __shared__ __align__(16) unsigned char ysm[];
@@ -157,9 +156,9 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
         {
             const int ol = tid / TT, tt = tid % TT;
             float2 *sm = Vf + (size_t)ol * NP;
-            fft_passes<LOG2N, TT>([&](int idx) { const float2 x = Xs[(size_t)idx * XP + ol]; return make_float2(x.x, -x.y); },
-                                  [&](int idx, float2 v) { Sb[(size_t)(TPAD - 1 + ol) * N + idx] = make_float2(v.x, -v.y); },
-                                  sm, tw, tt, false);
+            fft_passes<LOG2N, TT, Tw::Ahead>([&](int idx) { const float2 x = Xs[(size_t)idx * XP + ol]; return make_float2(x.x, -x.y); },
+                                             [&](int idx, float2 v) { Sb[(size_t)(TPAD - 1 + ol) * N + idx] = make_float2(v.x, -v.y); },
+                                             sm, tw, tt, false);
         }
         // (fft_passes ends with a CTA barrier)
         if (t >= t0) {
@@ -213,17 +212,13 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
 }
 
 template <int LOG2N, int TPAD> constexpr size_t synth_fused_smem() {
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;
-    constexpr int OB = 256 / TT;
-    return ((size_t)N * (OB + 1) + (size_t)OB * (N + N / 16) + (size_t)(TPAD - 1 + OB) * N) * sizeof(float2);
+    constexpr fftk::FftGeom G = fftk::fft_geom(LOG2N, 256);
+    return ((size_t)G.n * (G.fpb + 1) + (size_t)G.fpb * G.np + (size_t)(TPAD - 1 + G.fpb) * G.n) * sizeof(float2);
 }
 
 template <int LOG2N, int TPAD>
 int32_t synth_fused_launch(b2s_synth *s, const float2 *in, long long in_stride, float2 *out, long long k2) {
-    constexpr int N = 1 << LOG2N;
-    constexpr int TT = (N / 16 < 1) ? 1 : N / 16;
-    constexpr int OB = 256 / TT;
+    constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = synth_fused_smem<LOG2N, TPAD>();
     auto kern = synth_fused_kernel<LOG2N, TPAD>;
     static PerDeviceOnce optin;
@@ -249,16 +244,7 @@ int32_t synth_fused_launch(b2s_synth *s, const float2 *in, long long in_stride, 
 
 template <int TPAD>
 int32_t synth_fused_dispatch(b2s_synth *s, int log2n, const float2 *in, long long in_stride, float2 *out, long long k2) {
-    switch (log2n) {
-        case 2: return synth_fused_launch<2, TPAD>(s, in, in_stride, out, k2);
-        case 3: return synth_fused_launch<3, TPAD>(s, in, in_stride, out, k2);
-        case 4: return synth_fused_launch<4, TPAD>(s, in, in_stride, out, k2);
-        case 5: return synth_fused_launch<5, TPAD>(s, in, in_stride, out, k2);
-        case 6: return synth_fused_launch<6, TPAD>(s, in, in_stride, out, k2);
-        case 7: return synth_fused_launch<7, TPAD>(s, in, in_stride, out, k2);
-        case 8: return synth_fused_launch<8, TPAD>(s, in, in_stride, out, k2);
-    }
-    return B2S_EAGAIN;
+    return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN, [&](auto L) { return synth_fused_launch<L, TPAD>(s, in, in_stride, out, k2); });
 }
 
 int synth_fused_tpad(const b2s_synth *s) {
@@ -268,7 +254,7 @@ int synth_fused_tpad(const b2s_synth *s) {
     return s->T <= 8 ? 8 : (s->T <= 16 ? 16 : 32);
 }
 
-int synth_fused_ob(int log2n) { const int n = 1 << log2n; return 256 / ((n / 16 < 1) ? 1 : n / 16); }
+int synth_fused_ob(int log2n) { return fftk::fft_geom(log2n, 256).fpb; }
 // vectors at the start of a call that stay on the generic path: the warm-up tiles of the first CTA
 size_t synth_fused_lead(int log2n, int tpad) { const int ob = synth_fused_ob(log2n); return (size_t)((tpad - 1 + ob - 1) / ob) * ob; }
 
