@@ -31,8 +31,9 @@
 //                              into one of two 72 KiB operand stages
 //      warps 0-7  two math warpgroups, 64 output phases (M rows) each: 3 wgmma.m64n128k16 per K-step, only over
 //                 the K-steps whose Toeplitz slice holds a tap for the warpgroup's phases (20 of 24 at 256 taps),
-//                 into one of two sets of 64 FP32 accumulator registers per thread; while tile t's MMAs run, the
-//                 outputs of tile t-1 are stored from the other set straight from the registers.
+//                 into 64 FP32 accumulator registers per thread, stored straight from the registers.  The two
+//                 g_hi products take their A operand from registers (fragments loaded once per kernel), g_lo * x_hi
+//                 from the strip in shared memory.
 #include <cuda_bf16.h>
 
 #include <algorithm>
@@ -59,8 +60,8 @@ constexpr int kMathWarps = kNumMathThreads / 32;
 constexpr int kProdWarp0 = kMathWarps;               // warps 8..15 converters
 constexpr int kTmaWarp = kProdWarp0 + kProdWarps;    // warp 16
 // Registers per thread: __launch_bounds__(640, 1) gives every thread 96 (65536 / 640, in units of 8).  The math
-// warpgroups hold two 64-register accumulator sets plus descriptors and epilogue addresses (the f32 epilogue spills
-// at 168), so they take what the converters (48 suffice) and the loader give back; the CTA's allocation must cover
+// warpgroups hold 64 accumulators, 80 registers of g_hi fragments (4 per K-step) and the epilogue's addresses, so they
+// take what the converters (48 suffice) and the loader give back; the CTA's allocation must cover
 // the sum or setmaxnreg.inc never returns.  kRegsAtLaunch assumes ptxas gives the kernel exactly that count at entry
 // (-Xptxas -v: "Used 96 registers"); a lower entry count would shrink the pool below the budget, so fir_tc_prepare
 // refuses the plan if the built kernel reports any other count.
@@ -70,6 +71,9 @@ static_assert(kNumMathThreads * kMathRegs + kNumProducerThreads * kProdRegs + kN
               kThreadsTC * kRegsAtLaunch, "setmaxnreg budget exceeds the CTA's register allocation");
 constexpr int kAtomsOut = 16;                // N = 128 columns = 16 swizzle atoms of 8 rows
 constexpr int kMaxDK = 3;                    // K <= 384
+// K-steps one math warpgroup issues per tile: its 64 phases start on a multiple of 16 and lead + ntaps <= 128*DK - 127,
+// so its tap columns span at most floor((63 + 128*kMaxDK - 128) / 16) + 1 = 20 slices of 16
+constexpr int kMaxKSteps = (63 + 128 * kMaxDK - 128) / 16 + 1;
 constexpr int kSplitBytesMax = (kAtomsOut + kMaxDK - 1) * 1024 * 2;   // per split: 2 K-chunks x 18 atoms
 constexpr int kStageBytes = 2 * kSplitBytesMax;                       // hi + lo = 72 KiB
 constexpr int kACores = kMaxDK * 16 + 15;    // core matrices of the aliased Toeplitz strip (K/8 + 128/8 - 1)
@@ -111,9 +115,9 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// Predicated global stores, branch-free in PTX: the epilogue runs while wgmma.mma_async writes the other accumulator
-// set, and ptxas serialises every wgmma of a kernel when registers are read on a path it must assume divergent
-// between an mma_async and its wait_group.
+// Predicated global stores, branch-free in PTX: the epilogue needs no branches around its 32 stores, and ptxas
+// serialises every wgmma of a kernel when registers are read on a path it must assume divergent between an mma_async
+// and its wait_group.
 __device__ __forceinline__ void st_global_if(float2 *p, float a, float b, bool pred) {
     asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q st.global.v2.f32 [%0], {%1, %2};\n\t}"
                  ::"l"(p), "f"(a), "f"(b), "r"((int)pred) : "memory");
@@ -145,6 +149,33 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t a_desc, u
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
         : "l"(a_desc), "l"(b_desc), "r"(accumulate)
         : "memory");
+}
+// d[64] (+)= A[registers] * B[smem desc]: the A fragment of m64k16 as in mma.m16n8k16, one 16-row slice per warp
+__device__ __forceinline__ void wgmma_m64n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc,
+                                                 uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+        "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, "
+        "%44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+    return v;
 }
 
 // f32 pair -> packed bf16x2 {lo16 = a, hi16 = b}, round-to-nearest-even (one XU instruction)
@@ -463,31 +494,51 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         const int D = prm.decim, per_blk = 128 / D;
         const uint32_t a_hi = a_base + 1024u * wg, a_lo = a_hi + kABytes;   // row group a = 8*wg + a_local
         // The warpgroup's phases p in [p0, p0 + 63] meet taps only in the Toeplitz columns
-        // kappa in [p0 + lead, p0 + 63 + lead + ntaps - 1]: K-steps j (kappa = 16j .. 16j+15) outside [j0, j1] would
+        // kappa in [p0 + lead, p0 + 63 + lead + ntaps - 1]: K-steps j (kappa = 16j .. 16j+15) outside [j0, j0 + nsteps) would
         // add only zero products and are not issued.  flags bit2 (tuning switch): no MMAs at all.
         const int p0 = 64 * (1 - wg);
-        const int j0 = (p0 + prm.lead) / 16;
-        const int j1 = (prm.flags & 4) ? j0 - 1 : min((p0 + 63 + prm.lead + prm.ntaps - 1) / 16, 8 * DK - 1);
+        const int j0 = p0 / 16;                      // = (p0 + lead) / 16, lead < 16; a multiple of 4
+        const int nsteps = (prm.flags & 4) ? 0 : min((p0 + 63 + prm.lead + prm.ntaps - 1) / 16, 8 * DK - 1) - j0 + 1;
+
+        // g_hi feeds two of the three products of every K-step, so it is held in registers for the whole kernel (RS
+        // wgmma) instead of being read from shared memory by both MMAs of every K-step of every tile.  Fragment i
+        // (K-step j0 + i) of warp wl: rows 16*wl + lane/4 + {0, 8}, K pairs 2*(lane%4) + {0, 8}, i.e. the 32-bit word
+        // at row lane/4, element 2*(lane%4) of the strip's core matrices s, s + 1, s + 1, s + 2 (rows + 8 and K + 8
+        // are the same core matrix of the aliased strip), s = 8*wg + 2*wl + 2*j.  Loaded once; a fragment register is
+        // never written again, so no MMA in flight can see it change.
+        uint32_t ghi[kMaxKSteps][4];
+        {
+            const uint32_t f0 = a_hi + 256u * (uint32_t)(wl + j0) + 16u * (uint32_t)(lane >> 2) + 4u * (uint32_t)q4;
+#pragma unroll
+            for (int i = 0; i < kMaxKSteps; i++) {
+                const uint32_t f = f0 + 256u * i;
+                const bool used = i < nsteps;
+                ghi[i][0] = used ? ld_shared_b32(f) : 0u;
+                ghi[i][1] = used ? ld_shared_b32(f + 128u) : 0u;
+                ghi[i][2] = used ? ld_shared_b32(f + 128u) : 0u;
+                ghi[i][3] = used ? ld_shared_b32(f + 256u) : 0u;
+            }
+        }
+
+        const uint64_t a_lo_desc = make_a_desc(a_lo + 256u * j0);   // K-step j reads core matrices a + 2j, a + 2j + 1
 
         int stage = 0;
         uint32_t phase = 0;
-        // wait for the stage, issue its MMAs into acc and commit them (they run while the caller stores)
+        // wait for the stage, issue its MMAs into acc and commit them
         auto mma_tile = [&](float (&acc)[64]) {
             mbar_wait(full_bar(stage), phase);
             wgmma_fence();                           // earlier register reads of acc precede the async writes
-            const uint32_t sbase = base + stage * kStageBytes;
-#pragma unroll 1
-            for (int j = j0; j <= j1; j++) {
-                const int d = j >> 3, kc = (j >> 2) & 1, ks = j & 3;
-                const int kappa0 = d * 128 + kc * 64 + ks * 16;
-                const uint32_t aoff = (uint32_t)(kappa0 / 8) * 128u;                // core matrix a + j
-                const uint32_t boff = (uint32_t)(kc * chunk_bytes + d * 1024 + ks * 32);
-                const uint64_t bh = make_b_desc(sbase + boff);
-                const uint64_t bl = make_b_desc(sbase + split_bytes + boff);
-                const uint64_t ah = make_a_desc(a_hi + aoff);
-                wgmma_m64n128(acc, ah, bh, j != j0);                         // g_hi * x_hi
-                wgmma_m64n128(acc, ah, bl, 1u);                              // g_hi * x_lo
-                wgmma_m64n128(acc, make_a_desc(a_lo + aoff), bh, 1u);        // g_lo * x_hi
+            // Shared-memory addresses stay below 2^18, so a byte offset moves a descriptor's start field by offset / 16
+            // without a carry: the per-K-step descriptors are the tile's base descriptors plus small offsets.
+            const uint64_t b_desc = make_b_desc(base + stage * kStageBytes);
+#pragma unroll
+            for (int i = 0; i < kMaxKSteps; i++) {   // unrolled: the fragment index must be static
+                if (i >= nsteps) break;
+                const int m = (j0 >> 2) + (i >> 2);  // K-step j = j0 + i: d = m >> 1, kc = m & 1, ks = i & 3
+                const uint64_t bh = b_desc + (uint32_t)(((m & 1) * chunk_bytes + (m >> 1) * 1024 + (i & 3) * 32) >> 4);
+                wgmma_m64n128_rs(acc, ghi[i], bh, i != 0);                                // g_hi * x_hi
+                wgmma_m64n128_rs(acc, ghi[i], bh + (uint32_t)(split_bytes >> 4), 1u);     // g_hi * x_lo
+                wgmma_m64n128(acc, a_lo_desc + 16u * i, bh, 1u);                          // g_lo * x_hi
             }
             wgmma_commit();
         };
@@ -500,7 +551,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         };
         // ---- epilogue: for each (h, gamma) a warp writes 4 runs of 8 consecutive outputs (one per lane%4).  The
         // output of column gamma is kb + gamma * per_blk (+ 16 * per_blk for the second real value); it is written when
-        // its phase is kept and k < n_out, i.e. gamma * per_blk < room.  D is a power of two (D | 128).
+        // its phase is kept and k < n_out, i.e. gamma * per_blk < room, i.e. gamma < ncols.  D is a power of two
+        // (D | 128), and so is per_blk.
         const int log2D = __ffs(D) - 1;
         auto store_tile = [&](const float (&acc)[64], int tile) {
             if (prm.flags & 2) return;                      // tuning switch: skip the global stores
@@ -511,41 +563,33 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
                 const long long kb = ((long long)tile * TILE_BLOCKS + kAtomsOut * q4 * (COMPLEX ? 1 : 2)) * per_blk +
                                      (p >> log2D);
                 const int room = (int)max(min(prm.n_out - kb, (long long)INT_MAX), 0ll) & -keep;
+                const int ncols = (int)(((unsigned)room + (unsigned)per_blk - 1u) >> (7 - log2D));   // ceil(room / per_blk)
+                if constexpr (COMPLEX) {
 #pragma unroll
-                for (int gam = 0; gam < 16; gam++) {
-                    const float v0 = acc[4 * gam + 2 * h], v1 = acc[4 * gam + 2 * h + 1];
-                    const int kg = gam * per_blk;
-                    if constexpr (COMPLEX) {
-                        st_global_if(reinterpret_cast<float2 *>(prm.out) + kb + kg, v0, v1, kg < room);
-                    } else {
-                        const int kg1 = kg + kAtomsOut * per_blk;
-                        st_global_if(prm.out + (kb + kg), v0, kg < room);
-                        st_global_if(prm.out + (kb + kg1), v1, kg1 < room);
-                    }
+                    for (int gam = 0; gam < 16; gam++)
+                        st_global_if(reinterpret_cast<float2 *>(prm.out) + kb + gam * per_blk, acc[4 * gam + 2 * h],
+                                     acc[4 * gam + 2 * h + 1], gam < ncols);
+                } else {
+                    // the two values of column gamma are outputs gamma and gamma + 16 of one run of 32, per_blk apart:
+                    // one address stream, and predicates against constants, keep the epilogue inside the math
+                    // warpgroups' registers next to the g_hi fragments
+#pragma unroll
+                    for (int n = 0; n < 2 * kAtomsOut; n++)
+                        st_global_if(prm.out + (kb + n * per_blk), acc[4 * (n % kAtomsOut) + 2 * h + n / kAtomsOut],
+                                     n < ncols);
                 }
             }
         };
 
-        // Two accumulator sets: tile t's MMAs go to one while tile t-1 is stored from the other.  Unrolled by two so
-        // that every register index is static; at the top of the loop the MMAs of `tile` have completed into acc0.
-        float acc0[64], acc1[64];
+        // One accumulator set: the g_hi fragments take the registers a second set would need, so a tile is stored
+        // after its MMAs completed (the converters keep filling the other operand stage meanwhile).
+        float acc[64];
 #pragma unroll
-        for (int i = 0; i < 64; i++) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
-        int tile = blockIdx.x;
-        if (tile < prm.num_tiles) {
-            mma_tile(acc0);
+        for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+            mma_tile(acc);
             release_stage();
-        }
-        for (; tile < prm.num_tiles; tile += 2 * gridDim.x) {
-            const int next = tile + gridDim.x;
-            if (next >= prm.num_tiles) { store_tile(acc0, tile); break; }
-            mma_tile(acc1);
-            store_tile(acc0, tile);
-            release_stage();
-            if (next + (int)gridDim.x >= prm.num_tiles) { store_tile(acc1, next); break; }
-            mma_tile(acc0);
-            store_tile(acc1, next);
-            release_stage();
+            store_tile(acc, tile);
         }
     }
 }
