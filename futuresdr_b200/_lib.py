@@ -35,6 +35,7 @@ SIGNATURES = {
     "b2s_ctx_stream": (_vp, [_vp]),
     "b2s_ctx_sm_count": (_i32, [_vp]),
     "b2s_ctx_launch_count": (C.c_uint64, [_vp]),
+    "b2s_ctx_bytes_held": (C.c_uint64, [_vp]),
     "b2s_malloc": (_i32, [_vp, _sz, _vpp]),
     "b2s_free": (_i32, [_vp, _vp]),
     "b2s_host_alloc": (_i32, [_vp, _sz, _vpp]),
@@ -167,6 +168,23 @@ def _load() -> C.CDLL:
 
 
 lib = _load()
+
+
+class Handle:
+    """Owner of one C-ABI handle ``self._h``: ``close()`` -- and, failing that, ``__del__`` -- passes it to the class's
+    ``_destroy`` exactly once."""
+    _destroy = None
+
+    def close(self):
+        if getattr(self, "_h", None):
+            type(self)._destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:                                   # (module globals may already be gone at interpreter shutdown)
+            self.close()
+        except Exception:  # noqa: BLE001
+            pass
 
 
 def check(rc: int, ctx=None):

@@ -26,7 +26,7 @@ import numpy as np
 import torch
 
 from . import _lib, firdes
-from ._lib import lib, check
+from ._lib import Handle, lib, check
 from .context import Context, default_context
 from .filters import (ComputationStatus, DecimatingFirFilter, FirFilter, IirFilter, PolyphaseResamplingFir,
                       _FilterBase)
@@ -246,9 +246,10 @@ class SignalWave(enum.IntEnum):
     Square = _lib.WAVE_SQUARE
 
 
-class SignalSource(Block):
+class SignalSource(Block, Handle):
     """blocks::SignalSource (src/blocks/signal_source/mod.rs:29-108): a source without an input port.  Each ``work``
     fills the whole output slice and the block never finishes; the samples are bit-identical to the reference's."""
+    _destroy = lib.b2s_sigsrc_destroy
     in_dtype = None
 
     def __init__(self, wave: SignalWave, frequency: float, sample_rate: float, amplitude: float,
@@ -285,14 +286,6 @@ class SignalSource(Block):
     def work(self, io: WorkIo):
         o = self.output.slice()                                                 # mod.rs:94-104
         self.output.produce(self.generate(o))
-
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_sigsrc_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
 
 class SignalSourceBuilder:
@@ -341,8 +334,9 @@ class FftDirection(enum.Enum):
     Inverse = 1
 
 
-class Fft(Block):
+class Fft(Block, Handle):
     """blocks::Fft (src/blocks/fft.rs:30-221)."""
+    _destroy = lib.b2s_fft_destroy
 
     def __init__(self, len: int, direction: FftDirection = FftDirection.Forward, fft_shift: bool = False,
                  normalize: Optional[float] = None, ctx: Optional[Context] = None):
@@ -400,14 +394,6 @@ class Fft(Block):
         if self.input.finished() and m == (m // self.len) * self.len:           # fft.rs:216-218
             io.finished = True
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_fft_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
-
 
 class ApplyOp(enum.IntEnum):
     """The closures of the reference graphs that exist as device ops (b2s_op)."""
@@ -429,9 +415,10 @@ _APPLY_TYPES = {
 }
 
 
-class Apply(Block):
+class Apply(Block, Handle):
     """blocks::Apply (src/blocks/apply.rs:42-131) for the catalogue of closures in ApplyOp.
     Stateful closures (the FM demodulator's ``last`` sample) keep their state on the device."""
+    _destroy = lib.b2s_apply_destroy
 
     def __init__(self, op: ApplyOp, param: float = 1.0, ctx: Optional[Context] = None):
         self.ctx = ctx or default_context()
@@ -461,17 +448,10 @@ class Apply(Block):
         if self.input.finished() and m == i_len:                                 # apply.rs:126-128
             io.finished = True
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_apply_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
-
-class PfbArbResampler(Block):
+class PfbArbResampler(Block, Handle):
     """blocks::PfbArbResampler (src/blocks/pfb/arb_resampler.rs:72-231)."""
+    _destroy = lib.b2s_pfbarb_destroy
 
     def __init__(self, rate: float, taps, num_filters: int, ctx: Optional[Context] = None):
         taps = np.ascontiguousarray(taps, dtype=np.float32)
@@ -503,18 +483,11 @@ class PfbArbResampler(Block):
     def reset(self):
         check(lib.b2s_pfbarb_reset(self._h), self.ctx.handle)
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_pfbarb_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
-
-class Rotator:
+class Rotator(Handle):
     """futuredsp::Rotator (crates/futuredsp/src/rotator.rs:13-48): mixer / frequency shifter whose
     phase recurrence is replayed bit-for-bit (see csrc/rotator.cu)."""
+    _destroy = lib.b2s_rotator_destroy
 
     def __init__(self, phase_incr: float, ctx: Optional[Context] = None):
         self.ctx = ctx or default_context()
@@ -534,14 +507,6 @@ class Rotator:
 
     def reset(self):
         check(lib.b2s_rotator_reset(self._h), self.ctx.handle)
-
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_rotator_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
 
 class XlatingFir(Block):
@@ -577,9 +542,10 @@ class XlatingFir(Block):
             io.finished = True
 
 
-class PfbSynthesizer(Block):
+class PfbSynthesizer(Block, Handle):
     """blocks::PfbSynthesizer (src/blocks/pfb/synthesizer.rs:32-144): N input streams (one channel-major
     device buffer ``inputs`` [N, n] with per-call read position), one output stream."""
+    _destroy = lib.b2s_synth_destroy
 
     def __init__(self, num_channels: int, taps, ctx: Optional[Context] = None):
         taps = np.ascontiguousarray(taps, dtype=np.float32)
@@ -611,18 +577,11 @@ class PfbSynthesizer(Block):
         if n_in - c.value == 0 and self.inputs_finished:                          # :131-141
             io.finished = True
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_synth_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
-
-class MovingAvg(Block):
+class MovingAvg(Block, Handle):
     """blocks::MovingAvg<WIDTH> (src/blocks/moving_avg.rs:24-116): exponential average per bin over
     consecutive WIDTH-item chunks, one output chunk every ``history_size`` input chunks."""
+    _destroy = lib.b2s_mavg_destroy
     in_dtype = np.float32
     out_dtype = np.float32
 
@@ -646,22 +605,15 @@ class MovingAvg(Block):
         self.input.consume(c.value)
         self.output.produce(p.value)
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_mavg_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
-
-class SpectrumPipe(Block):
+class SpectrumPipe(Block, Handle):
     """The spectrum flowgraph's compute chain as ONE block (SURVEY 8f-3): ``Fft::with_options(n, Forward,
     fft_shift, None)`` -> ``Apply(|x|^2)`` -> ``MovingAvg<n>::new(decay_factor, history_size)`` of
     examples/spectrum/src/bin/cpu.rs:21-28, optionally followed by ``log10_scale * log10(.)`` (what the
     reference's CubeCL kernel fuses, perf/burn/src/bin/fft-cubecl-kernel.rs:115-146).  Complex<f32> in, f32 out;
     only 8 B/sample in and ``n`` floats per ``history_size`` frames out touch HBM.  Values agree with the three
     separate blocks to rounding (blocked-scan evaluation of the average), counts are MovingAvg's."""
+    _destroy = lib.b2s_spectrum_destroy
     in_dtype = np.complex64
     out_dtype = np.float32
 
@@ -694,19 +646,12 @@ class SpectrumPipe(Block):
     def reset(self):
         check(lib.b2s_spectrum_reset(self._h), self.ctx.handle)
 
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_spectrum_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
-
-class PfbChannelizer(Block):
+class PfbChannelizer(Block, Handle):
     """blocks::PfbChannelizer (src/blocks/pfb/channelizer.rs:72-223): one input, N output streams.
     The N output ports share one channel-major device buffer ``outputs`` of shape [N, capacity];
     ``produced`` items have been written to every row."""
+    _destroy = lib.b2s_chan_destroy
 
     def __init__(self, num_channels: int, taps, oversample_rate: float = 1.0, ctx: Optional[Context] = None):
         taps = np.ascontiguousarray(taps, dtype=np.float32)
@@ -743,14 +688,6 @@ class PfbChannelizer(Block):
             io.call_again = True
         elif n_in - c.value < self.decimation_factor and self.input.finished():      # :214-218
             io.finished = True
-
-    def __del__(self):
-        try:                                   # (module globals may already be gone at interpreter shutdown)
-            if getattr(self, "_h", None):
-                lib.b2s_chan_destroy(self._h)
-                self._h = None
-        except Exception:  # noqa: BLE001
-            pass
 
 
 class Mocker:

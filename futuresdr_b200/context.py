@@ -5,16 +5,17 @@ from __future__ import annotations
 import ctypes as C
 
 from . import _lib
-from ._lib import lib, check
+from ._lib import Handle, lib, check
 
 
-class Context:
+class Context(Handle):
     """One CUDA device + the stream all work of this context is ordered on.
 
     With ``stream=None`` and torch importable, the context adopts torch's *current* stream of
     that device, so torch tensors, ``torch.cuda.Event`` timing and NCCL collectives issued by
     ``torch.distributed`` are ordered with our kernels without extra synchronisation.
     """
+    _destroy = lib.b2s_ctx_destroy
 
     def __init__(self, device: int = 0, stream: int | None = None, own_stream: bool = False):
         self.device = int(device)
@@ -47,19 +48,13 @@ class Context:
         return int(lib.b2s_ctx_launch_count(self._h))
 
     @property
+    def bytes_held(self) -> int:
+        """Device + pinned bytes held by the objects created on this context."""
+        return int(lib.b2s_ctx_bytes_held(self._h))
+
+    @property
     def stream(self) -> int:
         return lib.b2s_ctx_stream(self._h) or 0
-
-    def close(self):
-        if getattr(self, "_h", None):
-            lib.b2s_ctx_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 _default: dict[int, Context] = {}

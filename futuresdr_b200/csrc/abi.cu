@@ -52,7 +52,7 @@ static int32_t ctx_create(int device, void *stream, bool own, b2s_ctx **out) {
     B2S_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
     B2S_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
     B2S_CUDA(ctx, cudaMalloc((void **)&ctx->d_status, 256));
-    B2S_CUDA(ctx, cudaMemset(ctx->d_status, 0, 256));
+    B2S_CUDA(ctx, cudaMemsetAsync(ctx->d_status, 0, 256, ctx->stream));
     *out = guard.release();
     return B2S_OK;
 }
@@ -100,6 +100,7 @@ int32_t b2s_ctx_sync(b2s_ctx *ctx) {
 void *b2s_ctx_stream(b2s_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
 int32_t b2s_ctx_sm_count(b2s_ctx *ctx) { return ctx ? ctx->sm_count : 0; }
 uint64_t b2s_ctx_launch_count(const b2s_ctx *ctx) { return ctx ? ctx->launches.load() : 0; }
+uint64_t b2s_ctx_bytes_held(const b2s_ctx *ctx) { return ctx ? ctx->bytes_held.load() : 0; }
 
 int32_t b2s_malloc(b2s_ctx *ctx, size_t bytes, void **dptr) {
     if (!ctx || !dptr) return b2s_fail(ctx, B2S_EINVAL, "b2s_malloc: NULL argument");
@@ -189,15 +190,13 @@ int32_t b2s_fir_plan(b2s_ctx *ctx, b2s_kind kind, const float *taps, size_t ntap
     if (ntaps > (1u << 20) || decim > (1u << 16))
         return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_fir_plan: ntaps/decim too large");
     DeviceGuard g(ctx->device);
-    b2s_fir *f = new b2s_fir();
+    PlanPtr<b2s_fir> f(new b2s_fir());
     f->ctx = ctx; f->kind = kind; f->ntaps = ntaps; f->decim = decim;
     f->taps_host.assign(taps, taps + ntaps * kind_tap_floats(kind));
-    int32_t rc = fir_direct_prepare(f);
-    if (rc != B2S_OK) { b2s_fir_destroy(f); return rc; }
-    resolve_algo(f);
-    rc = prepare_algo(f);
-    if (rc != B2S_OK) { b2s_fir_destroy(f); return rc; }
-    *out = f;
+    B2S_TRY(fir_direct_prepare(f.get()));
+    resolve_algo(f.get());
+    B2S_TRY(prepare_algo(f.get()));
+    *out = f.release();
     return B2S_OK;
 }
 int32_t b2s_fir_plan_f64_f64(b2s_ctx *ctx, const double *taps, size_t ntaps, size_t decim, b2s_fir **out) {
@@ -207,12 +206,11 @@ int32_t b2s_fir_plan_f64_f64(b2s_ctx *ctx, const double *taps, size_t ntaps, siz
     if (decim == 0) return b2s_fail(ctx, B2S_EINVAL, "b2s_fir_plan: decim must be > 0");
     if (ntaps > (1u << 20) || decim > (1u << 16)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_fir_plan: ntaps/decim too large");
     DeviceGuard g(ctx->device);
-    b2s_fir *f = new b2s_fir();
+    PlanPtr<b2s_fir> f(new b2s_fir());
     f->ctx = ctx; f->kind = B2S_F64_F64; f->ntaps = ntaps; f->decim = decim;
     f->algo_req = f->algo = B2S_ALGO_DIRECT;
-    const int32_t rc = fir_f64_prepare(f, taps);
-    if (rc != B2S_OK) { b2s_fir_destroy(f); return rc; }
-    *out = f;
+    B2S_TRY(fir_f64_prepare(f.get(), taps));
+    *out = f.release();
     return B2S_OK;
 }
 int32_t b2s_fir_plan_f32_f32(b2s_ctx *c, const float *t, size_t n, size_t d, b2s_fir **o) {
@@ -225,16 +223,7 @@ int32_t b2s_fir_plan_c32_c32(b2s_ctx *c, const float *t, size_t n, size_t d, b2s
     return b2s_fir_plan(c, B2S_C32_C32, t, n, d, o);
 }
 
-void b2s_fir_destroy(b2s_fir *f) {
-    if (!f) return;
-    DeviceGuard g(f->ctx->device);
-    cudaStreamSynchronize(f->ctx->stream);
-    fir_tc_release(f);
-    fir_fft_release(f);
-    fir_f64_release(f);
-    if (f->d_ptaps) cudaFree(f->d_ptaps);
-    delete f;
-}
+void b2s_fir_destroy(b2s_fir *f) { PlanDeleter<b2s_fir>()(f); }
 
 size_t b2s_fir_length(const b2s_fir *f) { return f ? f->ntaps : 0; }
 

@@ -13,7 +13,7 @@ struct b2s_apply {
     b2s_ctx *ctx = nullptr;
     b2s_op op = B2S_OP_SCALE_F32;
     float param = 1.0f;
-    float2 *d_carry = nullptr;   // closure state (QUAD_DEMOD*: last sample)
+    Buf<float2> d_carry;         // closure state (QUAD_DEMOD*: last sample)
 };
 
 namespace {
@@ -90,7 +90,7 @@ int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
     const int th = 256;
     const size_t want = ceil_div(n, (size_t)th);
     const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * 16);
-    apply_kernel<OP><<<grid, th, 0, ctx->stream>>>(in, out, (long long)n, a->param, a->d_carry);
+    apply_kernel<OP><<<grid, th, 0, ctx->stream>>>(in, out, (long long)n, a->param, a->d_carry.get());
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }
@@ -109,27 +109,21 @@ int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out) 
     *out = nullptr;
     if ((int)op < 0 || (int)op > (int)B2S_OP_LOG10_F32) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
     DeviceGuard g(ctx->device);
-    b2s_apply *a = new b2s_apply();
+    PlanPtr<b2s_apply> a(new b2s_apply());
     a->ctx = ctx; a->op = op; a->param = param;
-    cudaError_t e = cudaMalloc((void **)&a->d_carry, sizeof(float2));
-    if (e != cudaSuccess) { delete a; return b2s_fail(ctx, B2S_ENOMEM, "apply state"); }
-    *out = a;
-    return b2s_apply_reset(a);
+    B2S_TRY(a->d_carry.alloc(ctx, 1, "apply state"));
+    B2S_TRY(b2s_apply_reset(a.get()));
+    *out = a.release();
+    return B2S_OK;
 }
 
-void b2s_apply_destroy(b2s_apply *a) {
-    if (!a) return;
-    DeviceGuard g(a->ctx->device);
-    cudaStreamSynchronize(a->ctx->stream);
-    cudaFree(a->d_carry);
-    delete a;
-}
+void b2s_apply_destroy(b2s_apply *a) { PlanDeleter<b2s_apply>()(a); }
 
 // `let mut last = Complex32::new(0.0, 0.0)` (examples/fm-receiver/src/main.rs:98)
 int32_t b2s_apply_reset(b2s_apply *a) {
     if (!a) return b2s_fail(nullptr, B2S_EINVAL, "apply is NULL");
     DeviceGuard g(a->ctx->device);
-    B2S_CUDA(a->ctx, cudaMemsetAsync(a->d_carry, 0, sizeof(float2), a->ctx->stream));
+    B2S_CUDA(a->ctx, cudaMemsetAsync(a->d_carry.get(), 0, sizeof(float2), a->ctx->stream));
     return B2S_OK;
 }
 
@@ -164,7 +158,7 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
     if (rc != B2S_OK) return rc;
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {
         // last = in[m-1] for the next call (stream-ordered after the kernel that read the old carry)
-        B2S_CUDA(a->ctx, cudaMemcpyAsync(a->d_carry, (const float2 *)d_in + (m - 1), sizeof(float2),
+        B2S_CUDA(a->ctx, cudaMemcpyAsync(a->d_carry.get(), (const float2 *)d_in + (m - 1), sizeof(float2),
                                          cudaMemcpyDeviceToDevice, a->ctx->stream));
     }
     (void)in_is_complex;

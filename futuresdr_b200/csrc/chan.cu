@@ -27,19 +27,18 @@ int b2s_fft_log2n(const b2s_fft *p);
 struct b2s_chan {
     b2s_ctx *ctx = nullptr;
     size_t N = 0, D = 0, T = 0;
-    float *d_arms = nullptr;        // [T][N] (tap-major): d_arms[j*N + i] = arm_i[j] = taps[i + j*N] (utilities.rs:9-19;
+    Buf<float> d_arms;              // [T][N] (tap-major): d_arms[j*N + i] = arm_i[j] = taps[i + j*N] (utilities.rs:9-19;
                                     // newest sample <-> j = 0).  Tap-major so that adjacent windows -- which meet
                                     // adjacent arms -- read adjacent floats (arm-major cost 32 L1 lines per warp load)
-    float2 *d_circ = nullptr;       // [N][2T] circular windows (used while filling)
-    float2 *d_hist = nullptr;       // [N][T] windows in time order once filled
-    int *d_wstate = nullptr;        // [2N]: start_idx[N], missing[N]
+    Buf<float2> d_circ;             // [N][2T] circular windows (used while filling)
+    Buf<float2> d_hist;             // [N][T] windows in time order once filled
+    Buf<int> d_wstate;              // [2N]: start_idx[N], missing[N]
     std::vector<int> start_idx, missing;   // host mirror of the WindowBuffer bookkeeping
     size_t base_index = 0;
     bool all_filled = false;
-    b2s_fft *ifft = nullptr;
-    float2 *d_tmp = nullptr;        // 2 * tmp_items
-    size_t tmp_items = 0;
-    float *d_arms_pad = nullptr;    // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
+    PlanPtr<b2s_fft> ifft;
+    Buf<float2> d_tmp;              // two halves: bank outputs, spectra
+    Buf<float> d_arms_pad;          // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
     int tpad = 0;
 };
 
@@ -358,7 +357,7 @@ int32_t chan_fused_launch(b2s_chan *c, const float2 *in, float2 *out, long long 
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, 256, smem) != cudaSuccess || resident < 1) { cudaGetLastError(); resident = 1; }
     }
     const unsigned grid = (unsigned)std::min<size_t>(ntiles, (size_t)c->ctx->sm_count * resident);
-    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->d_arms_pad, b2s_fft_twiddles(c->ifft), out, (int)c->base_index, o_first,
+    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->d_arms_pad.get(), b2s_fft_twiddles(c->ifft.get()), out, (int)c->base_index, o_first,
                                              nprod, out_stride, (int)ntiles);
     B2S_CHECK_LAUNCH(c->ctx);
     return B2S_OK;
@@ -373,7 +372,7 @@ int32_t chan_fused_dispatch(b2s_chan *c, int log2n, const float2 *in, float2 *ou
 
 // TPAD (8 / 16 / 32) the fused kernel would use for this plan, 0 if the plan is outside its shapes
 int chan_fused_tpad(const b2s_chan *c) {
-    const int l2 = b2s_fft_log2n(c->ifft);
+    const int l2 = b2s_fft_log2n(c->ifft.get());
     if (getenv("B2S_CHAN_NO_FUSED")) return 0;
     if (l2 < 2 || l2 > 8 || c->D != c->N || c->T > 32) return 0;
     return c->T <= 8 ? 8 : (c->T <= 16 ? 16 : 32);
@@ -382,8 +381,6 @@ int chan_fused_tpad(const b2s_chan *c) {
 }  // namespace
 
 extern "C" {
-
-void b2s_chan_destroy(b2s_chan *c);
 
 int32_t b2s_chan_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps, size_t ntaps, float oversample_rate,
                           b2s_chan **out) {
@@ -395,7 +392,7 @@ int32_t b2s_chan_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps, 
     if (oversample_rate == 0.f || std::fmod((float)num_channels, oversample_rate) != 0.f)
         return b2s_fail(ctx, B2S_EINVAL, "pfb_channelizer: oversample rate must be N/i for i in [1, N]");
     DeviceGuard g(ctx->device);
-    b2s_chan *c = new b2s_chan();
+    PlanPtr<b2s_chan> c(new b2s_chan());
     c->ctx = ctx; c->N = num_channels;
     c->D = (size_t)((float)num_channels / oversample_rate);                      // channelizer.rs:106
     const size_t N = c->N, T = (size_t)std::ceil((float)ntaps / (float)N);       // utilities.rs:9
@@ -404,48 +401,29 @@ int32_t b2s_chan_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps, 
     for (size_t i = 0; i < N; i++) { size_t j = 0; for (size_t idx = i; idx < ntaps; idx += N) arms[(j++) * N + i] = taps[idx]; }
     c->start_idx.assign(N, 0); c->missing.assign(N, (int)T);
     c->base_index = N - 1;
-    int32_t rc = b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &c->ifft);              // plan_fft(n, Inverse) (:114)
-    if (rc != B2S_OK) { delete c; return rc; }
-    if (cudaMalloc((void **)&c->d_arms, arms.size() * sizeof(float)) != cudaSuccess ||
-        cudaMalloc((void **)&c->d_circ, N * 2 * T * sizeof(float2)) != cudaSuccess ||
-        cudaMalloc((void **)&c->d_hist, N * T * sizeof(float2)) != cudaSuccess ||
-        cudaMalloc((void **)&c->d_wstate, 2 * N * sizeof(int)) != cudaSuccess) {
-        b2s_chan_destroy(c);
-        return b2s_fail(ctx, B2S_ENOMEM, "channelizer buffers");
-    }
+    b2s_fft *ifft = nullptr;
+    B2S_TRY(b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &ifft));                    // plan_fft(n, Inverse) (:114)
+    c->ifft.reset(ifft);
     std::vector<int> ws(2 * N);
     for (size_t i = 0; i < N; i++) { ws[i] = 0; ws[N + i] = (int)T; }
-    B2S_CUDA(ctx, cudaMemcpyAsync(c->d_arms, arms.data(), arms.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaMemcpyAsync(c->d_wstate, ws.data(), ws.size() * sizeof(int), cudaMemcpyHostToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaMemsetAsync(c->d_circ, 0, N * 2 * T * sizeof(float2), ctx->stream));
-    c->tpad = chan_fused_tpad(c);
+    B2S_TRY(c->d_arms.upload(ctx, arms.data(), arms.size(), "channelizer arms"));
+    B2S_TRY(c->d_circ.alloc(ctx, N * 2 * T, "channelizer windows"));
+    B2S_TRY(c->d_hist.alloc(ctx, N * T, "channelizer history"));
+    B2S_TRY(c->d_wstate.upload(ctx, ws.data(), ws.size(), "channelizer window state"));
+    B2S_CUDA(ctx, cudaMemsetAsync(c->d_circ.get(), 0, N * 2 * T * sizeof(float2), ctx->stream));
+    c->tpad = chan_fused_tpad(c.get());
     std::vector<float> apad;
     if (c->tpad) {
         apad.assign((size_t)c->tpad * N, 0.0f);                                  // taps beyond T are zero (older samples)
         std::copy(arms.begin(), arms.end(), apad.begin());
-        if (cudaMalloc((void **)&c->d_arms_pad, apad.size() * sizeof(float)) != cudaSuccess) {
-            cudaGetLastError(); b2s_chan_destroy(c); return b2s_fail(ctx, B2S_ENOMEM, "channelizer buffers");
-        }
-        B2S_CUDA(ctx, cudaMemcpyAsync(c->d_arms_pad, apad.data(), apad.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        B2S_TRY(c->d_arms_pad.upload(ctx, apad.data(), apad.size(), "channelizer padded arms"));
     }
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = c;
+    *out = c.release();
     return B2S_OK;
 }
 
-void b2s_chan_destroy(b2s_chan *c) {
-    if (!c) return;
-    DeviceGuard g(c->ctx->device);
-    cudaStreamSynchronize(c->ctx->stream);
-    if (c->ifft) b2s_fft_destroy(c->ifft);
-    if (c->d_arms) cudaFree(c->d_arms);
-    if (c->d_circ) cudaFree(c->d_circ);
-    if (c->d_hist) cudaFree(c->d_hist);
-    if (c->d_wstate) cudaFree(c->d_wstate);
-    if (c->d_tmp) cudaFree(c->d_tmp);
-    if (c->d_arms_pad) cudaFree(c->d_arms_pad);
-    delete c;
-}
+void b2s_chan_destroy(b2s_chan *c) { PlanDeleter<b2s_chan>()(c); }
 
 size_t b2s_chan_decimation(const b2s_chan *c) { return c ? c->D : 0; }
 
@@ -473,13 +451,13 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
         }
         if (cnt) {
             if (!d_in) return b2s_fail(ctx, B2S_EINVAL, "b2s_chan_exec: NULL buffer");
-            chan_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, c->d_circ, c->d_wstate, N, T, (int)c->base_index, (int)cnt);
+            chan_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, c->d_circ.get(), c->d_wstate.get(), N, T, (int)c->base_index, (int)cnt);
             B2S_CHECK_LAUNCH(ctx);
         }
         c->base_index = base;
         if (!all_filled()) { *consumed = cnt; return B2S_OK; }               // input exhausted first (:165-170)
         c->all_filled = true;
-        chan_hist_from_circ<<<N, 64, 0, ctx->stream>>>(c->d_circ, c->d_wstate, c->d_hist, N, T);
+        chan_hist_from_circ<<<N, 64, 0, ctx->stream>>>(c->d_circ.get(), c->d_wstate.get(), c->d_hist.get(), N, T);
         B2S_CHECK_LAUNCH(ctx);
         if (n_in >= (size_t)D) *call_again = 1;                                // :176-177; NB nothing is consumed here
         return B2S_OK;
@@ -495,7 +473,7 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     NvtxRange nvtx("b2s_chan_exec");
     if (n_generic < nprod) {
         int32_t rc = B2S_EAGAIN;
-        const int l2 = b2s_fft_log2n(c->ifft);
+        const int l2 = b2s_fft_log2n(c->ifft.get());
         if (c->tpad == 8) rc = chan_fused_dispatch<8>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
         else if (c->tpad == 16) rc = chan_fused_dispatch<16>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
         else if (c->tpad == 32) rc = chan_fused_dispatch<32>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
@@ -504,14 +482,9 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     const size_t nprod_all = nprod;
     nprod = n_generic;
     const size_t items = nprod * N;
-    if (items && c->tmp_items < items) {
-        B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (c->d_tmp) cudaFree(c->d_tmp);
-        c->tmp_items = items * 5 / 4 + 1024;
-        cudaError_t e = cudaMalloc((void **)&c->d_tmp, 2 * c->tmp_items * sizeof(float2));
-        if (e != cudaSuccess) { c->d_tmp = nullptr; c->tmp_items = 0; cudaGetLastError(); return b2s_fail(ctx, B2S_ENOMEM, "channelizer workspace"); }
-    }
-    float2 *bank = c->d_tmp, *spec = c->d_tmp + c->tmp_items;
+    if (items && c->d_tmp.size() < 2 * items)
+        B2S_TRY(c->d_tmp.reserve(ctx, 2 * (items * 5 / 4 + 1024), "channelizer workspace"));
+    float2 *bank = c->d_tmp.get(), *spec = c->d_tmp.get() + c->d_tmp.size() / 2;
     if (items) {
     {
         const int th = (int)std::min<size_t>(128, round_up(N, 32));
@@ -520,12 +493,12 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
         const size_t want_y = std::max<size_t>(1, (size_t)ctx->sm_count * 16 / gx);
         const size_t orun = std::max<size_t>(32, ceil_div(nprod, want_y));
         dim3 grid(gx, (unsigned)ceil_div(nprod, orun));
-        chan_bank_kernel<<<grid, th, 0, ctx->stream>>>(in, c->d_hist, c->d_arms, bank, N, D, T, (int)c->base_index,
+        chan_bank_kernel<<<grid, th, 0, ctx->stream>>>(in, c->d_hist.get(), c->d_arms.get(), bank, N, D, T, (int)c->base_index,
                                                        (long long)nprod, (int)orun);
     }
     B2S_CHECK_LAUNCH(ctx);
     size_t fc = 0, fp = 0;
-    int32_t rc = b2s_fft_exec(c->ifft, bank, items, spec, items, &fc, &fp);
+    int32_t rc = b2s_fft_exec(c->ifft.get(), bank, items, spec, items, &fc, &fp);
     if (rc != B2S_OK) return rc;
     dim3 tg((unsigned)ceil_div(nprod, (size_t)32), (unsigned)ceil_div((size_t)N, (size_t)32));
     chan_transpose_kernel<<<tg, dim3(32, 8), 0, ctx->stream>>>(spec, (float2 *)d_out, N, (long long)nprod, (long long)out_stride);
@@ -533,7 +506,7 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     }
     nprod = nprod_all;
     const long long npush = (long long)nprod * D;
-    chan_hist_update<<<N, 64, T * sizeof(float2), ctx->stream>>>(c->d_hist, in, N, T, (int)c->base_index, npush);
+    chan_hist_update<<<N, 64, T * sizeof(float2), ctx->stream>>>(c->d_hist.get(), in, N, T, (int)c->base_index, npush);
     B2S_CHECK_LAUNCH(ctx);
     c->base_index = (size_t)((((long long)c->base_index - npush) % N + N) % N);
     *consumed = (size_t)npush; *produced_per_channel = nprod;

@@ -9,6 +9,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -34,6 +35,8 @@ struct b2s_ctx {
     // device status word (bit0: a cross-GPU flag wait timed out); checked by b2s_ctx_sync when flag_ops > 0
     unsigned *d_status = nullptr;
     uint64_t flag_ops = 0;
+    // device + pinned bytes held by the Bufs of the objects created on this context (b2s_ctx_bytes_held)
+    std::atomic<uint64_t> bytes_held{0};
 };
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per DEVICE and a process may hold contexts on several: a
@@ -93,6 +96,88 @@ struct DeviceGuard {
         if (prev >= 0) cudaSetDevice(prev);
     }
 };
+
+#define B2S_TRY(expr)                                                                         \
+    do {                                                                                      \
+        const int32_t rc__ = (expr);                                                          \
+        if (rc__ != B2S_OK) return rc__;                                                      \
+    } while (0)
+
+// Ownership: every buffer and sub-plan an object allocates is freed by its owner's destructor.  A Buf owns device
+// (or pinned host) memory and counts it in its context's bytes_held; a plan under construction lives in a PlanPtr
+// until it is handed out through *out, so an early return frees whatever was built so far.
+enum class Mem { Device, Pinned };
+
+template <typename T, Mem M = Mem::Device>
+class Buf {
+  public:
+    Buf() = default;
+    Buf(Buf &&o) noexcept { swap(o); }
+    Buf &operator=(Buf &&o) noexcept {
+        Buf(std::move(o)).swap(*this);
+        return *this;
+    }
+    ~Buf() { reset(); }
+
+    T *get() const { return p_; }
+    size_t size() const { return n_; }   // elements
+    explicit operator bool() const { return p_ != nullptr; }
+
+    void reset() {
+        if (!ctx_) return;
+        if (M == Mem::Device) cudaFree(p_);
+        else cudaFreeHost(p_);
+        ctx_->bytes_held -= n_ * sizeof(T);
+        ctx_ = nullptr; p_ = nullptr; n_ = 0;
+    }
+    // n uninitialised elements in place of what the buffer held
+    int32_t alloc(b2s_ctx *ctx, size_t n, const char *what) {
+        reset();
+        void *p = nullptr;
+        const cudaError_t e = M == Mem::Device ? cudaMalloc(&p, n * sizeof(T))
+                                               : cudaHostAlloc(&p, n * sizeof(T), cudaHostAllocDefault);
+        if (e != cudaSuccess) {
+            cudaGetLastError();   // reported here, not again by the next launch check
+            return b2s_fail(ctx, B2S_ENOMEM, "%s: %zu bytes: %s", what, n * sizeof(T), cudaGetErrorString(e));
+        }
+        ctx_ = ctx; p_ = static_cast<T *>(p); n_ = n;
+        ctx->bytes_held += n * sizeof(T);
+        return B2S_OK;
+    }
+    // alloc, then copy n elements from `host` on the context stream (the caller synchronises before `host` dies)
+    int32_t upload(b2s_ctx *ctx, const T *host, size_t n, const char *what) {
+        B2S_TRY(alloc(ctx, n, what));
+        B2S_CUDA(ctx, cudaMemcpyAsync(p_, host, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+        return B2S_OK;
+    }
+    // grow-on-demand workspace: nothing to do while it holds n elements; otherwise wait until the context stream no
+    // longer uses the old memory and allocate n (the buffer is left empty if that fails)
+    int32_t reserve(b2s_ctx *ctx, size_t n, const char *what) {
+        if (n_ >= n) return B2S_OK;
+        B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        return alloc(ctx, n, what);
+    }
+
+  private:
+    void swap(Buf &o) noexcept {
+        std::swap(ctx_, o.ctx_); std::swap(p_, o.p_); std::swap(n_, o.n_);
+    }
+    b2s_ctx *ctx_ = nullptr;
+    T *p_ = nullptr;
+    size_t n_ = 0;
+};
+
+// Every b2s_*_destroy: wait for the plan's context stream (queued work may still use the plan's memory), then
+// delete the plan on its device.
+template <typename P> struct PlanDeleter {
+    void operator()(P *p) const {
+        if (!p) return;
+        DeviceGuard g(p->ctx->device);
+        cudaStreamSynchronize(p->ctx->stream);
+        delete p;
+    }
+};
+template <typename P> using PlanPtr = std::unique_ptr<P, PlanDeleter<P>>;
 
 // peer.cu: NVTX ranges (visible to nsys / ncu --nvtx) and the cross-GPU flag kernels
 void nvtx_push(const char *name);

@@ -21,25 +21,6 @@
 #include "common.cuh"
 #include "fft_common.cuh"
 
-struct b2s_fft {
-    b2s_ctx *ctx = nullptr;
-    size_t n = 0;
-    int log2n = 0;
-    int inverse = 0, shift = 0, has_norm = 0;
-    float norm = 1.0f;
-    float2 *d_tw = nullptr;     // W_N[k] = exp(-2 pi i k / N), k in [0, N)  (W_M for Bluestein)
-    // Bluestein (chirp-z) path for lengths that are not a power of two
-    bool bluestein = false;
-    int log2m = 0;              // M = 2^log2m >= 2n - 1
-    float2 *d_chirp = nullptr;  // w[k] = exp(-i pi k^2 / n), k in [0, n)
-    float2 *d_bhat = nullptr;   // FFT_M of the wrapped conjugate chirp, pre-divided by M
-    // LARGE transforms (n > 16384, or Bluestein with M > 16384): four-step through HBM on top of two shared-memory plans
-    bool big = false;
-    size_t big_m = 0, big_n1 = 0, big_n2 = 0;     // M = n1 * n2 (M = n for powers of two)
-    b2s_fft *sub1 = nullptr, *sub2 = nullptr;     // forward n1- and n2-point plans (no shift, no scale)
-    float2 *d_work = nullptr;                     // 2 * M (four-step scratch) [+ 2 * M for Bluestein]
-};
-
 namespace {
 
 using namespace fftk;
@@ -281,7 +262,7 @@ __global__ void big_bs_post(const float2 *__restrict__ c, const float2 *__restri
 }
 
 // plan internals for the kernels that embed an N-point transform (chan.cu's fused channelizer)
-const float2 *b2s_fft_twiddles(const b2s_fft *p) { return p ? p->d_tw : nullptr; }
+const float2 *b2s_fft_twiddles(const b2s_fft *p) { return p ? p->d_tw.get() : nullptr; }
 int b2s_fft_log2n(const b2s_fft *p) { return (p && !p->bluestein && !p->big) ? p->log2n : -1; }
 
 // one M-point forward transform src -> dst through the four-step scratch (d_work[0 .. 2M))
@@ -289,18 +270,18 @@ static int32_t big_fft(b2s_fft *p, const float2 *src, float2 *dst, int conj_in, 
                        long long dst_rot, float scale, cudaStream_t st) {
     b2s_ctx *ctx = p->ctx;
     const long long M = (long long)p->big_m, n1 = (long long)p->big_n1, n2 = (long long)p->big_n2;
-    float2 *A = p->d_work, *B = p->d_work + M;
+    float2 *A = p->d_work.get(), *B = p->d_work.get() + M;
     size_t c = 0, q = 0;
     int32_t rc;
     BigT t{};
     t.M = M; t.scale = 1.0f;
     t.src = src; t.dst = A; t.R = n1; t.C = n2; t.conj_in = conj_in; t.src_rot = src_rot;       // x[i1][i2] -> A[i2][i1]
     if ((rc = big_transpose(ctx, t, st))) return rc;
-    if ((rc = b2s_fft_exec(p->sub1, A, (size_t)M, B, (size_t)M, &c, &q))) return rc;               // n2 transforms of length n1
+    if ((rc = b2s_fft_exec(p->sub1.get(), A, (size_t)M, B, (size_t)M, &c, &q))) return rc;               // n2 transforms of length n1
     t = BigT{}; t.M = M; t.scale = 1.0f;
     t.src = B; t.dst = A; t.R = n2; t.C = n1; t.twiddle = 1;                                       // Y[i2][k1] W_M^{i2 k1} -> A[k1][i2]
     if ((rc = big_transpose(ctx, t, st))) return rc;
-    if ((rc = b2s_fft_exec(p->sub2, A, (size_t)M, B, (size_t)M, &c, &q))) return rc;               // n1 transforms of length n2
+    if ((rc = b2s_fft_exec(p->sub2.get(), A, (size_t)M, B, (size_t)M, &c, &q))) return rc;               // n1 transforms of length n2
     t = BigT{}; t.M = M;
     t.src = B; t.dst = dst; t.R = n1; t.C = n2; t.conj_out = conj_out; t.dst_rot = dst_rot; t.scale = scale;   // Z[k1][k2] -> X[k2*n1 + k1]
     return big_transpose(ctx, t, st);
@@ -320,7 +301,7 @@ int32_t b2s_fft_plan_c32(b2s_ctx *ctx, size_t n, int32_t inverse, int32_t fft_sh
     if (pow2 && n > ((size_t)1 << 26)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_fft_plan_c32: n = %zu > 2^26", n);
     if (!pow2 && n > ((size_t)1 << 24)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_fft_plan_c32: non-power-of-two n = %zu > 2^24", n);
     DeviceGuard g(ctx->device);
-    b2s_fft *p = new b2s_fft();
+    PlanPtr<b2s_fft> p(new b2s_fft());
     p->ctx = ctx; p->n = n; p->big = big;
     p->inverse = inverse != 0; p->shift = fft_shift != 0; p->has_norm = has_normalize != 0; p->norm = normalize;
     const double PI = 3.14159265358979323846264338327950288;
@@ -339,17 +320,15 @@ int32_t b2s_fft_plan_c32(b2s_ctx *ctx, size_t n, int32_t inverse, int32_t fft_sh
         while (((size_t)1 << l2) < tw_n) l2++;
         p->big_n1 = (size_t)1 << ((l2 + 1) / 2);
         p->big_n2 = tw_n / p->big_n1;
-        int32_t rc = b2s_fft_plan_c32(ctx, p->big_n1, 0, 0, 0, 1.0f, &p->sub1);
-        if (rc == B2S_OK) rc = b2s_fft_plan_c32(ctx, p->big_n2, 0, 0, 0, 1.0f, &p->sub2);
-        if (rc != B2S_OK) { b2s_fft_destroy(p); return rc; }
-        if (cudaMalloc((void **)&p->d_work, (p->bluestein ? 4 : 2) * tw_n * sizeof(float2)) != cudaSuccess) {
-            cudaGetLastError(); b2s_fft_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "fft four-step scratch (%zu items)", (p->bluestein ? 4 : 2) * tw_n);
-        }
+        b2s_fft *sub = nullptr;
+        B2S_TRY(b2s_fft_plan_c32(ctx, p->big_n1, 0, 0, 0, 1.0f, &sub));
+        p->sub1.reset(sub);
+        B2S_TRY(b2s_fft_plan_c32(ctx, p->big_n2, 0, 0, 0, 1.0f, &sub));
+        p->sub2.reset(sub);
+        B2S_TRY(p->d_work.alloc(ctx, (p->bluestein ? 4 : 2) * tw_n, "fft four-step scratch"));
     }
     const std::vector<float2> tw = twiddle_table(big ? 1 : tw_n);   // four-step: W_1 = {1}, unused
-    cudaError_t e = cudaMalloc((void **)&p->d_tw, tw.size() * sizeof(float2));
-    if (e != cudaSuccess) { b2s_fft_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "fft twiddles"); }
-    B2S_CUDA(ctx, cudaMemcpyAsync(p->d_tw, tw.data(), tw.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+    B2S_TRY(p->d_tw.upload(ctx, tw.data(), tw.size(), "fft twiddles"));
     std::vector<float2> chirp, bhat;
     if (p->bluestein) {
         const size_t M = tw_n;
@@ -380,31 +359,15 @@ int32_t b2s_fft_plan_c32(b2s_ctx *ctx, size_t n, int32_t inverse, int32_t fft_sh
                 }
             }
         for (size_t k = 0; k < M; k++) bhat[k] = make_float2((float)(xr[k] / (double)M), (float)(xi[k] / (double)M));
-        if (cudaMalloc((void **)&p->d_chirp, n * sizeof(float2)) != cudaSuccess ||
-            cudaMalloc((void **)&p->d_bhat, M * sizeof(float2)) != cudaSuccess) {
-            b2s_fft_destroy(p);
-            return b2s_fail(ctx, B2S_ENOMEM, "fft bluestein tables");
-        }
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_chirp, chirp.data(), n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_bhat, bhat.data(), M * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+        B2S_TRY(p->d_chirp.upload(ctx, chirp.data(), n, "fft bluestein chirp"));
+        B2S_TRY(p->d_bhat.upload(ctx, bhat.data(), M, "fft bluestein kernel"));
     }
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = p;
+    *out = p.release();
     return B2S_OK;
 }
 
-void b2s_fft_destroy(b2s_fft *p) {
-    if (!p) return;
-    DeviceGuard g(p->ctx->device);
-    cudaStreamSynchronize(p->ctx->stream);
-    if (p->d_tw) cudaFree(p->d_tw);
-    if (p->d_chirp) cudaFree(p->d_chirp);
-    if (p->d_bhat) cudaFree(p->d_bhat);
-    if (p->d_work) cudaFree(p->d_work);
-    if (p->sub1) b2s_fft_destroy(p->sub1);
-    if (p->sub2) b2s_fft_destroy(p->sub2);
-    delete p;
-}
+void b2s_fft_destroy(b2s_fft *p) { PlanDeleter<b2s_fft>()(p); }
 
 size_t b2s_fft_length(const b2s_fft *p) { return p ? p->n : 0; }
 
@@ -436,28 +399,28 @@ int32_t b2s_fft_exec(b2s_fft *p, const void *d_in, size_t n_in, void *d_out, siz
                 if (rc) return rc;
                 continue;
             }
-            float2 *b0 = p->d_work + 2 * M, *b1 = p->d_work + 3 * M;
-            big_bs_pre<<<gridE, 256, 0, st>>>(in, p->d_chirp, b0, n, M, p->inverse, (p->inverse && p->shift) ? half : 0);
+            float2 *b0 = p->d_work.get() + 2 * M, *b1 = p->d_work.get() + 3 * M;
+            big_bs_pre<<<gridE, 256, 0, st>>>(in, p->d_chirp.get(), b0, n, M, p->inverse, (p->inverse && p->shift) ? half : 0);
             B2S_CHECK_LAUNCH(p->ctx);
             if ((rc = big_fft(p, b0, b1, 0, 0, 0, 0, 1.0f, st))) return rc;
-            big_bs_mul<<<gridE, 256, 0, st>>>(b1, p->d_bhat, M);
+            big_bs_mul<<<gridE, 256, 0, st>>>(b1, p->d_bhat.get(), M);
             B2S_CHECK_LAUNCH(p->ctx);
             if ((rc = big_fft(p, b1, b0, 0, 0, 0, 0, 1.0f, st))) return rc;
-            big_bs_post<<<gridE, 256, 0, st>>>(b0, p->d_chirp, out, n, p->inverse, (!p->inverse && p->shift) ? n - half : 0, scale);
+            big_bs_post<<<gridE, 256, 0, st>>>(b0, p->d_chirp.get(), out, n, p->inverse, (!p->inverse && p->shift) ? n - half : 0, scale);
             B2S_CHECK_LAUNCH(p->ctx);
         }
         return B2S_OK;
     }
     if (p->bluestein) {
         BsArgs b;
-        b.in = (const float2 *)d_in; b.out = (float2 *)d_out; b.tw = p->d_tw; b.chirp = p->d_chirp; b.bhat = p->d_bhat;
+        b.in = (const float2 *)d_in; b.out = (float2 *)d_out; b.tw = p->d_tw.get(); b.chirp = p->d_chirp.get(); b.bhat = p->d_bhat.get();
         b.nfft = (long long)(m / p->n); b.n = (int)p->n;
         b.inverse = p->inverse; b.shift = p->shift; b.has_norm = p->has_norm; b.norm = p->norm;
         const int rc = with_log2n<2, 14>(p->log2m, B2S_EUNSUPPORTED, [&](auto L) { return launch_bluestein<L>(p, b, p->ctx->stream); });
         return rc == B2S_EUNSUPPORTED ? b2s_fail(p->ctx, rc, "b2s_fft_exec: unsupported Bluestein size") : rc;
     }
     FftArgs a;
-    a.in = (const float2 *)d_in; a.out = (float2 *)d_out; a.tw = p->d_tw; a.nfft = (long long)(m / p->n);
+    a.in = (const float2 *)d_in; a.out = (float2 *)d_out; a.tw = p->d_tw.get(); a.nfft = (long long)(m / p->n);
     a.inverse = p->inverse; a.shift = p->shift; a.has_norm = p->has_norm; a.norm = p->norm;
     const int rc = with_log2n<1, 14>(p->log2n, B2S_EUNSUPPORTED, [&](auto L) { return launch_fft<L>(p, a, p->ctx->stream); });
     return rc == B2S_EUNSUPPORTED ? b2s_fail(p->ctx, rc, "b2s_fft_exec: unsupported size") : rc;

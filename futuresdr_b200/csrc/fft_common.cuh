@@ -8,6 +8,28 @@
 #include <type_traits>
 #include <vector>
 
+#include "common.cuh"
+
+// The FFT plan (fft.cu), complete here so that other plans can own one as a sub-plan (PlanPtr<b2s_fft>).
+struct b2s_fft {
+    b2s_ctx *ctx = nullptr;
+    size_t n = 0;
+    int log2n = 0;
+    int inverse = 0, shift = 0, has_norm = 0;
+    float norm = 1.0f;
+    Buf<float2> d_tw;           // W_N[k] = exp(-2 pi i k / N), k in [0, N)  (W_M for Bluestein)
+    // Bluestein (chirp-z) path for lengths that are not a power of two
+    bool bluestein = false;
+    int log2m = 0;              // M = 2^log2m >= 2n - 1
+    Buf<float2> d_chirp;        // w[k] = exp(-i pi k^2 / n), k in [0, n)
+    Buf<float2> d_bhat;         // FFT_M of the wrapped conjugate chirp, pre-divided by M
+    // LARGE transforms (n > 16384, or Bluestein with M > 16384): four-step through HBM on top of two shared-memory plans
+    bool big = false;
+    size_t big_m = 0, big_n1 = 0, big_n2 = 0;     // M = n1 * n2 (M = n for powers of two)
+    PlanPtr<b2s_fft> sub1, sub2;                  // forward n1- and n2-point plans (no shift, no scale)
+    Buf<float2> d_work;                           // 2 * M (four-step scratch) [+ 2 * M for Bluestein]
+};
+
 namespace fftk {
 
 __device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }

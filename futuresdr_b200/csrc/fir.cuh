@@ -11,21 +11,19 @@ struct b2s_fir {
 
     // ---- direct form (fir_direct.cu): per-phase, time-reversed, zero-padded taps in HBM.
     // G[q][u] = g[D*u + q - (D-1)] (u < Upad), then g[t] = taps[N-1-t]   (see DESIGN.md "direct FIR")
-    float *d_ptaps = nullptr;
+    Buf<float> d_ptaps;
     int Upad = 0;
 
     // ---- tensor-core form (fir_tc.cu): split-bf16 Toeplitz blocks, built lazily
-    void *d_toeplitz = nullptr;
     int tc_kblocks = 0;
     bool tc_ready = false;
     int tc_flags = 0;            // bring-up switches (env B2S_TC_FLAGS)
 
-    // ---- FFT overlap-save form (fir_fft.cu): H[NF] then W_NF[NF]
-    float2 *d_fftH = nullptr;
-    bool fft_ready = false;
+    // ---- FFT overlap-save form (fir_fft.cu): H[NF] then W_NF[NF], built lazily
+    Buf<float2> d_fftH;
 
     // ---- f64 x f64 (fir_f64.cu): reversed taps in double precision
-    double *d_taps64 = nullptr;
+    Buf<double> d_taps64;
 };
 
 // fir_direct.cu
@@ -56,14 +54,11 @@ int32_t fir_tc_launch_hist(b2s_fir *f, const FirHist *h, const void *d_in, size_
 int32_t fir_tc_prepare(b2s_fir *f);
 int32_t fir_tc_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out,
                       cudaStream_t stream);
-void    fir_tc_release(b2s_fir *f);
 // fir_f64.cu
 int32_t fir_f64_prepare(b2s_fir *f, const double *taps);
 int32_t fir_f64_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out, cudaStream_t stream);
-void    fir_f64_release(b2s_fir *f);
 // fir_fft.cu
 bool    fir_fft_supported(const b2s_fir *f);
 int32_t fir_fft_prepare(b2s_fir *f);
 int32_t fir_fft_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out,
                        cudaStream_t stream);
-void    fir_fft_release(b2s_fir *f);

@@ -411,14 +411,14 @@ int32_t launch_typed(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, siz
     const SlideLayout lay = slide_layout(1, D, f->Upad, sizeof(S), sizeof(T));
     if (lay.smem > kSmemMax) {
         // the naive kernel reads the plain reversed taps behind the phase table
-        const T *rt = reinterpret_cast<const T *>(f->d_ptaps) + (size_t)D * f->Upad;
+        const T *rt = reinterpret_cast<const T *>(f->d_ptaps.get()) + (size_t)D * f->Upad;
         const int th = 256;
         fir_naive_kernel<S, T><<<(unsigned)ceil_div(n_out, th), th, 0, stream>>>(
             (const S *)d_in, (S *)d_out, rt, (int)f->ntaps, D, (long long)n_out);
         B2S_CHECK_LAUNCH(f->ctx);
         return B2S_OK;
     }
-    return slide_launch<S, T, 1>(f->ctx, reinterpret_cast<const T *>(f->d_ptaps), 1, D, f->Upad, lay, d_in, n_in, d_out,
+    return slide_launch<S, T, 1>(f->ctx, reinterpret_cast<const T *>(f->d_ptaps.get()), 1, D, f->Upad, lay, d_in, n_in, d_out,
                                  n_out, stream);
 }
 
@@ -464,9 +464,7 @@ int32_t fir_direct_prepare(b2s_fir *f) {
     std::vector<float> h = slide_table(f->taps_host.data(), tf, 1, D, N, D - 1);
     for (size_t t = 0; t < N; t++)
         for (size_t c = 0; c < tf; c++) h.push_back(f->taps_host[(N - 1 - t) * tf + c]);
-    B2S_CUDA(ctx, cudaMalloc((void **)&f->d_ptaps, h.size() * sizeof(float)));
-    B2S_CUDA(ctx, cudaMemcpyAsync(f->d_ptaps, h.data(), h.size() * sizeof(float),
-                                  cudaMemcpyHostToDevice, ctx->stream));
+    B2S_TRY(f->d_ptaps.upload(ctx, h.data(), h.size(), "FIR taps"));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // h goes out of scope
     return B2S_OK;
 }

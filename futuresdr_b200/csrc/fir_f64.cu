@@ -32,18 +32,9 @@ int32_t fir_f64_prepare(b2s_fir *f, const double *taps) {
     b2s_ctx *ctx = f->ctx;
     std::vector<double> g(f->ntaps);
     for (size_t t = 0; t < f->ntaps; t++) g[t] = taps[f->ntaps - 1 - t];
-    if (cudaMalloc((void **)&f->d_taps64, f->ntaps * sizeof(double)) != cudaSuccess) {
-        cudaGetLastError();
-        return b2s_fail(ctx, B2S_ENOMEM, "f64 taps");
-    }
-    B2S_CUDA(ctx, cudaMemcpyAsync(f->d_taps64, g.data(), g.size() * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    B2S_TRY(f->d_taps64.upload(ctx, g.data(), g.size(), "f64 taps"));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2S_OK;
-}
-
-void fir_f64_release(b2s_fir *f) {
-    if (f->d_taps64) cudaFree(f->d_taps64);
-    f->d_taps64 = nullptr;
 }
 
 int32_t fir_f64_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out, cudaStream_t stream) {
@@ -53,7 +44,7 @@ int32_t fir_f64_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, s
     const int smem_taps = f->ntaps <= kF64TapsSmem;
     const unsigned grid = (unsigned)std::min<size_t>(ceil_div(n_out, (size_t)kF64Threads), (size_t)ctx->sm_count * 16);
     fir_f64_kernel<<<grid, kF64Threads, smem_taps ? f->ntaps * sizeof(double) : 0, stream>>>(
-        (const double *)d_in, (double *)d_out, f->d_taps64, (int)f->ntaps, (long long)f->decim, (long long)n_out, smem_taps);
+        (const double *)d_in, (double *)d_out, f->d_taps64.get(), (int)f->ntaps, (long long)f->decim, (long long)n_out, smem_taps);
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }

@@ -73,13 +73,12 @@ bool fir_fft_supported(const b2s_fir *f) {
 
 int32_t fir_fft_prepare(b2s_fir *f) {
     b2s_ctx *ctx = f->ctx;
-    if (f->fft_ready) return B2S_OK;
+    if (f->d_fftH) return B2S_OK;
     if (!fir_fft_supported(f)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "FFT FIR: unsupported plan");
     const size_t N = f->ntaps;
     const bool ctap = f->kind == B2S_C32_C32;
     const double PI = 3.14159265358979323846264338327950288;
     std::vector<float2> H(kNF);
-    const std::vector<float2> tw = twiddle_table(kNF);
     // H[f] = (1/NF) sum_t g[t] e^{+2 pi i f t / NF},  g[t] = taps[N-1-t]
     std::vector<double> cs(kNF), sn(kNF);
     for (int k = 0; k < kNF; k++) {
@@ -98,29 +97,22 @@ int32_t fir_fft_prepare(b2s_fir *f) {
         }
         H[fr] = make_float2((float)(re / kNF), (float)(im / kNF));
     }
-    B2S_CUDA(ctx, cudaMalloc((void **)&f->d_fftH, 2 * kNF * sizeof(float2)));
-    B2S_CUDA(ctx, cudaMemcpyAsync(f->d_fftH, H.data(), kNF * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaMemcpyAsync(f->d_fftH + kNF, tw.data(), kNF * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+    const std::vector<float2> tw = twiddle_table(kNF);
+    H.insert(H.end(), tw.begin(), tw.end());
+    B2S_TRY(f->d_fftH.upload(ctx, H.data(), H.size(), "FFT FIR spectrum"));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    f->fft_ready = true;
     return B2S_OK;
-}
-
-void fir_fft_release(b2s_fir *f) {
-    if (f->d_fftH) cudaFree(f->d_fftH);
-    f->d_fftH = nullptr;
-    f->fft_ready = false;
 }
 
 int32_t fir_fft_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out, cudaStream_t stream) {
     b2s_ctx *ctx = f->ctx;
     if (n_out == 0) return B2S_OK;
-    if (!f->fft_ready) return b2s_fail(ctx, B2S_ESTATE, "FFT FIR not prepared");
+    if (!f->d_fftH) return b2s_fail(ctx, B2S_ESTATE, "FFT FIR not prepared");
     if ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) & 7)
         return fir_direct_launch(f, d_in, n_in, d_out, n_out, stream);
     FftFirArgs a;
     a.in = (const float2 *)d_in; a.out = (float2 *)d_out;
-    a.H = f->d_fftH; a.tw = f->d_fftH + kNF;
+    a.H = f->d_fftH.get(); a.tw = f->d_fftH.get() + kNF;
     a.n_in = (long long)n_in; a.n_out = (long long)n_out;
     a.V = kNF - (int)(f->ntaps - 1);
     const unsigned grid = (unsigned)ceil_div(n_out, (size_t)a.V);

@@ -625,8 +625,6 @@ int32_t fir_tc_prepare(b2s_fir *f) {
     return B2S_OK;
 }
 
-void fir_tc_release(b2s_fir *f) { f->tc_ready = false; }
-
 // The tensor kernel moves its input with 16-byte bulk copies.  A slice that starts on an item boundary but not on a
 // 16-byte one (a ring slot's [halo | chunk] with 255 items of history, say) is handled by starting `lead` items
 // early and shifting the Toeplitz operand by `lead` zero taps; a DETACHED history (hist, possibly peer memory) is
@@ -668,7 +666,7 @@ int32_t fir_tc_launch_hist(b2s_fir *f, const FirHist *h, const void *d_in, size_
     prm.pub_value = h ? h->publish_value : 0;
     prm.status = ctx->d_status;
     prm.out = (float *)d_out;
-    prm.g = f->d_ptaps + (size_t)f->decim * f->Upad;      // plain reversed taps (fir_direct_prepare)
+    prm.g = f->d_ptaps.get() + (size_t)f->decim * f->Upad;      // plain reversed taps (fir_direct_prepare)
     prm.n_in = (long long)(lead + n_hist + n_in);
     prm.n_out = (long long)n_out;                        // decimated count
     prm.decim = (int)f->decim;

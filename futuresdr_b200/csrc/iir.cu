@@ -19,7 +19,7 @@
 #include <cmath>
 #include <vector>
 
-#include "common.cuh"
+#include "fir.cuh"
 
 namespace {
 
@@ -299,15 +299,15 @@ struct b2s_iir {
     b2s_algo algo_req = B2S_ALGO_AUTO, algo = B2S_ALGO_DIRECT;
     bool scan_ok = false;                      // plan admitted to the chained scan
     size_t fill = 0;                           // memory items filled so far (data-independent host mirror)
-    void *d_a = nullptr, *d_b = nullptr, *d_mem = nullptr;
-    b2s_fir *fir = nullptr;                    // AUTO with n_a == 0: the FIR plan with taps = b
+    Buf<char> d_a, d_b, d_mem;                 // T = float or double (f64) taps and filter memory
+    PlanPtr<b2s_fir> fir;                      // AUTO with n_a == 0: the FIR plan with taps = b
     // scan state
-    float *d_tables = nullptr;
-    unsigned long long *d_counter = nullptr;
+    Buf<float> d_tables;
+    Buf<unsigned long long> d_counter;
     unsigned long long tiles_launched = 0;
     unsigned seq = 0;
-    unsigned *d_status = nullptr;
-    float *d_agg = nullptr, *d_pre = nullptr;
+    Buf<unsigned> d_status;
+    Buf<float> d_agg, d_pre;
     size_t status_tiles = 0;
 };
 
@@ -350,16 +350,13 @@ int32_t scan_prepare(b2s_iir *f) {
         for (int i = 0; i < dd; i++) h[(n_thr + m) * dd + i] = (float)p[i];
         p = mat_mul(p, AT, d);
     }
-    if (cudaMalloc((void **)&f->d_tables, h.size() * sizeof(float)) != cudaSuccess) {
-        cudaGetLastError();
-        return b2s_fail(ctx, B2S_ENOMEM, "iir scan tables");
-    }
-    B2S_CUDA(ctx, cudaMemcpy(f->d_tables, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice));
-    if (cudaMalloc((void **)&f->d_counter, sizeof(unsigned long long)) != cudaSuccess) {
-        cudaGetLastError();
-        return b2s_fail(ctx, B2S_ENOMEM, "iir scan counter");
-    }
-    B2S_CUDA(ctx, cudaMemset(f->d_counter, 0, sizeof(unsigned long long)));
+    Buf<float> tables;
+    Buf<unsigned long long> counter;
+    B2S_TRY(tables.upload(ctx, h.data(), h.size(), "iir scan tables"));   // pageable h is staged before the call returns
+    B2S_TRY(counter.alloc(ctx, 1, "iir scan counter"));
+    B2S_CUDA(ctx, cudaMemsetAsync(counter.get(), 0, sizeof(unsigned long long), ctx->stream));
+    f->d_tables = std::move(tables);                         // the plan is scan-ready only with both
+    f->d_counter = std::move(counter);
     f->tiles_launched = 0;
     return B2S_OK;
 }
@@ -367,27 +364,23 @@ int32_t scan_prepare(b2s_iir *f) {
 int32_t scan_reserve(b2s_iir *f, size_t tiles) {
     if (tiles <= f->status_tiles) return B2S_OK;
     b2s_ctx *ctx = f->ctx;
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));       // nothing queued may still use the old arrays
-    cudaFree(f->d_status); cudaFree(f->d_agg); cudaFree(f->d_pre);
-    f->d_status = nullptr; f->d_agg = f->d_pre = nullptr; f->status_tiles = 0;
+    f->status_tiles = 0;
     const size_t cap = std::max<size_t>(tiles, 64);
-    if (cudaMalloc((void **)&f->d_status, cap * sizeof(unsigned)) != cudaSuccess ||
-        cudaMalloc((void **)&f->d_agg, cap * f->n_a * sizeof(float)) != cudaSuccess ||
-        cudaMalloc((void **)&f->d_pre, cap * f->n_a * sizeof(float)) != cudaSuccess) {
-        cudaGetLastError();
-        return b2s_fail(ctx, B2S_ENOMEM, "iir scan status (%zu tiles)", cap);
-    }
-    B2S_CUDA(ctx, cudaMemset(f->d_status, 0, cap * sizeof(unsigned)));   // tag 0 never matches a call's sequence
+    B2S_TRY(f->d_status.reserve(ctx, cap, "iir scan status"));
+    B2S_TRY(f->d_agg.reserve(ctx, cap * f->n_a, "iir scan aggregates"));
+    B2S_TRY(f->d_pre.reserve(ctx, cap * f->n_a, "iir scan prefixes"));
+    // tag 0 never matches a call's sequence
+    B2S_CUDA(ctx, cudaMemsetAsync(f->d_status.get(), 0, cap * sizeof(unsigned), ctx->stream));
     f->status_tiles = cap;
     return B2S_OK;
 }
 
 template <int NA>
 void scan_launch_na(b2s_iir *f, const float *in, float *out, long long n, unsigned grid, cudaStream_t st) {
-    ScanTables tab{f->d_tables, f->d_tables + (size_t)(kScanThreads + 1) * NA * NA};
-    iir_scan_kernel<NA><<<grid, kScanThreads, 0, st>>>(in, out, n, (const float *)f->d_a, (const float *)f->d_b,
-                                                       (int)f->n_b, (float *)f->d_mem, tab, f->d_counter,
-                                                       f->tiles_launched, f->d_status, f->d_agg, f->d_pre, f->seq,
+    ScanTables tab{f->d_tables.get(), f->d_tables.get() + (size_t)(kScanThreads + 1) * NA * NA};
+    iir_scan_kernel<NA><<<grid, kScanThreads, 0, st>>>(in, out, n, (const float *)f->d_a.get(), (const float *)f->d_b.get(),
+                                                       (int)f->n_b, (float *)f->d_mem.get(), tab, f->d_counter.get(),
+                                                       f->tiles_launched, f->d_status.get(), f->d_agg.get(), f->d_pre.get(), f->seq,
                                                        f->ctx->d_status);
 }
 
@@ -429,8 +422,8 @@ int32_t seq_launch(b2s_iir *f, const void *d_in, void *d_out, size_t n) {
     }
     const size_t smem = (f->n_b + 2 * f->n_a + kSeqTile + f->n_b - 1 + kSeqTile) * sizeof(T);
     iir_seq_kernel<T><<<1, kSeqThreads, smem, f->ctx->stream>>>((const T *)d_in, (T *)d_out, (long long)n,
-                                                               (const T *)f->d_a, (int)f->n_a, (const T *)f->d_b,
-                                                               (int)f->n_b, (T *)f->d_mem);
+                                                               (const T *)f->d_a.get(), (int)f->n_a, (const T *)f->d_b.get(),
+                                                               (int)f->n_b, (T *)f->d_mem.get());
     B2S_CHECK_LAUNCH(f->ctx);
     return B2S_OK;
 }
@@ -438,7 +431,7 @@ int32_t seq_launch(b2s_iir *f, const void *d_in, void *d_out, size_t n) {
 void resolve_algo(b2s_iir *f) {
     if (f->algo_req == B2S_ALGO_SCAN) f->algo = B2S_ALGO_SCAN;           // set_algo checked admission
     else if (f->algo_req == B2S_ALGO_AUTO && f->scan_ok) f->algo = B2S_ALGO_SCAN;
-    else if (f->algo_req == B2S_ALGO_AUTO && f->fir) f->algo = (b2s_algo)b2s_fir_get_algo(f->fir);
+    else if (f->algo_req == B2S_ALGO_AUTO && f->fir) f->algo = (b2s_algo)b2s_fir_get_algo(f->fir.get());
     else f->algo = B2S_ALGO_DIRECT;
 }
 
@@ -450,29 +443,25 @@ int32_t iir_plan(b2s_ctx *ctx, const T *a_taps, size_t n_a, const T *b_taps, siz
     if (n_a > kSeqMaxTaps || n_b > kSeqMaxTaps)
         return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_iir_plan: at most %zu a taps and %zu b taps", kSeqMaxTaps, kSeqMaxTaps);
     DeviceGuard g(ctx->device);
-    b2s_iir *f = new b2s_iir();
+    PlanPtr<b2s_iir> f(new b2s_iir());
     f->ctx = ctx; f->f64 = f64; f->n_a = n_a; f->n_b = n_b;
     f->a.assign(a_taps, a_taps + n_a);
     f->b.assign(b_taps, b_taps + n_b);
-    auto fail = [&](int32_t rc) { b2s_iir_destroy(f); return rc; };
     const size_t sz = sizeof(T);
-    if (cudaMalloc(&f->d_a, std::max<size_t>(n_a, 1) * sz) != cudaSuccess ||
-        cudaMalloc(&f->d_b, n_b * sz) != cudaSuccess || cudaMalloc(&f->d_mem, std::max<size_t>(n_a, 1) * sz) != cudaSuccess) {
-        cudaGetLastError();
-        return fail(b2s_fail(ctx, B2S_ENOMEM, "iir plan"));
-    }
-    if (n_a && cudaMemcpy(f->d_a, a_taps, n_a * sz, cudaMemcpyHostToDevice) != cudaSuccess)
-        return fail(b2s_fail(ctx, B2S_ECUDA, "iir taps upload"));
-    if (cudaMemcpy(f->d_b, b_taps, n_b * sz, cudaMemcpyHostToDevice) != cudaSuccess)
-        return fail(b2s_fail(ctx, B2S_ECUDA, "iir taps upload"));
-    f->scan_ok = scan_admits(f);
+    B2S_TRY(f->d_a.alloc(ctx, std::max<size_t>(n_a, 1) * sz, "iir a taps"));
+    B2S_TRY(f->d_b.upload(ctx, (const char *)b_taps, n_b * sz, "iir b taps"));
+    B2S_TRY(f->d_mem.alloc(ctx, std::max<size_t>(n_a, 1) * sz, "iir memory"));
+    if (n_a) B2S_CUDA(ctx, cudaMemcpyAsync(f->d_a.get(), a_taps, n_a * sz, cudaMemcpyHostToDevice, ctx->stream));
+    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    f->scan_ok = scan_admits(f.get());
     if (n_a == 0) {
-        int32_t rc = f64 ? b2s_fir_plan_f64_f64(ctx, (const double *)(const void *)b_taps, n_b, 1, &f->fir)
-                         : b2s_fir_plan_f32_f32(ctx, (const float *)(const void *)b_taps, n_b, 1, &f->fir);
-        if (rc != B2S_OK) return fail(rc);
+        b2s_fir *fir = nullptr;
+        B2S_TRY(f64 ? b2s_fir_plan_f64_f64(ctx, (const double *)(const void *)b_taps, n_b, 1, &fir)
+                    : b2s_fir_plan_f32_f32(ctx, (const float *)(const void *)b_taps, n_b, 1, &fir));
+        f->fir.reset(fir);
     }
-    resolve_algo(f);
-    *out = f;
+    resolve_algo(f.get());
+    *out = f.release();
     return B2S_OK;
 }
 
@@ -508,16 +497,7 @@ int32_t b2s_iir_plan_f64(b2s_ctx *ctx, const double *a_taps, size_t n_a, const d
     return iir_plan<double>(ctx, a_taps, n_a, b_taps, n_b, true, out);
 }
 
-void b2s_iir_destroy(b2s_iir *f) {
-    if (!f) return;
-    DeviceGuard g(f->ctx->device);
-    cudaStreamSynchronize(f->ctx->stream);
-    if (f->fir) b2s_fir_destroy(f->fir);
-    cudaFree(f->d_a); cudaFree(f->d_b); cudaFree(f->d_mem);
-    cudaFree(f->d_tables); cudaFree(f->d_counter);
-    cudaFree(f->d_status); cudaFree(f->d_agg); cudaFree(f->d_pre);
-    delete f;
-}
+void b2s_iir_destroy(b2s_iir *f) { PlanDeleter<b2s_iir>()(f); }
 
 size_t b2s_iir_length(const b2s_iir *f) { return f ? f->n_b : 0; }
 
@@ -557,12 +537,12 @@ int32_t b2s_iir_exec(b2s_iir *f, const void *d_in, size_t n_in, void *d_out, siz
     NvtxRange nvtx("b2s_iir_exec");
     cudaStream_t st = f->ctx->stream;
     if (fill_n)                                                              // memory[j] = x[j] (:116)
-        B2S_CUDA(f->ctx, cudaMemcpyAsync((char *)f->d_mem + fill_from * isz, (const char *)d_in + fill_from * isz,
+        B2S_CUDA(f->ctx, cudaMemcpyAsync(f->d_mem.get() + fill_from * isz, (const char *)d_in + fill_from * isz,
                                          fill_n * isz, cudaMemcpyDeviceToDevice, st));
     if (n == 0) return B2S_OK;
     if (f->fir && f->algo_req == B2S_ALGO_AUTO) {                            // n_a == 0: the same sum on the FIR plan
         size_t c = 0, p = 0; int32_t s = 0;
-        return b2s_fir_exec(f->fir, d_in, n_in, d_out, n, &c, &p, &s);
+        return b2s_fir_exec(f->fir.get(), d_in, n_in, d_out, n, &c, &p, &s);
     }
     if (f->algo == B2S_ALGO_SCAN) return scan_launch(f, d_in, d_out, n);
     return f->f64 ? seq_launch<double>(f, d_in, d_out, n) : seq_launch<float>(f, d_in, d_out, n);

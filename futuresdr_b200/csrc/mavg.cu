@@ -16,7 +16,7 @@ struct b2s_mavg {
     b2s_ctx *ctx = nullptr;
     size_t width = 0, history = 1;
     float decay = 0.1f;
-    float *d_avg = nullptr;
+    Buf<float> d_avg;
     size_t i = 0;                 // chunks since the last emission (host mirror; data-independent)
 };
 
@@ -115,21 +115,15 @@ int32_t b2s_mavg_create(b2s_ctx *ctx, size_t width, float decay_factor, size_t h
     if (!(decay_factor >= 0.0f && decay_factor <= 1.0f))                        // moving_avg.rs:58-61
         return b2s_fail(ctx, B2S_EINVAL, "decay_factor must be in [0, 1]");
     DeviceGuard g(ctx->device);
-    b2s_mavg *m = new b2s_mavg();
+    PlanPtr<b2s_mavg> m(new b2s_mavg());
     m->ctx = ctx; m->width = width; m->history = history_size; m->decay = decay_factor;
-    if (cudaMalloc((void **)&m->d_avg, width * sizeof(float)) != cudaSuccess) { delete m; return b2s_fail(ctx, B2S_ENOMEM, "mavg state"); }
-    B2S_CUDA(ctx, cudaMemsetAsync(m->d_avg, 0, width * sizeof(float), ctx->stream));
-    *out = m;
+    B2S_TRY(m->d_avg.alloc(ctx, width, "mavg state"));
+    B2S_CUDA(ctx, cudaMemsetAsync(m->d_avg.get(), 0, width * sizeof(float), ctx->stream));
+    *out = m.release();
     return B2S_OK;
 }
 
-void b2s_mavg_destroy(b2s_mavg *m) {
-    if (!m) return;
-    DeviceGuard g(m->ctx->device);
-    cudaStreamSynchronize(m->ctx->stream);
-    if (m->d_avg) cudaFree(m->d_avg);
-    delete m;
-}
+void b2s_mavg_destroy(b2s_mavg *m) { PlanDeleter<b2s_mavg>()(m); }
 
 // One Kernel::work call (moving_avg.rs:72-115).  consumed / produced are in ITEMS (multiples of WIDTH).
 int32_t b2s_mavg_exec(b2s_mavg *m, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
@@ -151,7 +145,7 @@ int32_t b2s_mavg_exec(b2s_mavg *m, const void *d_in, size_t n_in, void *d_out, s
     DeviceGuard g(m->ctx->device);
     NvtxRange nvtx("b2s_mavg_exec");
     mavg_kernel<<<(unsigned)ceil_div(W, (size_t)kMaBins), 32 * kMaWarps, 0, m->ctx->stream>>>(
-        (const float *)d_in, (float *)d_out, m->d_avg, (int)W, (long long)c, (int)m->history, (int)m->i, m->decay,
+        (const float *)d_in, (float *)d_out, m->d_avg.get(), (int)W, (long long)c, (int)m->history, (int)m->i, m->decay,
         (long long)p);
     B2S_CHECK_LAUNCH(m->ctx);
     m->i = i;

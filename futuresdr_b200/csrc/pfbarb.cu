@@ -46,10 +46,10 @@ struct b2s_pfbarb {
     b2s_ctx *ctx = nullptr;
     size_t num_filters = 0, T = 0, ntaps = 0;
     float rate = 1.f, delay = 1.f;
-    float2 *d_arms = nullptr;      // [num_filters][T] PAIRS (arm_b[T-1-j], arm_{(b+1) % N}[T-1-j]), time-reversed: an output blends
+    Buf<float2> d_arms;            // [num_filters][T] PAIRS (arm_b[T-1-j], arm_{(b+1) % N}[T-1-j]), time-reversed: an output blends
                                    // arm b and its successor (arm 0 after the last one: the Boundary state), one 8-byte load per tap
-    float2 *d_circ = nullptr;      // 2*T, the reference's circular buffer (only used while filling)
-    float2 *d_hist = nullptr;      // T samples of history once filled
+    Buf<float2> d_circ;            // 2*T, the reference's circular buffer (only used while filling)
+    Buf<float2> d_hist;            // T samples of history once filled
     // WindowBuffer bookkeeping (host)
     size_t start_idx = 0, missing = 0;
     // State (host): arb_resampler.rs:40-52
@@ -60,11 +60,10 @@ struct b2s_pfbarb {
     bool periodic = false;
     uint64_t lambda = 0, out_per_period = 0, gpos = 0;   // gpos: samples processed since the window filled
     std::vector<SubRec> tab;       // host copy, tab[j] = state before sample kPerSB*j of the period (out0 = outputs so far)
-    SubRec *d_tab = nullptr;
+    Buf<SubRec> d_tab;
     // per-call records
-    SubRec *h_recs = nullptr;      // pinned
-    SubRec *d_recs = nullptr;
-    size_t recs_cap = 0;
+    Buf<SubRec, Mem::Pinned> h_recs;
+    Buf<SubRec> d_recs;
 };
 
 namespace {
@@ -383,7 +382,7 @@ int32_t b2s_pfbarb_plan_c32(b2s_ctx *ctx, const float *taps, size_t ntaps, size_
     // a 32-sample sub-block must fit the descriptor tile of a CTA: (ceil(rate) + 1) * 32 <= kDescCap
     if (num_filters > (1u << 20) || rate > 126.f) return b2s_fail(ctx, B2S_EUNSUPPORTED, "PfbArbResampler: num_filters / rate too large (rate <= 126)");
     DeviceGuard g(ctx->device);
-    b2s_pfbarb *p = new b2s_pfbarb();
+    PlanPtr<b2s_pfbarb> p(new b2s_pfbarb());
     p->ctx = ctx; p->num_filters = num_filters; p->ntaps = ntaps; p->rate = rate;
     p->delay = 1.0f / rate;
     // partition_filter_taps (utilities.rs:9-19): T = ceil(len as f32 / n as f32); arm i = taps[i::n] zero padded
@@ -397,36 +396,19 @@ int32_t b2s_pfbarb_plan_c32(b2s_ctx *ctx, const float *taps, size_t ntaps, size_
     std::vector<float2> pairs(num_filters * T);
     for (size_t b = 0; b < num_filters; b++)
         for (size_t j = 0; j < T; j++) pairs[b * T + j] = make_float2(arms[b * T + j], arms[((b + 1) % num_filters) * T + j]);
-    cudaError_t e1 = cudaMalloc((void **)&p->d_arms, pairs.size() * sizeof(float2));
-    cudaError_t e2 = cudaMalloc((void **)&p->d_circ, 2 * T * sizeof(float2));
-    cudaError_t e3 = cudaMalloc((void **)&p->d_hist, T * sizeof(float2));
-    if (e1 != cudaSuccess || e2 != cudaSuccess || e3 != cudaSuccess) { b2s_pfbarb_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "pfbarb buffers"); }
-    B2S_CUDA(ctx, cudaMemcpyAsync(p->d_arms, pairs.data(), pairs.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    p->periodic = getenv("B2S_PFBARB_NO_PERIODIC") ? false : build_periodic_schedule(p);
-    if (p->periodic) {
-        if (cudaMalloc((void **)&p->d_tab, p->tab.size() * sizeof(SubRec)) != cudaSuccess) {
-            cudaGetLastError(); b2s_pfbarb_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "pfbarb schedule table");
-        }
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_tab, p->tab.data(), p->tab.size() * sizeof(SubRec), cudaMemcpyHostToDevice, ctx->stream));
-    }
+    B2S_TRY(p->d_arms.upload(ctx, pairs.data(), pairs.size(), "pfbarb arms"));
+    B2S_TRY(p->d_circ.alloc(ctx, 2 * T, "pfbarb window"));
+    B2S_TRY(p->d_hist.alloc(ctx, T, "pfbarb history"));
+    p->periodic = getenv("B2S_PFBARB_NO_PERIODIC") ? false : build_periodic_schedule(p.get());
+    if (p->periodic) B2S_TRY(p->d_tab.upload(ctx, p->tab.data(), p->tab.size(), "pfbarb schedule table"));
     B2S_CUDA(ctx, cudaFuncSetAttribute(pfb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPaSmemMax));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = p;
-    return b2s_pfbarb_reset(p);
+    B2S_TRY(b2s_pfbarb_reset(p.get()));
+    *out = p.release();
+    return B2S_OK;
 }
 
-void b2s_pfbarb_destroy(b2s_pfbarb *p) {
-    if (!p) return;
-    DeviceGuard g(p->ctx->device);
-    cudaStreamSynchronize(p->ctx->stream);
-    if (p->d_arms) cudaFree(p->d_arms);
-    if (p->d_circ) cudaFree(p->d_circ);
-    if (p->d_hist) cudaFree(p->d_hist);
-    if (p->d_recs) cudaFree(p->d_recs);
-    if (p->d_tab) cudaFree(p->d_tab);
-    if (p->h_recs) cudaFreeHost(p->h_recs);
-    delete p;
-}
+void b2s_pfbarb_destroy(b2s_pfbarb *p) { PlanDeleter<b2s_pfbarb>()(p); }
 
 int32_t b2s_pfbarb_reset(b2s_pfbarb *p) {
     if (!p) return b2s_fail(nullptr, B2S_EINVAL, "pfbarb is NULL");
@@ -434,8 +416,8 @@ int32_t b2s_pfbarb_reset(b2s_pfbarb *p) {
     p->start_idx = 0; p->missing = p->T;                           // WindowBuffer::new(len, pad_start=false)
     p->tau = 0.f; p->bf = 0.f; p->mu = 0.f; p->base_index = 0; p->boundary = false;
     p->gpos = 0;
-    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_circ, 0, 2 * p->T * sizeof(float2), p->ctx->stream));
-    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_hist, 0, p->T * sizeof(float2), p->ctx->stream));
+    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_circ.get(), 0, 2 * p->T * sizeof(float2), p->ctx->stream));
+    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_hist.get(), 0, p->T * sizeof(float2), p->ctx->stream));
     return B2S_OK;
 }
 
@@ -451,12 +433,12 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
     if (p->missing != 0) {
         const size_t c = std::min(p->missing, n_in);
         if (c) {
-            pfb_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, p->d_circ, T, (int)p->start_idx, (int)p->missing, (int)c);
+            pfb_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, p->d_circ.get(), T, (int)p->start_idx, (int)p->missing, (int)c);
             B2S_CHECK_LAUNCH(ctx);
             p->missing -= c;
             p->start_idx = (p->start_idx + c) % p->T;
             if (p->missing == 0) {
-                pfb_hist_from_circ<<<1, 256, 0, ctx->stream>>>(p->d_circ, p->d_hist, T, (int)p->start_idx);
+                pfb_hist_from_circ<<<1, 256, 0, ctx->stream>>>(p->d_circ.get(), p->d_hist.get(), T, (int)p->start_idx);
                 B2S_CHECK_LAUNCH(ctx);
             }
         }
@@ -472,7 +454,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
     if (n >= (1ull << 31)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_pfbarb_exec: more than 2^31 items per call");
     NvtxRange nvtx("b2s_pfbarb_exec");
     PaParams P{};
-    P.in = in; P.hist = p->d_hist; P.out = (float2 *)d_out; P.arms = p->d_arms;
+    P.in = in; P.hist = p->d_hist.get(); P.out = (float2 *)d_out; P.arms = p->d_arms.get();
     P.n_in = (long long)n; P.N = (int)p->num_filters; P.T = T; P.delay = p->delay;
     size_t nout;
     Timing after;                                  // fallback path: the state to commit once the call is accepted
@@ -486,7 +468,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
             return b2s_fail(ctx, B2S_ESTATE, "pfbarb: schedule produces %zu > capacity %zu (the reference would overrun its slice)", nout, n_out_cap);
         const uint64_t lsb_first = g0 / kPerSB;                                   // g0 < lambda
         const uint64_t gl = g1 - 1, lsb_last = (gl / lam) * R + (gl % lam) / kPerSB;
-        P.periodic = 1; P.recs = p->d_tab; P.sb_len = kPerSB;
+        P.periodic = 1; P.recs = p->d_tab.get(); P.sb_len = kPerSB;
         P.lambda = lam; P.out_per_period = p->out_per_period; P.R = R; P.g0 = g0; P.lsb_first = lsb_first;
         P.O_g0 = (long long)O0;
         P.nsub = (long long)(lsb_last - lsb_first + 1);
@@ -494,30 +476,26 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
         // per-call host replay (trajectories with a pre-period / very long cycles): the state at every 32nd sample
         const size_t nsub = ceil_div(n, (size_t)kSB);
         B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));        // the pinned records of the previous call may still be in flight
-        if (p->recs_cap < nsub + 1) {
-            if (p->d_recs) cudaFree(p->d_recs);
-            if (p->h_recs) cudaFreeHost(p->h_recs);
-            p->d_recs = nullptr; p->h_recs = nullptr; p->recs_cap = 0;
+        if (std::min(p->d_recs.size(), p->h_recs.size()) < nsub + 1) {
             const size_t want = (nsub + 1) * 5 / 4 + 16;
-            B2S_CUDA(ctx, cudaMalloc((void **)&p->d_recs, want * sizeof(SubRec)));
-            B2S_CUDA(ctx, cudaHostAlloc((void **)&p->h_recs, want * sizeof(SubRec), cudaHostAllocDefault));
-            p->recs_cap = want;
+            B2S_TRY(p->d_recs.reserve(ctx, want, "pfbarb records"));
+            B2S_TRY(p->h_recs.reserve(ctx, want, "pfbarb pinned records"));
         }
         Timing t;                                  // replay on a COPY: nothing is committed if the call is refused
         t.tau = p->tau; t.mu = p->mu; t.base = (uint32_t)p->base_index; t.boundary = p->boundary;
         const uint32_t N = (uint32_t)p->num_filters;
         uint64_t o = 0;
         for (size_t s = 0; s < n; s++) {
-            if ((s % kSB) == 0) p->h_recs[s / kSB] = t.rec((uint32_t)o);
+            if ((s % kSB) == 0) p->h_recs.get()[s / kSB] = t.rec((uint32_t)o);
             o += t.step(N, (float)N, p->delay);
         }
-        p->h_recs[nsub] = t.rec((uint32_t)o);
+        p->h_recs.get()[nsub] = t.rec((uint32_t)o);
         nout = (size_t)o;
         if (nout > n_out_cap || o >= (1ull << 32))
             return b2s_fail(ctx, B2S_ESTATE, "pfbarb: schedule produces %zu > capacity %zu (the reference would overrun its slice)", nout, n_out_cap);
         after = t;
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_recs, p->h_recs, (nsub + 1) * sizeof(SubRec), cudaMemcpyHostToDevice, ctx->stream));
-        P.periodic = 0; P.recs = p->d_recs; P.sb_len = kSB; P.nsub = (long long)nsub;
+        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_recs.get(), p->h_recs.get(), (nsub + 1) * sizeof(SubRec), cudaMemcpyHostToDevice, ctx->stream));
+        P.periodic = 0; P.recs = p->d_recs.get(); P.sb_len = kSB; P.nsub = (long long)nsub;
     }
     P.nout = (long long)nout;
     // CTA tiling: sub-blocks per CTA so that a CTA never exceeds kDescCap outputs
@@ -536,7 +514,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
                         (P.arms_in_smem ? arms_smem_bytes : 0);
     pfb_kernel<<<grid, kPaThreads, smem, ctx->stream>>>(P);
     B2S_CHECK_LAUNCH(ctx);
-    pfb_hist_update<<<1, 256, T * sizeof(float2), ctx->stream>>>(p->d_hist, in, T, (long long)n);
+    pfb_hist_update<<<1, 256, T * sizeof(float2), ctx->stream>>>(p->d_hist.get(), in, T, (long long)n);
     B2S_CHECK_LAUNCH(ctx);
     // the call is on the stream: commit the timing state
     if (p->periodic) p->gpos = (p->gpos + n) % p->lambda;

@@ -19,8 +19,8 @@ struct b2s_resamp {
     b2s_kind kind = B2S_C32_F32;
     size_t ntaps = 0, interp = 1, decim = 1, T = 0;
     int pitch = 0;
-    float *d_banks = nullptr;    // [L][pitch]
-    float *d_gtab = nullptr;     // [L][M][Upad] per-phase taps of the sliding-window kernel (fir_direct.cu), or NULL
+    Buf<float> d_banks;          // [L][pitch]
+    Buf<float> d_gtab;           // [L][M][Upad] per-phase taps of the sliding-window kernel (fir_direct.cu), or empty
 };
 
 namespace {
@@ -111,35 +111,24 @@ int32_t b2s_resamp_plan(b2s_ctx *ctx, b2s_kind kind, const float *taps, size_t n
         return b2s_fail(ctx, B2S_EINVAL, "b2s_resamp_plan: ntaps (%zu) must be a multiple of interp (%zu)", ntaps, interp);
     if (interp > 4096 || decim > 65536 || ntaps > (1u << 20)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_resamp_plan: factors too large");
     DeviceGuard g(ctx->device);
-    b2s_resamp *r = new b2s_resamp();
+    PlanPtr<b2s_resamp> r(new b2s_resamp());
     r->ctx = ctx; r->kind = kind; r->ntaps = ntaps; r->interp = interp; r->decim = decim; r->T = ntaps / interp;
     r->pitch = (int)(r->T | 1);                                   // odd row pitch
     std::vector<float> h(interp * r->pitch, 0.0f);
     for (size_t b = 0; b < interp; b++)
         for (size_t t = 0; t < r->T; t++) h[b * r->pitch + t] = taps[interp * (r->T - 1 - t) + b];   // :114
-    cudaError_t e = cudaMalloc((void **)&r->d_banks, h.size() * sizeof(float));
-    if (e != cudaSuccess) { delete r; return b2s_fail(ctx, B2S_ENOMEM, "resampler taps"); }
-    B2S_CUDA(ctx, cudaMemcpyAsync(r->d_banks, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    B2S_TRY(r->d_banks.upload(ctx, h.data(), h.size(), "resampler taps"));
     std::vector<float> gt;
     if (resamp_slide_supported(interp, decim, r->T, kind_in_bytes(kind))) {
         gt = slide_table(taps, 1, interp, decim, r->T, 0);
-        e = cudaMalloc((void **)&r->d_gtab, gt.size() * sizeof(float));
-        if (e != cudaSuccess) { cudaFree(r->d_banks); delete r; return b2s_fail(ctx, B2S_ENOMEM, "resampler phase taps"); }
-        B2S_CUDA(ctx, cudaMemcpyAsync(r->d_gtab, gt.data(), gt.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        B2S_TRY(r->d_gtab.upload(ctx, gt.data(), gt.size(), "resampler phase taps"));
     }
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = r;
+    *out = r.release();
     return B2S_OK;
 }
 
-void b2s_resamp_destroy(b2s_resamp *r) {
-    if (!r) return;
-    DeviceGuard g(r->ctx->device);
-    cudaStreamSynchronize(r->ctx->stream);
-    if (r->d_banks) cudaFree(r->d_banks);
-    if (r->d_gtab) cudaFree(r->d_gtab);
-    delete r;
-}
+void b2s_resamp_destroy(b2s_resamp *r) { PlanDeleter<b2s_resamp>()(r); }
 
 size_t b2s_resamp_length(const b2s_resamp *r) { return r ? r->ntaps : 0; }   // Filter::length = taps.num_taps() (:141-143)
 
@@ -160,7 +149,7 @@ int32_t b2s_resamp_exec(b2s_resamp *r, const void *d_in, size_t n_in, void *d_ou
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("b2s_resamp_exec");
     if (r->d_gtab)   // small L*M: L decimate-by-M sliding-window passes over one staged tile (fir_direct.cu)
-        return resamp_slide_launch(ctx, r->kind, r->d_gtab, L, M, T, d_in, n_in, d_out, p, ctx->stream);
+        return resamp_slide_launch(ctx, r->kind, r->d_gtab.get(), L, M, T, d_in, n_in, d_out, p, ctx->stream);
     const size_t isz = kind_in_bytes(r->kind);
     const int G = (int)ceil_div((size_t)kRsThreads, L);                      // S = L*G >= 256 outputs per slab
     const size_t tile_out = (size_t)kRsR * L * G;
@@ -172,10 +161,10 @@ int32_t b2s_resamp_exec(b2s_resamp *r, const void *d_in, size_t n_in, void *d_ou
     if (xs_bytes > 200 * 1024) {   // the span does not fit one tile in shared memory
         const unsigned nb = (unsigned)ceil_div(p, (size_t)kRsThreads);
         if (r->kind == B2S_F32_F32)
-            resamp_naive_kernel<float><<<nb, kRsThreads, 0, ctx->stream>>>((const float *)d_in, (float *)d_out, r->d_banks,
+            resamp_naive_kernel<float><<<nb, kRsThreads, 0, ctx->stream>>>((const float *)d_in, (float *)d_out, r->d_banks.get(),
                                                                            (int)L, (int)M, (int)T, r->pitch, (long long)p);
         else
-            resamp_naive_kernel<float2><<<nb, kRsThreads, 0, ctx->stream>>>((const float2 *)d_in, (float2 *)d_out, r->d_banks,
+            resamp_naive_kernel<float2><<<nb, kRsThreads, 0, ctx->stream>>>((const float2 *)d_in, (float2 *)d_out, r->d_banks.get(),
                                                                              (int)L, (int)M, (int)T, r->pitch, (long long)p);
         B2S_CHECK_LAUNCH(ctx);
         return B2S_OK;
@@ -189,7 +178,7 @@ int32_t b2s_resamp_exec(b2s_resamp *r, const void *d_in, size_t n_in, void *d_ou
             B2S_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024)); \
             optin.done(ctx->device);                                                                         \
         }                                                                                                    \
-        kern<<<grid, kRsThreads, smem, ctx->stream>>>((const S *)d_in, (S *)d_out, r->d_banks, (int)L, (int)M, \
+        kern<<<grid, kRsThreads, smem, ctx->stream>>>((const S *)d_in, (S *)d_out, r->d_banks.get(), (int)L, (int)M, \
                                                       (int)T, r->pitch, (long long)p, G, (int)(xs_bytes / isz)); \
     } while (0)
     if (r->kind == B2S_F32_F32) { if (taps_smem) RS_LAUNCH(float, true); else RS_LAUNCH(float, false); }

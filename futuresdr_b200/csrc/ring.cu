@@ -34,9 +34,13 @@ struct b2s_ring {
     std::vector<b2s_slot> slots;
     std::deque<int> empty, full;
     mutable std::mutex mu;
-    char *d_mem = nullptr;
-    char *h_mem = nullptr;
+    Buf<char> d_mem;
+    Buf<char, Mem::Pinned> h_mem;
     size_t slot_bytes = 0, halo_bytes = 0, total_bytes = 0, flags_off = 0;
+
+    ~b2s_ring() {
+        for (auto &s : slots) if (s.ev) cudaEventDestroy(s.ev);
+    }
 };
 
 extern "C" {
@@ -48,7 +52,7 @@ int32_t b2s_ring_create(b2s_ctx *ctx, size_t item_bytes, size_t chunk_items, siz
     if (item_bytes == 0 || chunk_items == 0 || n_slots < 1 || n_slots > 1024)
         return b2s_fail(ctx, B2S_EINVAL, "b2s_ring_create: bad geometry");
     DeviceGuard g(ctx->device);
-    b2s_ring *r = new b2s_ring();
+    PlanPtr<b2s_ring> r(new b2s_ring());
     r->ctx = ctx; r->item_bytes = item_bytes; r->chunk_items = chunk_items; r->halo_items = halo_items;
     const size_t halo_bytes = round_up(halo_items * item_bytes, 256);
     const size_t data_bytes = round_up(chunk_items * item_bytes, 256);
@@ -57,35 +61,23 @@ int32_t b2s_ring_create(b2s_ctx *ctx, size_t item_bytes, size_t chunk_items, siz
     // system-scope flags {ready, consumed} for the cross-GPU halo handshake (peer.cu)
     r->slot_bytes = slot_bytes; r->halo_bytes = halo_bytes; r->flags_off = slot_bytes * n_slots;
     r->total_bytes = r->flags_off + 256;
-    cudaError_t e = cudaMalloc((void **)&r->d_mem, r->total_bytes);
-    if (e != cudaSuccess) { cudaGetLastError(); delete r; return b2s_fail(ctx, B2S_ENOMEM, "ring: %zu bytes of device memory", r->total_bytes); }
-    cudaMemsetAsync(r->d_mem + r->flags_off, 0, 256, ctx->stream);
-    if (with_host_staging) {
-        e = cudaHostAlloc((void **)&r->h_mem, data_bytes * n_slots, cudaHostAllocDefault);
-        if (e != cudaSuccess) { cudaGetLastError(); cudaFree(r->d_mem); delete r; return b2s_fail(ctx, B2S_ENOMEM, "ring: pinned staging"); }
-    }
+    B2S_TRY(r->d_mem.alloc(ctx, r->total_bytes, "ring device memory"));
+    cudaMemsetAsync(r->d_mem.get() + r->flags_off, 0, 256, ctx->stream);
+    if (with_host_staging) B2S_TRY(r->h_mem.alloc(ctx, data_bytes * n_slots, "ring pinned staging"));
     r->slots.resize(n_slots);
     for (int i = 0; i < n_slots; i++) {
         b2s_slot &s = r->slots[i];
-        s.ring = r; s.index = i;
-        s.d_data = r->d_mem + (size_t)i * slot_bytes + halo_bytes;
-        s.h_stage = r->h_mem ? r->h_mem + (size_t)i * data_bytes : nullptr;
+        s.ring = r.get(); s.index = i;
+        s.d_data = r->d_mem.get() + (size_t)i * slot_bytes + halo_bytes;
+        s.h_stage = r->h_mem ? r->h_mem.get() + (size_t)i * data_bytes : nullptr;
         B2S_CUDA(ctx, cudaEventCreateWithFlags(&s.ev, cudaEventDisableTiming));
         r->empty.push_back(i);
     }
-    *out = r;
+    *out = r.release();
     return B2S_OK;
 }
 
-void b2s_ring_destroy(b2s_ring *r) {
-    if (!r) return;
-    DeviceGuard g(r->ctx->device);
-    cudaStreamSynchronize(r->ctx->stream);
-    for (auto &s : r->slots) if (s.ev) cudaEventDestroy(s.ev);
-    if (r->d_mem) cudaFree(r->d_mem);
-    if (r->h_mem) cudaFreeHost(r->h_mem);
-    delete r;
-}
+void b2s_ring_destroy(b2s_ring *r) { PlanDeleter<b2s_ring>()(r); }
 
 int32_t b2s_ring_acquire_empty(b2s_ring *r, b2s_slot **slot) {
     if (!r || !slot) return b2s_fail(r ? r->ctx : nullptr, B2S_EINVAL, "b2s_ring_acquire_empty: NULL argument");
@@ -183,7 +175,7 @@ int32_t b2s_slot_wait(b2s_slot *s) {
     return B2S_OK;
 }
 
-void *b2s_ring_base(const b2s_ring *r) { return r ? r->d_mem : nullptr; }
+void *b2s_ring_base(const b2s_ring *r) { return r ? r->d_mem.get() : nullptr; }
 size_t b2s_ring_bytes(const b2s_ring *r) { return r ? r->total_bytes : 0; }
 size_t b2s_ring_slot_offset(const b2s_ring *r, int32_t slot_index) {
     if (!r || slot_index < 0 || (size_t)slot_index >= r->slots.size()) return 0;

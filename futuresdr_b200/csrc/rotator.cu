@@ -30,9 +30,8 @@ constexpr size_t kBatchRecs = 1u << 14;         // the worker publishes its prog
 struct b2s_rotator {
     b2s_ctx *ctx = nullptr;
     float incr[2] = {1.f, 0.f};
-    float2 *h_ring = nullptr;                    // pinned, kRingRecs records; record r lives at r % kRingRecs
-    float2 *d_recs = nullptr;                    // records of the calls in flight on the device (two halves)
-    size_t d_cap = 0;
+    Buf<float2, Mem::Pinned> h_ring;             // kRingRecs records; record r lives at r % kRingRecs
+    Buf<float2> d_recs;                          // records of the calls in flight on the device (two halves)
     int half = 0;
     cudaEvent_t ev[2] = {nullptr, nullptr};      // H2D of half i done -> its ring span may be overwritten
     uint64_t span_end[2] = {0, 0};               // one past the last record each half's copy read
@@ -45,6 +44,16 @@ struct b2s_rotator {
     uint64_t released = 0;                       // records below this may be overwritten
     uint64_t epoch = 0;                          // bumped by reset
     bool quit = false;
+
+    void stop_worker() {
+        { std::lock_guard<std::mutex> lk(mu); quit = true; }
+        cv.notify_all();
+        if (worker.joinable()) worker.join();
+    }
+    ~b2s_rotator() {
+        stop_worker();
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    }
 };
 
 namespace {
@@ -65,7 +74,7 @@ void rotator_worker(b2s_rotator *r) {
         // host replay of the recurrence: plain binary32 SSE operations (host code is built with -ffp-contract=off and
         // without -ffast-math, so every product and sum is rounded separately) -- rotator.rs:26, num_complex Mul
         for (; next < limit; next++) {
-            r->h_ring[next % kRingRecs] = make_float2(pr, pi);
+            r->h_ring.get()[next % kRingRecs] = make_float2(pr, pi);
             for (int k = 0; k < kRotSub; k++) {
                 const float a = pr * ir, b = pi * ii, c = pr * ii, d = pi * ir;
                 pr = a - b; pi = c + d;
@@ -107,31 +116,21 @@ int32_t b2s_rotator_create(b2s_ctx *ctx, float phase_incr, b2s_rotator **out) {
     if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_rotator_create: NULL argument");
     *out = nullptr;
     DeviceGuard g(ctx->device);
-    b2s_rotator *r = new b2s_rotator();
+    PlanPtr<b2s_rotator> r(new b2s_rotator());
     r->ctx = ctx;
     // Complex32::from_polar(1.0, phase_incr) = (1.0 * cos, 1.0 * sin) in f32 (rotator.rs:17)
     r->incr[0] = 1.0f * std::cos(phase_incr);
     r->incr[1] = 1.0f * std::sin(phase_incr);
-    if (cudaHostAlloc((void **)&r->h_ring, kRingRecs * sizeof(float2), cudaHostAllocDefault) != cudaSuccess) {
-        cudaGetLastError(); delete r; return b2s_fail(ctx, B2S_ENOMEM, "rotator: pinned record ring");
-    }
+    B2S_TRY(r->h_ring.alloc(ctx, kRingRecs, "rotator: pinned record ring"));
     for (int i = 0; i < 2; i++) B2S_CUDA(ctx, cudaEventCreateWithFlags(&r->ev[i], cudaEventDisableTiming));
-    r->worker = std::thread(rotator_worker, r);
-    *out = r;
+    r->worker = std::thread(rotator_worker, r.get());
+    *out = r.release();
     return B2S_OK;
 }
 
 void b2s_rotator_destroy(b2s_rotator *r) {
-    if (!r) return;
-    DeviceGuard g(r->ctx->device);
-    { std::lock_guard<std::mutex> lk(r->mu); r->quit = true; }
-    r->cv.notify_all();
-    if (r->worker.joinable()) r->worker.join();
-    cudaStreamSynchronize(r->ctx->stream);
-    for (int i = 0; i < 2; i++) if (r->ev[i]) cudaEventDestroy(r->ev[i]);
-    if (r->d_recs) cudaFree(r->d_recs);
-    if (r->h_ring) cudaFreeHost(r->h_ring);
-    delete r;
+    if (r) r->stop_worker();
+    PlanDeleter<b2s_rotator>()(r);
 }
 
 int32_t b2s_rotator_reset(b2s_rotator *r) {
@@ -162,13 +161,8 @@ int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_
     // pieces of at most a quarter of the ring, so that the worker can keep running ahead while a piece is in flight
     const size_t piece_max = (kRingRecs / 4) * kRotSub;
     const size_t d_need = std::min(n, piece_max) / kRotSub + 2;
-    if (r->d_cap < d_need) {
-        B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (r->d_recs) cudaFree(r->d_recs);
-        r->d_recs = nullptr; r->d_cap = 0;
-        B2S_CUDA(ctx, cudaMalloc((void **)&r->d_recs, 2 * d_need * sizeof(float2)));
-        r->d_cap = d_need;
-    }
+    B2S_TRY(r->d_recs.reserve(ctx, 2 * d_need, "rotator records"));
+    const size_t d_cap = r->d_recs.size() / 2;
     size_t done = 0;
     while (done < n) {
         const size_t m = std::min(n - done, piece_max);
@@ -198,12 +192,12 @@ int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_
             std::lock_guard<std::mutex> lk2(r->mu);
             if (r->released + kRingRecs < rec1) return b2s_fail(ctx, B2S_ESTATE, "rotator: record ring accounting");
         }
-        float2 *drec = r->d_recs + (size_t)h * r->d_cap;
+        float2 *drec = r->d_recs.get() + (size_t)h * d_cap;
         const size_t i0 = rec0 % kRingRecs, cnt = rec1 - rec0;
         const size_t first = std::min(cnt, kRingRecs - i0);
-        B2S_CUDA(ctx, cudaMemcpyAsync(drec, r->h_ring + i0, first * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+        B2S_CUDA(ctx, cudaMemcpyAsync(drec, r->h_ring.get() + i0, first * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
         if (cnt > first)
-            B2S_CUDA(ctx, cudaMemcpyAsync(drec + first, r->h_ring, (cnt - first) * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
+            B2S_CUDA(ctx, cudaMemcpyAsync(drec + first, r->h_ring.get(), (cnt - first) * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
         B2S_CUDA(ctx, cudaEventRecord(r->ev[h], ctx->stream));
         r->span_end[h] = rec0;                                      // records below rec0 are never needed again
         const int th = 256;

@@ -150,7 +150,7 @@ struct b2s_sigsrc {
     bool cplx = false;
     uint32_t phase = 0, inc = 0;       // NCO (fxpt_nco.rs:5-9), advanced by each exec
     float amplitude = 0.0f;
-    float *d_table = nullptr;          // slope[1024] then offset[1024]
+    Buf<SineTable> d_table;            // slope[1024] then offset[1024]
 };
 
 extern "C" {
@@ -175,7 +175,7 @@ int32_t b2s_sigsrc_create(b2s_ctx *ctx, b2s_wave wave, int32_t complex_items, fl
     if (wave != B2S_WAVE_COS && wave != B2S_WAVE_SIN && wave != B2S_WAVE_SQUARE)
         return b2s_fail(ctx, B2S_EINVAL, "b2s_sigsrc_create: wave %d is not COS, SIN or SQUARE", (int)wave);
     DeviceGuard g(ctx->device);
-    b2s_sigsrc *s = new b2s_sigsrc();
+    PlanPtr<b2s_sigsrc> s(new b2s_sigsrc());
     s->ctx = ctx;
     s->wave = wave;
     s->cplx = complex_items != 0;
@@ -185,28 +185,12 @@ int32_t b2s_sigsrc_create(b2s_ctx *ctx, b2s_wave wave, int32_t complex_items, fl
     const float w = two_pi * frequency;
     s->phase = (uint32_t)fxpt_phase_new(initial_phase);
     s->inc = (uint32_t)fxpt_phase_new(w / sample_rate);
-    const SineTable &t = sine_table();
-    if (cudaMalloc((void **)&s->d_table, sizeof(SineTable)) != cudaSuccess) {
-        cudaGetLastError();
-        delete s;
-        return b2s_fail(ctx, B2S_ENOMEM, "sigsrc table");
-    }
-    if (cudaMemcpy(s->d_table, &t, sizeof(SineTable), cudaMemcpyHostToDevice) != cudaSuccess) {
-        cudaFree(s->d_table);
-        delete s;
-        return b2s_fail(ctx, B2S_ECUDA, "sigsrc table upload");
-    }
-    *out = s;
+    B2S_TRY(s->d_table.upload(ctx, &sine_table(), 1, "sigsrc table"));
+    *out = s.release();
     return B2S_OK;
 }
 
-void b2s_sigsrc_destroy(b2s_sigsrc *s) {
-    if (!s) return;
-    DeviceGuard g(s->ctx->device);
-    cudaStreamSynchronize(s->ctx->stream);
-    cudaFree(s->d_table);
-    delete s;
-}
+void b2s_sigsrc_destroy(b2s_sigsrc *s) { PlanDeleter<b2s_sigsrc>()(s); }
 
 int32_t b2s_sigsrc_set_amplitude(b2s_sigsrc *s, float amplitude) {
     if (!s) return b2s_fail(nullptr, B2S_EINVAL, "sigsrc is NULL");
@@ -240,13 +224,14 @@ int32_t b2s_sigsrc_exec(b2s_sigsrc *s, void *d_out, size_t n_out_cap, size_t *pr
     const uint32_t ph = s->phase, inc = s->inc;
     const float amp = s->amplitude;
     const uint32_t nan_bits = x86_nan_of_product(amp);
+    const float *table = reinterpret_cast<const float *>(s->d_table.get());
     switch (s->wave * 2 + (s->cplx ? 1 : 0)) {
-        case B2S_WAVE_COS * 2: launch<B2S_WAVE_COS, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, s->d_table); break;
-        case B2S_WAVE_SIN * 2: launch<B2S_WAVE_SIN, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, s->d_table); break;
-        case B2S_WAVE_SQUARE * 2: launch<B2S_WAVE_SQUARE, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, s->d_table); break;
+        case B2S_WAVE_COS * 2: launch<B2S_WAVE_COS, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, table); break;
+        case B2S_WAVE_SIN * 2: launch<B2S_WAVE_SIN, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, table); break;
+        case B2S_WAVE_SQUARE * 2: launch<B2S_WAVE_SQUARE, false>(grid, st, o, nf, head, ph, inc, amp, nan_bits, table); break;
         case B2S_WAVE_COS * 2 + 1:                      // Complex32 cos is sin (mod.rs:175-182)
-        case B2S_WAVE_SIN * 2 + 1: launch<B2S_WAVE_SIN, true>(grid, st, o, nf, head, ph, inc, amp, nan_bits, s->d_table); break;
-        default: launch<B2S_WAVE_SQUARE, true>(grid, st, o, nf, head, ph, inc, amp, nan_bits, s->d_table); break;
+        case B2S_WAVE_SIN * 2 + 1: launch<B2S_WAVE_SIN, true>(grid, st, o, nf, head, ph, inc, amp, nan_bits, table); break;
+        default: launch<B2S_WAVE_SQUARE, true>(grid, st, o, nf, head, ph, inc, amp, nan_bits, table); break;
     }
     B2S_CHECK_LAUNCH(s->ctx);
     s->phase += (uint32_t)n_out_cap * s->inc;           // n steps of the NCO, wrapping

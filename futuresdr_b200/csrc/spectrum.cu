@@ -31,11 +31,10 @@ struct b2s_spectrum {
     int log2n = 0, shift = 0;
     size_t history = 1;
     float decay = 0.1f, log10_k = 0.0f;
-    float2 *d_tw = nullptr;
-    float *d_avg = nullptr;        // [n] running average, OUTPUT (post-shift) bin order
-    float *d_final = nullptr;      // [groups][n] local final states / carries (grown on demand)
-    float *d_pow = nullptr;        // a^k, k = 0..cap
-    size_t final_cap = 0, pow_cap = 0;
+    Buf<float2> d_tw;
+    Buf<float> d_avg;              // [n] running average, OUTPUT (post-shift) bin order
+    Buf<float> d_final;            // [groups][n] local final states / carries (grown on demand)
+    Buf<float> d_pow;              // a^k, k = 0..cap
     size_t i = 0;                  // frames since the last emission (moving_avg.rs: self.i)
     int resident = 0;              // CTAs per SM of the kernel instantiation (occupancy query, first exec)
 };
@@ -226,37 +225,26 @@ int32_t b2s_spectrum_plan(b2s_ctx *ctx, size_t n, int32_t fft_shift, float decay
     if (!(decay_factor >= 0.0f && decay_factor <= 1.0f)) return b2s_fail(ctx, B2S_EINVAL, "decay_factor must be in [0, 1]");
     if (history_size == 0) return b2s_fail(ctx, B2S_EINVAL, "b2s_spectrum_plan: history_size must be > 0");
     DeviceGuard g(ctx->device);
-    b2s_spectrum *p = new b2s_spectrum();
+    PlanPtr<b2s_spectrum> p(new b2s_spectrum());
     p->ctx = ctx; p->n = n; p->shift = fft_shift != 0; p->decay = decay_factor; p->history = history_size;
     p->log10_k = log10_scale;
     while (((size_t)1 << p->log2n) < n) p->log2n++;
     const std::vector<float2> tw = twiddle_table(n);
-    if (cudaMalloc((void **)&p->d_tw, n * sizeof(float2)) != cudaSuccess || cudaMalloc((void **)&p->d_avg, n * sizeof(float)) != cudaSuccess) {
-        cudaGetLastError(); b2s_spectrum_destroy(p); return b2s_fail(ctx, B2S_ENOMEM, "spectrum tables");
-    }
-    B2S_CUDA(ctx, cudaMemcpyAsync(p->d_tw, tw.data(), n * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaMemsetAsync(p->d_avg, 0, n * sizeof(float), ctx->stream));
+    B2S_TRY(p->d_tw.upload(ctx, tw.data(), n, "spectrum twiddles"));
+    B2S_TRY(p->d_avg.alloc(ctx, n, "spectrum average"));
+    B2S_CUDA(ctx, cudaMemsetAsync(p->d_avg.get(), 0, n * sizeof(float), ctx->stream));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = p;
+    *out = p.release();
     return B2S_OK;
 }
 
-void b2s_spectrum_destroy(b2s_spectrum *p) {
-    if (!p) return;
-    DeviceGuard g(p->ctx->device);
-    cudaStreamSynchronize(p->ctx->stream);
-    if (p->d_tw) cudaFree(p->d_tw);
-    if (p->d_avg) cudaFree(p->d_avg);
-    if (p->d_final) cudaFree(p->d_final);
-    if (p->d_pow) cudaFree(p->d_pow);
-    delete p;
-}
+void b2s_spectrum_destroy(b2s_spectrum *p) { PlanDeleter<b2s_spectrum>()(p); }
 
 int32_t b2s_spectrum_reset(b2s_spectrum *p) {
     if (!p) return b2s_fail(nullptr, B2S_EINVAL, "spectrum is NULL");
     DeviceGuard g(p->ctx->device);
     p->i = 0;
-    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_avg, 0, p->n * sizeof(float), p->ctx->stream));
+    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_avg.get(), 0, p->n * sizeof(float), p->ctx->stream));
     return B2S_OK;
 }
 
@@ -290,29 +278,18 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     const size_t g_target = (size_t)ctx->sm_count * resident * FPB;
     const size_t C = std::max<size_t>(4, ceil_div(frames, g_target));
     const size_t groups = ceil_div(frames, C);
-    if (p->final_cap < groups * N) {
-        B2S_CUDA(ctx, cudaStreamSynchronize(st));
-        if (p->d_final) cudaFree(p->d_final);
-        p->d_final = nullptr; p->final_cap = 0;
-        const size_t want = groups * N * 5 / 4;
-        if (cudaMalloc((void **)&p->d_final, want * sizeof(float)) != cudaSuccess) { cudaGetLastError(); return b2s_fail(ctx, B2S_ENOMEM, "spectrum carries"); }
-        p->final_cap = want;
-    }
-    if (p->pow_cap < C + 1) {
-        B2S_CUDA(ctx, cudaStreamSynchronize(st));
-        if (p->d_pow) cudaFree(p->d_pow);
-        p->d_pow = nullptr; p->pow_cap = 0;
+    if (p->d_final.size() < groups * N) B2S_TRY(p->d_final.reserve(ctx, groups * N * 5 / 4, "spectrum carries"));
+    if (p->d_pow.size() < C + 1) {
         const size_t want = (C + 1) * 2;
-        if (cudaMalloc((void **)&p->d_pow, want * sizeof(float)) != cudaSuccess) { cudaGetLastError(); return b2s_fail(ctx, B2S_ENOMEM, "spectrum powers"); }
+        B2S_TRY(p->d_pow.reserve(ctx, want, "spectrum powers"));
         std::vector<float> pw(want);
         const double a = (double)(1.0f - p->decay);
         for (size_t k = 0; k < want; k++) pw[k] = (float)std::pow(a, (double)k);
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_pow, pw.data(), want * sizeof(float), cudaMemcpyHostToDevice, st));
+        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_pow.get(), pw.data(), want * sizeof(float), cudaMemcpyHostToDevice, st));
         B2S_CUDA(ctx, cudaStreamSynchronize(st));            // pw is a stack-owned vector
-        p->pow_cap = want;
     }
     SpArgs a;
-    a.in = (const float2 *)d_in; a.out = (float *)d_out; a.fin = p->d_final; a.tw = p->d_tw;
+    a.in = (const float2 *)d_in; a.out = (float *)d_out; a.fin = p->d_final.get(); a.tw = p->d_tw.get();
     a.nframes = (long long)frames; a.C = (long long)C; a.groups = (int)groups; a.shift = p->shift;
     a.history = (int)h; a.i0 = (int)p->i; a.a = 1.0f - p->decay; a.d = p->decay;
     const int32_t rc = with_log2n<5, 13>(p->log2n, B2S_EUNSUPPORTED, [&](auto L) { return launch_spectrum<L>(p, a, st); });
@@ -320,11 +297,11 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     const double ad = (double)(1.0f - p->decay);
     const size_t c_last = frames - (groups - 1) * C;
     spectrum_scan<<<(unsigned)ceil_div(N, (size_t)32), 32 * kScanSegs, 0, st>>>(
-        p->d_final, p->d_avg, (int)N, (int)groups, (float)std::pow(ad, (double)C), (float)std::pow(ad, (double)c_last));
+        p->d_final.get(), p->d_avg.get(), (int)N, (int)groups, (float)std::pow(ad, (double)C), (float)std::pow(ad, (double)c_last));
     B2S_CHECK_LAUNCH(ctx);
     if (rows) {
         dim3 grid((unsigned)rows, (unsigned)ceil_div(N, (size_t)1024));
-        spectrum_fixup<<<grid, 256, 0, st>>>((float *)d_out, p->d_final, p->d_pow, (int)N, (long long)C, (int)h, (int)p->i, p->log10_k);
+        spectrum_fixup<<<grid, 256, 0, st>>>((float *)d_out, p->d_final.get(), p->d_pow.get(), (int)N, (long long)C, (int)h, (int)p->i, p->log10_k);
         B2S_CHECK_LAUNCH(ctx);
     }
     p->i = (p->i + frames) % h;

@@ -22,15 +22,14 @@ int b2s_fft_log2n(const b2s_fft *p);
 struct b2s_synth {
     b2s_ctx *ctx = nullptr;
     size_t N = 0, T = 0;
-    float *d_arms = nullptr;        // [T][N] tap-major: d_arms[j*N + w] = arm_w[j] = taps[w + j*N]; newest sample <-> j = 0
-    float2 *d_circ = nullptr;       // [N][T] window positions while filling
-    float2 *d_hist = nullptr;       // [N][T] FIFO order once filled
+    Buf<float> d_arms;              // [T][N] tap-major: d_arms[j*N + w] = arm_w[j] = taps[w + j*N]; newest sample <-> j = 0
+    Buf<float2> d_circ;             // [N][T] window positions while filling
+    Buf<float2> d_hist;             // [N][T] FIFO order once filled
     size_t start_idx = 0, missing = 0;
     bool all_filled = false;
-    b2s_fft *ifft = nullptr;
-    float2 *d_tmp = nullptr;        // 2 * tmp_items: gathered vectors, spun vectors
-    size_t tmp_items = 0;
-    float *d_arms_pad = nullptr;    // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
+    PlanPtr<b2s_fft> ifft;
+    Buf<float2> d_tmp;              // two halves: gathered vectors, spun vectors
+    Buf<float> d_arms_pad;          // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
     int tpad = 0;
 };
 
@@ -236,7 +235,7 @@ int32_t synth_fused_launch(b2s_synth *s, const float2 *in, long long in_stride, 
     const long long grid = std::min<long long>(ntiles, (long long)s->ctx->sm_count * resident);
     const long long tpc = (ntiles + grid - 1) / grid;
     const long long grid2 = (ntiles + tpc - 1) / tpc;         // no empty CTAs (the last tile must be owned by the last CTA)
-    kern<<<(unsigned)grid2, 256, smem, s->ctx->stream>>>(in, in_stride, s->d_arms_pad, b2s_fft_twiddles(s->ifft), out, s->d_hist,
+    kern<<<(unsigned)grid2, 256, smem, s->ctx->stream>>>(in, in_stride, s->d_arms_pad.get(), b2s_fft_twiddles(s->ifft.get()), out, s->d_hist.get(),
                                                           (int)s->T, k2, (int)ntiles, (int)tpc);
     B2S_CHECK_LAUNCH(s->ctx);
     return B2S_OK;
@@ -248,7 +247,7 @@ int32_t synth_fused_dispatch(b2s_synth *s, int log2n, const float2 *in, long lon
 }
 
 int synth_fused_tpad(const b2s_synth *s) {
-    const int l2 = b2s_fft_log2n(s->ifft);
+    const int l2 = b2s_fft_log2n(s->ifft.get());
     if (getenv("B2S_SYNTH_NO_FUSED")) return 0;
     if (l2 < 2 || l2 > 8 || s->T > 32) return 0;
     return s->T <= 8 ? 8 : (s->T <= 16 ? 16 : 32);
@@ -262,56 +261,37 @@ size_t synth_fused_lead(int log2n, int tpad) { const int ob = synth_fused_ob(log
 
 extern "C" {
 
-void b2s_synth_destroy(b2s_synth *s);
-
 int32_t b2s_synth_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps, size_t ntaps, b2s_synth **out) {
     if (!ctx || !out || !taps) return b2s_fail(ctx, B2S_EINVAL, "b2s_synth_plan_c32: NULL argument");
     *out = nullptr;
     if (num_channels < 2 || ntaps == 0) return b2s_fail(ctx, B2S_EINVAL, "b2s_synth_plan_c32: need >= 2 channels and taps");
     DeviceGuard g(ctx->device);
-    b2s_synth *s = new b2s_synth();
+    PlanPtr<b2s_synth> s(new b2s_synth());
     s->ctx = ctx; s->N = num_channels;
     const size_t N = s->N, T = (size_t)std::ceil((float)ntaps / (float)N);     // utilities.rs:9
     s->T = T; s->missing = T;
     std::vector<float> arms(N * T, 0.0f);
     for (size_t i = 0; i < N; i++) { size_t j = 0; for (size_t idx = i; idx < ntaps; idx += N) arms[(j++) * N + i] = taps[idx]; }
-    int32_t rc = b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &s->ifft);            // plan_fft(n, Inverse) (synthesizer.rs:65)
-    if (rc != B2S_OK) { delete s; return rc; }
-    if (cudaMalloc((void **)&s->d_arms, arms.size() * sizeof(float)) != cudaSuccess ||
-        cudaMalloc((void **)&s->d_circ, N * T * sizeof(float2)) != cudaSuccess ||
-        cudaMalloc((void **)&s->d_hist, N * T * sizeof(float2)) != cudaSuccess) {
-        b2s_synth_destroy(s);
-        return b2s_fail(ctx, B2S_ENOMEM, "synthesizer buffers");
-    }
-    B2S_CUDA(ctx, cudaMemcpyAsync(s->d_arms, arms.data(), arms.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaMemsetAsync(s->d_circ, 0, N * T * sizeof(float2), ctx->stream));
-    s->tpad = synth_fused_tpad(s);
+    b2s_fft *ifft = nullptr;
+    B2S_TRY(b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &ifft));                  // plan_fft(n, Inverse) (synthesizer.rs:65)
+    s->ifft.reset(ifft);
+    B2S_TRY(s->d_arms.upload(ctx, arms.data(), arms.size(), "synthesizer arms"));
+    B2S_TRY(s->d_circ.alloc(ctx, N * T, "synthesizer windows"));
+    B2S_TRY(s->d_hist.alloc(ctx, N * T, "synthesizer history"));
+    B2S_CUDA(ctx, cudaMemsetAsync(s->d_circ.get(), 0, N * T * sizeof(float2), ctx->stream));
+    s->tpad = synth_fused_tpad(s.get());
     std::vector<float> apad;
     if (s->tpad) {
         apad.assign((size_t)s->tpad * N, 0.0f);                                  // taps beyond T are zero (older samples)
         std::copy(arms.begin(), arms.end(), apad.begin());
-        if (cudaMalloc((void **)&s->d_arms_pad, apad.size() * sizeof(float)) != cudaSuccess) {
-            cudaGetLastError(); b2s_synth_destroy(s); return b2s_fail(ctx, B2S_ENOMEM, "synthesizer buffers");
-        }
-        B2S_CUDA(ctx, cudaMemcpyAsync(s->d_arms_pad, apad.data(), apad.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+        B2S_TRY(s->d_arms_pad.upload(ctx, apad.data(), apad.size(), "synthesizer padded arms"));
     }
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *out = s;
+    *out = s.release();
     return B2S_OK;
 }
 
-void b2s_synth_destroy(b2s_synth *s) {
-    if (!s) return;
-    DeviceGuard g(s->ctx->device);
-    cudaStreamSynchronize(s->ctx->stream);
-    if (s->ifft) b2s_fft_destroy(s->ifft);
-    if (s->d_arms) cudaFree(s->d_arms);
-    if (s->d_circ) cudaFree(s->d_circ);
-    if (s->d_hist) cudaFree(s->d_hist);
-    if (s->d_tmp) cudaFree(s->d_tmp);
-    if (s->d_arms_pad) cudaFree(s->d_arms_pad);
-    delete s;
-}
+void b2s_synth_destroy(b2s_synth *s) { PlanDeleter<b2s_synth>()(s); }
 
 // One Kernel::work call (synthesizer.rs:80-144).  d_in is channel-major (stream w at d_in + w*in_stride),
 // n_in the shortest input slice, d_out the single output slice of n_out_cap items.
@@ -346,38 +326,30 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
     NvtxRange nvtx("b2s_synth_exec");
     // steady calls long enough for two tiles: the first OB vectors (their windows reach into the previous call's
     // history) through the three kernels below, everything after them through the fused kernel
-    const int l2n = b2s_fft_log2n(s->ifft);
+    const int l2n = b2s_fft_log2n(s->ifft.get());
     const size_t ob = s->tpad ? (size_t)synth_fused_ob(l2n) : 0;
     const size_t lead = s->tpad ? synth_fused_lead(l2n, s->tpad) : 0;
     const bool fused = s->tpad && s->all_filled && k1 == 0 && k2 >= lead + ob && k2 >= lead + T;
     const size_t k2_all = k2;
     if (fused) k2 = lead;                                 // the generic part
     const size_t items = (k1 + k2) * N;
-    if (s->tmp_items < items) {
-        B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (s->d_tmp) cudaFree(s->d_tmp);
-        s->tmp_items = items * 5 / 4 + 1024;
-        if (cudaMalloc((void **)&s->d_tmp, 2 * s->tmp_items * sizeof(float2)) != cudaSuccess) {
-            s->d_tmp = nullptr; s->tmp_items = 0; cudaGetLastError();
-            return b2s_fail(ctx, B2S_ENOMEM, "synthesizer workspace");
-        }
-    }
-    float2 *vec = s->d_tmp, *spun = s->d_tmp + s->tmp_items;
+    if (s->d_tmp.size() < 2 * items) B2S_TRY(s->d_tmp.reserve(ctx, 2 * (items * 5 / 4 + 1024), "synthesizer workspace"));
+    float2 *vec = s->d_tmp.get(), *spun = s->d_tmp.get() + s->d_tmp.size() / 2;
     const size_t nvg = k1 + k2;                           // vectors of the generic part
     dim3 gg((unsigned)ceil_div(nvg, (size_t)32), (unsigned)ceil_div(N, (size_t)32));
     synth_gather_kernel<<<gg, dim3(32, 8), 0, ctx->stream>>>((const float2 *)d_in, vec, (int)N, (long long)nvg, (long long)in_stride);
     B2S_CHECK_LAUNCH(ctx);
     size_t fc = 0, fp = 0;
-    int32_t rc = b2s_fft_exec(s->ifft, vec, items, spun, items, &fc, &fp);
+    int32_t rc = b2s_fft_exec(s->ifft.get(), vec, items, spun, items, &fc, &fp);
     if (rc != B2S_OK) return rc;
     if (k1) {
-        synth_fill_kernel<<<(unsigned)ceil_div(N, (size_t)128), 128, 0, ctx->stream>>>(spun, s->d_circ, (int)N, (int)T,
+        synth_fill_kernel<<<(unsigned)ceil_div(N, (size_t)128), 128, 0, ctx->stream>>>(spun, s->d_circ.get(), (int)N, (int)T,
                                                                                          (int)s->start_idx, (int)s->missing, (int)k1);
         B2S_CHECK_LAUNCH(ctx);
         s->missing -= k1;
         s->start_idx = (s->start_idx + k1) % T;
         if (completes) {
-            synth_hist_from_circ<<<(unsigned)N, 64, 0, ctx->stream>>>(s->d_circ, s->d_hist, (int)N, (int)T, (int)s->start_idx);
+            synth_hist_from_circ<<<(unsigned)N, 64, 0, ctx->stream>>>(s->d_circ.get(), s->d_hist.get(), (int)N, (int)T, (int)s->start_idx);
             B2S_CHECK_LAUNCH(ctx);
             s->all_filled = true;
         }
@@ -386,7 +358,7 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
         const int u0 = completes ? -1 : 0;
         const size_t total = (k2 - (long long)u0) * N;
         const unsigned grid = (unsigned)std::min<size_t>(ceil_div(total, (size_t)256), (size_t)ctx->sm_count * 32);
-        synth_bank_kernel<<<grid, 256, 0, ctx->stream>>>(spun + k1 * N, s->d_hist, s->d_arms, (float2 *)d_out, (int)N, (int)T,
+        synth_bank_kernel<<<grid, 256, 0, ctx->stream>>>(spun + k1 * N, s->d_hist.get(), s->d_arms.get(), (float2 *)d_out, (int)N, (int)T,
                                                          u0, (long long)k2);
         B2S_CHECK_LAUNCH(ctx);
     }
@@ -398,7 +370,7 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
         else if (s->tpad == 32) frc = synth_fused_dispatch<32>(s, l2n, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
         if (frc != B2S_OK) return frc == B2S_EAGAIN ? b2s_fail(ctx, B2S_ESTATE, "synthesizer: fused shape mismatch") : frc;
     } else if (k2) {
-        synth_hist_update<<<(unsigned)N, 64, T * sizeof(float2), ctx->stream>>>(s->d_hist, spun + k1 * N, (int)N, (int)T, (long long)k2);
+        synth_hist_update<<<(unsigned)N, 64, T * sizeof(float2), ctx->stream>>>(s->d_hist.get(), spun + k1 * N, (int)N, (int)T, (long long)k2);
         B2S_CHECK_LAUNCH(ctx);
     }
     *consumed_per_channel = nv; *produced = p;

@@ -17,7 +17,7 @@ import enum
 import numpy as np
 
 from . import _lib
-from ._lib import lib, check
+from ._lib import Handle, lib, check
 from .context import Context, default_context
 
 
@@ -73,10 +73,9 @@ def _buf(x, want_dtype, writable=False):
     return a.ctypes.data, a.size, False, a
 
 
-class _FilterBase:
+class _FilterBase(Handle):
     _exec = None
     _host = None
-    _destroy = None
     _length = None
 
     def __init__(self, ctx: Context | None):
@@ -102,17 +101,6 @@ class _FilterBase:
         check(fn(self._h, C.c_void_p(ip), n_in, C.c_void_p(op), n_out, C.byref(c), C.byref(p),
                  C.byref(st)), self.ctx.handle)
         return c.value, p.value, ComputationStatus(st.value)
-
-    def close(self):
-        if getattr(self, "_h", None):
-            type(self)._destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class DecimatingFirFilter(_FilterBase):

@@ -98,6 +98,9 @@ void       *b2s_ctx_stream(b2s_ctx *ctx);
 int32_t     b2s_ctx_sm_count(b2s_ctx *ctx);
 /* number of kernels this context has launched so far (bench.py's gpu_launches) */
 uint64_t    b2s_ctx_launch_count(const b2s_ctx *ctx);
+/* device + pinned bytes currently held by the objects created on this context (plans, sub-plans, rings and their
+   exec-time workspaces); the context's own status word and host-pipeline workspace are not counted */
+uint64_t    b2s_ctx_bytes_held(const b2s_ctx *ctx);
 
 /* device / pinned-host memory (≙ Instance::create_buffer, buffer/vulkan/mod.rs:132) */
 int32_t b2s_malloc(b2s_ctx *ctx, size_t bytes, void **dptr);

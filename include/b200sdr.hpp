@@ -40,6 +40,20 @@ inline void check(int32_t rc, const b2s_ctx *ctx = nullptr) {
     if (rc < 0) throw Error(rc, std::string("libb200sdr: ") + b2s_last_error(ctx));
 }
 
+// Owner of one ABI object: destroyed with its b2s_*_destroy when the owner goes away, so an owner is move-only and a
+// constructor that throws after the create call still frees what it created.
+template <typename T, void (*Destroy)(T *)> struct HandleDeleter { void operator()(T *p) const { Destroy(p); } };
+template <typename T, void (*Destroy)(T *)> using Handle = std::unique_ptr<T, HandleDeleter<T, Destroy>>;
+// The out-parameter of a create call, handed to the Handle at the end of the full expression:
+//     check(b2s_fft_plan_c32(..., out_ptr(plan_)), ...);
+template <typename H> struct OutPtr {
+    H &h;
+    typename H::pointer p = nullptr;
+    ~OutPtr() { h.reset(p); }
+    operator typename H::pointer *() { return &p; }
+};
+template <typename H> OutPtr<H> out_ptr(H &h) { return OutPtr<H>{h}; }
+
 // futuredsp::ComputationStatus (lib.rs:33-45)
 enum class ComputationStatus : int32_t { InsufficientInput = 0, InsufficientOutput = 1, BothSufficient = 2 };
 using FilterResult = std::tuple<size_t, size_t, ComputationStatus>;
@@ -47,30 +61,27 @@ using FilterResult = std::tuple<size_t, size_t, ComputationStatus>;
 // ≙ runtime::buffer::vulkan::Instance (buffer/vulkan/mod.rs:45-153)
 class Instance {
 public:
-    explicit Instance(int device = 0) { check(b2s_ctx_create(device, &ctx_)); }
-    ~Instance() { b2s_ctx_destroy(ctx_); }
-    Instance(const Instance &) = delete;
-    Instance &operator=(const Instance &) = delete;
-    b2s_ctx *get() const { return ctx_; }
-    void sync() const { check(b2s_ctx_sync(ctx_), ctx_); }
-    uint64_t launch_count() const { return b2s_ctx_launch_count(ctx_); }
+    explicit Instance(int device = 0) { check(b2s_ctx_create(device, out_ptr(ctx_))); }
+    b2s_ctx *get() const { return ctx_.get(); }
+    void sync() const { check(b2s_ctx_sync(ctx_.get()), ctx_.get()); }
+    uint64_t launch_count() const { return b2s_ctx_launch_count(ctx_.get()); }
 
     template <typename T> T *device_alloc(size_t items) const {
         void *p = nullptr;
-        check(b2s_malloc(ctx_, items * sizeof(T), &p), ctx_);
+        check(b2s_malloc(ctx_.get(), items * sizeof(T), &p), ctx_.get());
         return static_cast<T *>(p);
     }
-    void device_free(void *p) const { b2s_free(ctx_, p); }
+    void device_free(void *p) const { b2s_free(ctx_.get(), p); }
     template <typename T> void upload(T *dst, const T *src, size_t items) const {
-        check(b2s_memcpy_h2d(ctx_, dst, src, items * sizeof(T)), ctx_);
+        check(b2s_memcpy_h2d(ctx_.get(), dst, src, items * sizeof(T)), ctx_.get());
     }
     template <typename T> void download(T *dst, const T *src, size_t items) const {
-        check(b2s_memcpy_d2h(ctx_, dst, src, items * sizeof(T)), ctx_);
+        check(b2s_memcpy_d2h(ctx_.get(), dst, src, items * sizeof(T)), ctx_.get());
         sync();
     }
 
 private:
-    b2s_ctx *ctx_ = nullptr;
+    Handle<b2s_ctx, b2s_ctx_destroy> ctx_;
 };
 
 template <typename Sample, typename Tap> constexpr b2s_kind kind_of() {
@@ -103,27 +114,26 @@ public:
     DecimatingFirFilter(const Instance &inst, size_t decimation, const std::vector<Tap> &taps, b2s_algo algo = B2S_ALGO_AUTO)
         : inst_(inst) {
         check(b2s_fir_plan(inst.get(), kind_of<Sample, Tap>(), reinterpret_cast<const float *>(taps.data()), taps.size(),
-                           decimation, &plan_), inst.get());
-        if (algo != B2S_ALGO_AUTO) check(b2s_fir_set_algo(plan_, algo), inst.get());
+                           decimation, out_ptr(plan_)), inst.get());
+        if (algo != B2S_ALGO_AUTO) check(b2s_fir_set_algo(plan_.get(), algo), inst.get());
     }
-    ~DecimatingFirFilter() override { b2s_fir_destroy(plan_); }
     FilterResult filter(const Sample *i, size_t n_in, Sample *o, size_t n_out) const override {
         size_t c = 0, p = 0; int32_t st = 0;
-        check(b2s_fir_filter_host(plan_, i, n_in, o, n_out, &c, &p, &st), inst_.get());
+        check(b2s_fir_filter_host(plan_.get(), i, n_in, o, n_out, &c, &p, &st), inst_.get());
         return {c, p, static_cast<ComputationStatus>(st)};
     }
     FilterResult filter_device(const Sample *i, size_t n_in, Sample *o, size_t n_out) const override {
         size_t c = 0, p = 0; int32_t st = 0;
-        check(b2s_fir_exec(plan_, i, n_in, o, n_out, &c, &p, &st), inst_.get());
+        check(b2s_fir_exec(plan_.get(), i, n_in, o, n_out, &c, &p, &st), inst_.get());
         return {c, p, static_cast<ComputationStatus>(st)};
     }
     using Filter<Sample>::filter;
-    size_t length() const override { return b2s_fir_length(plan_); }
-    int algo() const { return b2s_fir_get_algo(plan_); }
+    size_t length() const override { return b2s_fir_length(plan_.get()); }
+    int algo() const { return b2s_fir_get_algo(plan_.get()); }
 
 protected:
     const Instance &inst_;
-    b2s_fir *plan_ = nullptr;
+    Handle<b2s_fir, b2s_fir_destroy> plan_;
 };
 
 template <typename Sample, typename Tap> class FirFilter : public DecimatingFirFilter<Sample, Tap> {
@@ -137,10 +147,9 @@ template <typename Sample> class PolyphaseResamplingFir : public Filter<Sample> 
 public:
     PolyphaseResamplingFir(const Instance &inst, size_t interp, size_t decim, const std::vector<float> &taps)
         : inst_(inst) {
-        check(b2s_resamp_plan(inst.get(), kind_of<Sample, float>(), taps.data(), taps.size(), interp, decim, &plan_),
+        check(b2s_resamp_plan(inst.get(), kind_of<Sample, float>(), taps.data(), taps.size(), interp, decim, out_ptr(plan_)),
               inst.get());
     }
-    ~PolyphaseResamplingFir() override { b2s_resamp_destroy(plan_); }
     FilterResult filter(const Sample *i, size_t n_in, Sample *o, size_t n_out) const override {
         // host slices: stage through device memory (no internal pipeline for this core yet)
         Sample *di = inst_.device_alloc<Sample>(n_in + 1), *dout = inst_.device_alloc<Sample>(n_out + 1);
@@ -152,15 +161,15 @@ public:
     }
     FilterResult filter_device(const Sample *i, size_t n_in, Sample *o, size_t n_out) const override {
         size_t c = 0, p = 0; int32_t st = 0;
-        check(b2s_resamp_exec(plan_, i, n_in, o, n_out, &c, &p, &st), inst_.get());
+        check(b2s_resamp_exec(plan_.get(), i, n_in, o, n_out, &c, &p, &st), inst_.get());
         return {c, p, static_cast<ComputationStatus>(st)};
     }
     using Filter<Sample>::filter;
-    size_t length() const override { return b2s_resamp_length(plan_); }
+    size_t length() const override { return b2s_resamp_length(plan_.get()); }
 
 private:
     const Instance &inst_;
-    b2s_resamp *plan_ = nullptr;
+    Handle<b2s_resamp, b2s_resamp_destroy> plan_;
 };
 
 // ≙ futuredsp::IirFilter (crates/futuredsp/src/iir.rs:33-178), a StatefulFilter: memory and its fill count live in the
@@ -172,21 +181,18 @@ public:
               b2s_algo algo = B2S_ALGO_AUTO)
         : inst_(inst) {
         if constexpr (std::is_same_v<Sample, float>)
-            check(b2s_iir_plan_f32(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), &plan_), inst.get());
+            check(b2s_iir_plan_f32(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), out_ptr(plan_)), inst.get());
         else
-            check(b2s_iir_plan_f64(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), &plan_), inst.get());
+            check(b2s_iir_plan_f64(inst.get(), a_taps.data(), a_taps.size(), b_taps.data(), b_taps.size(), out_ptr(plan_)), inst.get());
         if (algo != B2S_ALGO_AUTO) set_algo(algo);
     }
-    ~IirFilter() { b2s_iir_destroy(plan_); }
-    IirFilter(const IirFilter &) = delete;
-    IirFilter &operator=(const IirFilter &) = delete;
-    void set_algo(b2s_algo algo) { check(b2s_iir_set_algo(plan_, algo), inst_.get()); }
-    int algo() const { return b2s_iir_get_algo(plan_); }
-    size_t length() const { return b2s_iir_length(plan_); }
+    void set_algo(b2s_algo algo) { check(b2s_iir_set_algo(plan_.get(), algo), inst_.get()); }
+    int algo() const { return b2s_iir_get_algo(plan_.get()); }
+    size_t length() const { return b2s_iir_length(plan_.get()); }
     // device slices (asynchronous on the instance's stream)
     FilterResult filter_device(const Sample *i, size_t n_in, Sample *o, size_t n_out) {
         size_t c = 0, p = 0; int32_t st = 0;
-        check(b2s_iir_exec(plan_, i, n_in, o, n_out, &c, &p, &st), inst_.get());
+        check(b2s_iir_exec(plan_.get(), i, n_in, o, n_out, &c, &p, &st), inst_.get());
         return {c, p, static_cast<ComputationStatus>(st)};
     }
     // host slices: staged through device memory
@@ -202,7 +208,7 @@ public:
 
 private:
     const Instance &inst_;
-    b2s_iir *plan_ = nullptr;
+    Handle<b2s_iir, b2s_iir_destroy> plan_;
 };
 
 // ---- firdes (futuredsp::firdes::kaiser, firdes/basic.rs:310-459) ---------------------------------
@@ -229,6 +235,8 @@ template <typename T> class Reader {
 public:
     explicit Reader(const Instance &i) : inst_(i) {}
     ~Reader() { if (d_) inst_.device_free(d_); }
+    Reader(const Reader &) = delete;
+    Reader &operator=(const Reader &) = delete;
     void set(const std::vector<T> &v) {
         if (d_) inst_.device_free(d_);
         d_ = inst_.device_alloc<T>(v.size() + 1); n_ = v.size(); pos_ = 0;
@@ -245,6 +253,8 @@ template <typename T> class Writer {
 public:
     explicit Writer(const Instance &i) : inst_(i) {}
     ~Writer() { if (d_) inst_.device_free(d_); }
+    Writer(const Writer &) = delete;
+    Writer &operator=(const Writer &) = delete;
     void reserve(size_t n) { if (d_) inst_.device_free(d_); d_ = inst_.device_alloc<T>(n + 1); cap_ = n; len_ = 0; }
     T *slice() { return d_ + len_; }
     size_t capacity() const { return cap_ - len_; }
@@ -343,26 +353,23 @@ public:
                  float initial_phase)
         : output(inst), inst_(inst) {
         check(b2s_sigsrc_create(inst.get(), wave, std::is_same_v<T, Complex32> ? 1 : 0, frequency, sample_rate,
-                                amplitude, initial_phase, &h_), inst.get());
+                                amplitude, initial_phase, out_ptr(h_)), inst.get());
     }
-    ~SignalSource() { b2s_sigsrc_destroy(h_); }
-    SignalSource(const SignalSource &) = delete;
-    SignalSource &operator=(const SignalSource &) = delete;
-    void set_amplitude(float amplitude) { check(b2s_sigsrc_set_amplitude(h_, amplitude), inst_.get()); }   // :71-73
+    void set_amplitude(float amplitude) { check(b2s_sigsrc_set_amplitude(h_.get(), amplitude), inst_.get()); }   // :71-73
     // (the next sample's phase, the increment)
     std::pair<FixedPointPhase, FixedPointPhase> phase() const {
         FixedPointPhase v, inc;
-        check(b2s_sigsrc_phase(h_, &v.value, &inc.value), inst_.get());
+        check(b2s_sigsrc_phase(h_.get(), &v.value, &inc.value), inst_.get());
         return {v, inc};
     }
     void work(WorkIo &) {                                                           // mod.rs:88-107
         size_t p = 0;
-        check(b2s_sigsrc_exec(h_, output.slice(), output.capacity(), &p), inst_.get());
+        check(b2s_sigsrc_exec(h_.get(), output.slice(), output.capacity(), &p), inst_.get());
         output.produce(p);
     }
     Writer<T> output;
 private:
-    const Instance &inst_; b2s_sigsrc *h_ = nullptr;
+    const Instance &inst_; Handle<b2s_sigsrc, b2s_sigsrc_destroy> h_;
 };
 
 // ≙ blocks::SignalSourceBuilder (src/blocks/signal_source/mod.rs:110-227)
@@ -406,39 +413,37 @@ public:
     Fft(const Instance &inst, size_t len, FftDirection dir = FftDirection::Forward, bool fft_shift = false,
         bool has_normalize = false, float normalize = 1.0f)
         : input(inst), output(inst), inst_(inst), len_(len) {
-        check(b2s_fft_plan_c32(inst.get(), len, dir == FftDirection::Inverse, fft_shift, has_normalize, normalize, &plan_), inst.get());
+        check(b2s_fft_plan_c32(inst.get(), len, dir == FftDirection::Inverse, fft_shift, has_normalize, normalize, out_ptr(plan_)), inst.get());
     }
-    ~Fft() { b2s_fft_destroy(plan_); }
     void work(WorkIo &io) {                                                        // fft.rs:160-221
         size_t c = 0, p = 0;
-        check(b2s_fft_exec(plan_, input.slice(), input.len(), output.slice(), output.capacity(), &c, &p), inst_.get());
+        check(b2s_fft_exec(plan_.get(), input.slice(), input.len(), output.slice(), output.capacity(), &c, &p), inst_.get());
         input.consume(c); output.produce(p);
         if (input.finished() && c == (c / len_) * len_) io.finished = true;
     }
     Reader<Complex32> input;
     Writer<Complex32> output;
 private:
-    const Instance &inst_; size_t len_; b2s_fft *plan_ = nullptr;
+    const Instance &inst_; size_t len_; Handle<b2s_fft, b2s_fft_destroy> plan_;
 };
 
 // ≙ blocks::Apply (src/blocks/apply.rs:100-131) for the device op catalogue
 template <typename A, typename B> class Apply {
 public:
     Apply(const Instance &inst, b2s_op op, float param = 1.0f) : input(inst), output(inst), inst_(inst) {
-        check(b2s_apply_create(inst.get(), op, param, &h_), inst.get());
+        check(b2s_apply_create(inst.get(), op, param, out_ptr(h_)), inst.get());
     }
-    ~Apply() { b2s_apply_destroy(h_); }
     void work(WorkIo &io) {
         const size_t i_len = input.len();
         size_t c = 0, p = 0;
-        check(b2s_apply_exec(h_, input.slice(), i_len, output.slice(), output.capacity(), &c, &p), inst_.get());
+        check(b2s_apply_exec(h_.get(), input.slice(), i_len, output.slice(), output.capacity(), &c, &p), inst_.get());
         input.consume(c); output.produce(p);
         if (input.finished() && c == i_len) io.finished = true;                     // apply.rs:126-128
     }
     Reader<A> input;
     Writer<B> output;
 private:
-    const Instance &inst_; b2s_apply *h_ = nullptr;
+    const Instance &inst_; Handle<b2s_apply, b2s_apply_destroy> h_;
 };
 
 // ≙ blocks::PfbArbResampler (src/blocks/pfb/arb_resampler.rs:72-231)
@@ -446,13 +451,12 @@ class PfbArbResampler {
 public:
     PfbArbResampler(const Instance &inst, float rate, const std::vector<float> &taps, size_t num_filters)
         : input(inst), output(inst), inst_(inst) {
-        check(b2s_pfbarb_plan_c32(inst.get(), taps.data(), taps.size(), num_filters, rate, &h_), inst.get());
+        check(b2s_pfbarb_plan_c32(inst.get(), taps.data(), taps.size(), num_filters, rate, out_ptr(h_)), inst.get());
     }
-    ~PfbArbResampler() { b2s_pfbarb_destroy(h_); }
     void work(WorkIo &io) {
         size_t c = 0, p = 0; int32_t again = 0;
         const size_t n = input.len();
-        check(b2s_pfbarb_exec(h_, input.slice(), n, output.slice(), output.capacity(), &c, &p, &again), inst_.get());
+        check(b2s_pfbarb_exec(h_.get(), input.slice(), n, output.slice(), output.capacity(), &c, &p, &again), inst_.get());
         input.consume(c); output.produce(p);
         if (again) io.call_again = true;
         else if (n - c == 0 && input.finished()) io.finished = true;
@@ -460,24 +464,22 @@ public:
     Reader<Complex32> input;
     Writer<Complex32> output;
 private:
-    const Instance &inst_; b2s_pfbarb *h_ = nullptr;
+    const Instance &inst_; Handle<b2s_pfbarb, b2s_pfbarb_destroy> h_;
 };
 
 // ≙ futuredsp::Rotator (crates/futuredsp/src/rotator.rs:13-48): phase recurrence replayed bit for bit
 class Rotator {
 public:
-    Rotator(const Instance &inst, float phase_incr) : inst_(inst) { check(b2s_rotator_create(inst.get(), phase_incr, &h_), inst.get()); }
-    ~Rotator() { b2s_rotator_destroy(h_); }
-    Rotator(const Rotator &) = delete;
+    Rotator(const Instance &inst, float phase_incr) : inst_(inst) { check(b2s_rotator_create(inst.get(), phase_incr, out_ptr(h_)), inst.get()); }
     // Rotator::rotate (:32-47) on device slices; d_in == d_out is rotate_inplace (:24-29)
     std::pair<size_t, ComputationStatus> rotate_device(const Complex32 *d_in, size_t n_in, Complex32 *d_out, size_t n_out) {
         size_t n = 0; int32_t st = 0;
-        check(b2s_rotator_exec(h_, d_in, n_in, d_out, n_out, &n, &st), inst_.get());
+        check(b2s_rotator_exec(h_.get(), d_in, n_in, d_out, n_out, &n, &st), inst_.get());
         return {n, static_cast<ComputationStatus>(st)};
     }
-    void reset() { check(b2s_rotator_reset(h_), inst_.get()); }
+    void reset() { check(b2s_rotator_reset(h_.get()), inst_.get()); }
 private:
-    const Instance &inst_; b2s_rotator *h_ = nullptr;
+    const Instance &inst_; Handle<b2s_rotator, b2s_rotator_destroy> h_;
 };
 
 // ≙ blocks::XlatingFir (src/blocks/xlating_fir.rs:22-126): band-pass complex taps (:80-86), decimating FIR,
@@ -523,20 +525,19 @@ class MovingAvg {
 public:
     MovingAvg(const Instance &inst, size_t width, float decay_factor, size_t history_size)
         : input(inst), output(inst), inst_(inst), width_(width) {
-        check(b2s_mavg_create(inst.get(), width, decay_factor, history_size, &h_), inst.get());   // asserts of :58-61 -> EINVAL
+        check(b2s_mavg_create(inst.get(), width, decay_factor, history_size, out_ptr(h_)), inst.get());   // asserts of :58-61 -> EINVAL
     }
-    ~MovingAvg() { b2s_mavg_destroy(h_); }
     void work(WorkIo &io) {                                                        // moving_avg.rs:72-115
         const size_t n = input.len();
         size_t c = 0, p = 0;
-        check(b2s_mavg_exec(h_, input.slice(), n, output.slice(), output.capacity(), &c, &p), inst_.get());
+        check(b2s_mavg_exec(h_.get(), input.slice(), n, output.slice(), output.capacity(), &c, &p), inst_.get());
         if (input.finished() && c / width_ == n / width_) io.finished = true;       // :106-108
         input.consume(c); output.produce(p);
     }
     Reader<float> input;
     Writer<float> output;
 private:
-    const Instance &inst_; size_t width_; b2s_mavg *h_ = nullptr;
+    const Instance &inst_; size_t width_; Handle<b2s_mavg, b2s_mavg_destroy> h_;
 };
 
 // The spectrum flowgraph's compute chain as one block: Fft::with_options(n, Forward, fft_shift, None) ->
@@ -547,20 +548,19 @@ public:
     SpectrumPipe(const Instance &inst, size_t n, float decay_factor, size_t history_size, bool fft_shift = true,
                  float log10_scale = 0.0f)
         : input(inst), output(inst), inst_(inst), n_(n) {
-        check(b2s_spectrum_plan(inst.get(), n, fft_shift ? 1 : 0, decay_factor, history_size, log10_scale, &h_), inst.get());
+        check(b2s_spectrum_plan(inst.get(), n, fft_shift ? 1 : 0, decay_factor, history_size, log10_scale, out_ptr(h_)), inst.get());
     }
-    ~SpectrumPipe() { b2s_spectrum_destroy(h_); }
     void work(WorkIo &io) {
         const size_t n = input.len();
         size_t c = 0, p = 0;
-        check(b2s_spectrum_exec(h_, input.slice(), n, output.slice(), output.capacity(), &c, &p), inst_.get());
+        check(b2s_spectrum_exec(h_.get(), input.slice(), n, output.slice(), output.capacity(), &c, &p), inst_.get());
         if (input.finished() && c / n_ == n / n_) io.finished = true;               // moving_avg.rs:106-108
         input.consume(c); output.produce(p);
     }
     Reader<Complex32> input;
     Writer<float> output;
 private:
-    const Instance &inst_; size_t n_; b2s_spectrum *h_ = nullptr;
+    const Instance &inst_; size_t n_; Handle<b2s_spectrum, b2s_spectrum_destroy> h_;
 };
 
 // ≙ runtime::mocker::Mocker (mocker.rs:33-190): run one block without a scheduler
