@@ -6,66 +6,28 @@
 // after each group of D = N / oversample_rate pushes, arm i (taps[i::N]) filters window
 // (base_index + i + 1) % N into fft_buf[that window], an un-normalised inverse FFT over the N
 // buffers de-spins, and element ch goes to output stream ch.
-//   * start-up: windows fill through WindowBuffer::push, which scatters the first T samples of a
-//     window (window_buffer.rs:24-32), and the call in which the last window fills returns
+//   * start-up: the windows fill through the shared window buffer of pfb_common.cuh (sample c of the
+//     stream goes to window N-1 - c mod N), and the call in which the last window fills returns
 //     WITHOUT consuming (channelizer.rs:170-180), so those samples are pushed a second time.
-//     Both are reproduced: a one-thread kernel replays the pushes on the data, the host mirrors
-//     the bookkeeping (it is data-independent).
 //   * steady state is closed-form: one thread per (output vector o, window b) gathers the T newest
 //     samples of its phase (history buffer + this call's input) and dots them with its arm; the
 //     N-point inverse FFT is the batched FFT kernel of fft.cu (any N: radix or Bluestein), a
 //     transposing store writes channel-major output streams.
-#include <cmath>
 #include <cstdlib>
 
-#include "common.cuh"
-#include "fft_common.cuh"
-
-const float2 *b2s_fft_twiddles(const b2s_fft *p);   // fft.cu
-int b2s_fft_log2n(const b2s_fft *p);
+#include "pfb_common.cuh"
 
 struct b2s_chan {
     b2s_ctx *ctx = nullptr;
     size_t N = 0, D = 0, T = 0;
-    Buf<float> d_arms;              // [T][N] (tap-major): d_arms[j*N + i] = arm_i[j] = taps[i + j*N] (utilities.rs:9-19;
-                                    // newest sample <-> j = 0).  Tap-major so that adjacent windows -- which meet
-                                    // adjacent arms -- read adjacent floats (arm-major cost 32 L1 lines per warp load)
-    Buf<float2> d_circ;             // [N][2T] circular windows (used while filling)
-    Buf<float2> d_hist;             // [N][T] windows in time order once filled
-    Buf<int> d_wstate;              // [2N]: start_idx[N], missing[N]
-    std::vector<int> start_idx, missing;   // host mirror of the WindowBuffer bookkeeping
+    PfbBankTaps taps;               // arm i meets window (base_index + i + 1) % N
+    PfbWindows win;                 // N windows, mirrored: window base_index receives the next sample
     size_t base_index = 0;
-    bool all_filled = false;
     PlanPtr<b2s_fft> ifft;
     Buf<float2> d_tmp;              // two halves: bank outputs, spectra
-    Buf<float> d_arms_pad;          // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
-    int tpad = 0;
 };
 
 namespace {
-
-__global__ void chan_fill_kernel(const float2 *__restrict__ in, float2 *circ, int *wstate, int N, int T,
-                                 int base_index, int count) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    int *start = wstate, *missing = wstate + N;
-    for (int c = 0; c < count; c++) {
-        const int w = base_index;
-        int idx = (start[w] - missing[w]) % T;
-        if (idx < 0) idx += T;
-        float2 *cw = circ + (size_t)w * 2 * T;
-        cw[idx] = in[c]; cw[idx + T] = in[c];
-        if (missing[w] > 0) missing[w]--;
-        start[w] = (start[w] + 1) % T;
-        base_index = base_index == 0 ? N - 1 : base_index - 1;
-    }
-}
-
-__global__ void chan_hist_from_circ(const float2 *__restrict__ circ, const int *__restrict__ wstate, float2 *hist,
-                                    int N, int T) {
-    const int w = blockIdx.x;
-    const int s = wstate[w];
-    for (int t = threadIdx.x; t < T; t += blockDim.x) hist[(size_t)w * T + t] = circ[(size_t)w * 2 * T + s + t];
-}
 
 // Critically sampled steady state (D == N, the window already holds T samples of this call): every output
 // pushes exactly one new sample into every window and the window keeps meeting the same arm, so the T samples
@@ -176,37 +138,6 @@ __global__ void chan_bank_kernel(const float2 *__restrict__ in, const float2 *__
     }
 }
 
-__global__ void chan_hist_update(float2 *hist, const float2 *__restrict__ in, int N, int T, int base0, long long npush) {
-    extern __shared__ float2 tmp[];
-    const int b = blockIdx.x;
-    const int r = ((base0 - b) % N + N) % N;
-    long long c_new = -1; int m = 0;
-    if (npush - 1 >= r) { c_new = r + ((npush - 1 - r) / N) * N; m = (int)((c_new - r) / N) + 1; }
-    for (int t = threadIdx.x; t < T; t += blockDim.x) {
-        const int j = T - 1 - t;                                       // new hist[t] = j-th newest
-        tmp[t] = (j < m) ? in[c_new - (long long)j * N] : hist[(size_t)b * T + (T - 1 - (j - m))];
-    }
-    __syncthreads();
-    for (int t = threadIdx.x; t < T; t += blockDim.x) hist[(size_t)b * T + t] = tmp[t];
-}
-
-// out[ch * stride + o] = spec[o * N + ch]
-__global__ void chan_transpose_kernel(const float2 *__restrict__ spec, float2 *__restrict__ out, int N, long long nprod,
-                                      long long stride) {
-    __shared__ float2 tile[32][33];
-    const long long o0 = (long long)blockIdx.x * 32;
-    const int c0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const long long o = o0 + i; const int ch = c0 + threadIdx.x;
-        if (o < nprod && ch < N) tile[i][threadIdx.x] = spec[o * N + ch];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int ch = c0 + i; const long long o = o0 + threadIdx.x;
-        if (o < nprod && ch < N) out[(long long)ch * stride + o] = tile[threadIdx.x][i];
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // FUSED steady state (critically sampled, N a power of two <= 256, T <= 32): FIR bank + N-point inverse FFT +
 // channel-major store in ONE kernel -- 8 B/sample in, 8 B/sample out, nothing in between touches HBM (the three
@@ -298,18 +229,8 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
         // ---- B: FIR bank (every sample of the column is loaded once and multiplied into all outputs that contain it)
         {
             float2 acc[RL];
-#pragma unroll
-            for (int u = 0; u < RL; u++) acc[u] = make_float2(0.f, 0.f);
-            const float2 *col = X + (size_t)(run * RL) * N + r;   // tile row (run*RL + k) <-> sample row o_run - TPAD + 1 + k
-#pragma unroll
-            for (int k = 0; k < RL + TPAD - 1; k++) {
-                const float2 x = col[(size_t)k * N];
-#pragma unroll
-                for (int u = 0; u < RL; u++) {
-                    const int j = u + TPAD - 1 - k;          // output u sees this row as its j-th newest sample
-                    if (j >= 0 && j < TPAD) mac(acc[u], x, tap[j]);
-                }
-            }
+            // tile row (run*RL + k) <-> sample row o_run - TPAD + 1 + k
+            pfb_bank_column<N, RL, TPAD>(X + (size_t)(run * RL) * N + r, tap, acc);
 #pragma unroll
             for (int u = 0; u < RL; u++)                      // conjugated: the inverse transform is conj(FFT(conj(.)))
                 V[(size_t)(run * RL + u) * NP + pad(b)] = make_float2(acc[u].x, -acc[u].y);
@@ -344,38 +265,16 @@ template <int LOG2N, int TPAD>
 int32_t chan_fused_launch(b2s_chan *c, const float2 *in, float2 *out, long long o_first, long long nprod, long long out_stride) {
     constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = chan_fused_smem<LOG2N, TPAD>();
-    auto kern = chan_fused_kernel<LOG2N, TPAD>;
-    static PerDeviceOnce optin;
     if (ntiles_overflow(nprod, o_first, OB)) return b2s_fail(c->ctx, B2S_EUNSUPPORTED, "channelizer: too many output vectors in one call");
-    if (smem > 48 * 1024 && optin.need(c->ctx->device)) {
-        B2S_CUDA(c->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        optin.done(c->ctx->device);
-    }
+    constexpr auto kern = chan_fused_kernel<LOG2N, TPAD>;
+    int resident = 1;
+    B2S_TRY(smem_optin<kern>(c->ctx, smem, 256, &resident));
     const size_t ntiles = ceil_div((size_t)(nprod - o_first), (size_t)OB);
-    static int resident = 0;                                  // CTAs per SM of this instantiation
-    if (!resident) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, 256, smem) != cudaSuccess || resident < 1) { cudaGetLastError(); resident = 1; }
-    }
     const unsigned grid = (unsigned)std::min<size_t>(ntiles, (size_t)c->ctx->sm_count * resident);
-    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->d_arms_pad.get(), b2s_fft_twiddles(c->ifft.get()), out, (int)c->base_index, o_first,
+    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->taps.arms_pad.get(), b2s_fft_twiddles(c->ifft.get()), out, (int)c->base_index, o_first,
                                              nprod, out_stride, (int)ntiles);
     B2S_CHECK_LAUNCH(c->ctx);
     return B2S_OK;
-}
-
-template <int TPAD>
-int32_t chan_fused_dispatch(b2s_chan *c, int log2n, const float2 *in, float2 *out, long long o_first, long long nprod,
-                            long long out_stride) {
-    return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN,
-                                  [&](auto L) { return chan_fused_launch<L, TPAD>(c, in, out, o_first, nprod, out_stride); });
-}
-
-// TPAD (8 / 16 / 32) the fused kernel would use for this plan, 0 if the plan is outside its shapes
-int chan_fused_tpad(const b2s_chan *c) {
-    const int l2 = b2s_fft_log2n(c->ifft.get());
-    if (getenv("B2S_CHAN_NO_FUSED")) return 0;
-    if (l2 < 2 || l2 > 8 || c->D != c->N || c->T > 32) return 0;
-    return c->T <= 8 ? 8 : (c->T <= 16 ? 16 : 32);
 }
 
 }  // namespace
@@ -395,29 +294,17 @@ int32_t b2s_chan_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps, 
     PlanPtr<b2s_chan> c(new b2s_chan());
     c->ctx = ctx; c->N = num_channels;
     c->D = (size_t)((float)num_channels / oversample_rate);                      // channelizer.rs:106
-    const size_t N = c->N, T = (size_t)std::ceil((float)ntaps / (float)N);       // utilities.rs:9
+    const size_t N = c->N;
+    std::vector<float> arms;
+    const size_t T = pfb_partition(taps, ntaps, N, arms);
     c->T = T;
-    std::vector<float> arms(N * T, 0.0f);
-    for (size_t i = 0; i < N; i++) { size_t j = 0; for (size_t idx = i; idx < ntaps; idx += N) arms[(j++) * N + i] = taps[idx]; }
-    c->start_idx.assign(N, 0); c->missing.assign(N, (int)T);
     c->base_index = N - 1;
     b2s_fft *ifft = nullptr;
     B2S_TRY(b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &ifft));                    // plan_fft(n, Inverse) (:114)
     c->ifft.reset(ifft);
-    std::vector<int> ws(2 * N);
-    for (size_t i = 0; i < N; i++) { ws[i] = 0; ws[N + i] = (int)T; }
-    B2S_TRY(c->d_arms.upload(ctx, arms.data(), arms.size(), "channelizer arms"));
-    B2S_TRY(c->d_circ.alloc(ctx, N * 2 * T, "channelizer windows"));
-    B2S_TRY(c->d_hist.alloc(ctx, N * T, "channelizer history"));
-    B2S_TRY(c->d_wstate.upload(ctx, ws.data(), ws.size(), "channelizer window state"));
-    B2S_CUDA(ctx, cudaMemsetAsync(c->d_circ.get(), 0, N * 2 * T * sizeof(float2), ctx->stream));
-    c->tpad = chan_fused_tpad(c.get());
-    std::vector<float> apad;
-    if (c->tpad) {
-        apad.assign((size_t)c->tpad * N, 0.0f);                                  // taps beyond T are zero (older samples)
-        std::copy(arms.begin(), arms.end(), apad.begin());
-        B2S_TRY(c->d_arms_pad.upload(ctx, apad.data(), apad.size(), "channelizer padded arms"));
-    }
+    const int tpad = getenv("B2S_CHAN_NO_FUSED") || c->D != N ? 0 : pfb_fused_tpad(b2s_fft_log2n(ifft), T);
+    B2S_TRY(c->taps.upload(ctx, arms, N, T, tpad, "channelizer arms"));
+    B2S_TRY(c->win.init(ctx, (int)N, (int)T, true, "channelizer windows"));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *out = c.release();
     return B2S_OK;
@@ -438,27 +325,12 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     DeviceGuard g(ctx->device);
     const int N = (int)c->N, T = (int)c->T, D = (int)c->D;
     const float2 *in = (const float2 *)d_in;
-    if (!c->all_filled) {
-        // host mirror of the push bookkeeping decides how many samples this call pushes
-        size_t cnt = 0;
-        size_t base = c->base_index;
-        auto all_filled = [&]() { for (int m : c->missing) if (m) return false; return true; };
-        while (!all_filled() && cnt < n_in) {
-            if (c->missing[base] > 0) c->missing[base]--;
-            c->start_idx[base] = (c->start_idx[base] + 1) % T;
-            base = base == 0 ? (size_t)N - 1 : base - 1;
-            cnt++;
-        }
-        if (cnt) {
-            if (!d_in) return b2s_fail(ctx, B2S_EINVAL, "b2s_chan_exec: NULL buffer");
-            chan_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, c->d_circ.get(), c->d_wstate.get(), N, T, (int)c->base_index, (int)cnt);
-            B2S_CHECK_LAUNCH(ctx);
-        }
-        c->base_index = base;
-        if (!all_filled()) { *consumed = cnt; return B2S_OK; }               // input exhausted first (:165-170)
-        c->all_filled = true;
-        chan_hist_from_circ<<<N, 64, 0, ctx->stream>>>(c->d_circ.get(), c->d_wstate.get(), c->d_hist.get(), N, T);
-        B2S_CHECK_LAUNCH(ctx);
+    if (!c->win.full()) {
+        const size_t cnt = std::min(n_in, c->win.missing());
+        if (cnt && !d_in) return b2s_fail(ctx, B2S_EINVAL, "b2s_chan_exec: NULL buffer");
+        B2S_TRY(c->win.push(ctx, in, cnt));
+        c->base_index = (size_t)((((long long)c->base_index - (long long)cnt) % N + N) % N);
+        if (!c->win.full()) { *consumed = cnt; return B2S_OK; }              // input exhausted first (:165-170)
         if (n_in >= (size_t)D) *call_again = 1;                                // :176-177; NB nothing is consumed here
         return B2S_OK;
     }
@@ -468,15 +340,13 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     if (!d_in || !d_out) return b2s_fail(ctx, B2S_EINVAL, "b2s_chan_exec: NULL buffer");
     // the first T-1 output vectors of a call still reach into the previous call's history: generic path; the rest
     // (windows entirely inside this call's input) go through the fused kernel
-    const bool fused_ok = c->tpad && (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;      // the tile copy uses 16-byte loads
+    const bool fused_ok = c->taps.tpad && (reinterpret_cast<uintptr_t>(d_in) & 15) == 0;      // the tile copy uses 16-byte loads
     const size_t n_generic = fused_ok ? std::min<size_t>(nprod, (size_t)T - 1) : nprod;
     NvtxRange nvtx("b2s_chan_exec");
     if (n_generic < nprod) {
-        int32_t rc = B2S_EAGAIN;
-        const int l2 = b2s_fft_log2n(c->ifft.get());
-        if (c->tpad == 8) rc = chan_fused_dispatch<8>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
-        else if (c->tpad == 16) rc = chan_fused_dispatch<16>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
-        else if (c->tpad == 32) rc = chan_fused_dispatch<32>(c, l2, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
+        const int32_t rc = pfb_fused_dispatch(b2s_fft_log2n(c->ifft.get()), c->taps.tpad, [&](auto L, auto P) {
+            return chan_fused_launch<L, P>(c, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
+        });
         if (rc != B2S_OK) return rc == B2S_EAGAIN ? b2s_fail(ctx, B2S_ESTATE, "channelizer: fused shape mismatch") : rc;
     }
     const size_t nprod_all = nprod;
@@ -493,21 +363,18 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
         const size_t want_y = std::max<size_t>(1, (size_t)ctx->sm_count * 16 / gx);
         const size_t orun = std::max<size_t>(32, ceil_div(nprod, want_y));
         dim3 grid(gx, (unsigned)ceil_div(nprod, orun));
-        chan_bank_kernel<<<grid, th, 0, ctx->stream>>>(in, c->d_hist.get(), c->d_arms.get(), bank, N, D, T, (int)c->base_index,
+        chan_bank_kernel<<<grid, th, 0, ctx->stream>>>(in, c->win.hist.get(), c->taps.arms.get(), bank, N, D, T, (int)c->base_index,
                                                        (long long)nprod, (int)orun);
     }
     B2S_CHECK_LAUNCH(ctx);
     size_t fc = 0, fp = 0;
     int32_t rc = b2s_fft_exec(c->ifft.get(), bank, items, spec, items, &fc, &fp);
     if (rc != B2S_OK) return rc;
-    dim3 tg((unsigned)ceil_div(nprod, (size_t)32), (unsigned)ceil_div((size_t)N, (size_t)32));
-    chan_transpose_kernel<<<tg, dim3(32, 8), 0, ctx->stream>>>(spec, (float2 *)d_out, N, (long long)nprod, (long long)out_stride);
-    B2S_CHECK_LAUNCH(ctx);
+    B2S_TRY(pfb_transpose(ctx, spec, (float2 *)d_out, nprod, N, N, out_stride));   // out[ch * out_stride + o] = spec[o * N + ch]
     }
     nprod = nprod_all;
     const long long npush = (long long)nprod * D;
-    chan_hist_update<<<N, 64, T * sizeof(float2), ctx->stream>>>(c->d_hist.get(), in, N, T, (int)c->base_index, npush);
-    B2S_CHECK_LAUNCH(ctx);
+    B2S_TRY(c->win.slide(ctx, in, N - 1 - (long long)c->base_index, npush));   // sample 0 goes to window base_index
     c->base_index = (size_t)((((long long)c->base_index - npush) % N + N) % N);
     *consumed = (size_t)npush; *produced_per_channel = nprod;
     return B2S_OK;

@@ -39,8 +39,8 @@ struct b2s_ctx {
     std::atomic<uint64_t> bytes_held{0};
 };
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per DEVICE and a process may hold contexts on several: a
-// `static PerDeviceOnce` next to each kernel instantiation remembers which devices have been opted in.
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per DEVICE and a process may hold contexts on several: the
+// PerDeviceOnce of each kernel in smem_optin (below) remembers which devices have been opted in.
 struct PerDeviceOnce {
     std::atomic<uint64_t> mask{0};
     bool need(int dev) const { return ((mask.load(std::memory_order_acquire) >> (dev & 63)) & 1ull) == 0; }
@@ -102,6 +102,29 @@ struct DeviceGuard {
         const int32_t rc__ = (expr);                                                          \
         if (rc__ != B2S_OK) return rc__;                                                      \
     } while (0)
+
+// Opt kernel K in to `bytes` of dynamic shared memory on the context's device, once per device; with `resident`, also
+// report how many CTAs of K at `threads` threads and `bytes` fit one SM (queried once per device, at least 1).  Every
+// call site of one K passes the same figures.
+template <auto K>
+int32_t smem_optin(b2s_ctx *ctx, size_t bytes, int threads = 0, int *resident = nullptr) {
+    static PerDeviceOnce optin;
+    static std::atomic<int> ctas[64];
+    if (bytes > 48 * 1024 && optin.need(ctx->device)) {
+        B2S_CUDA(ctx, cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        optin.done(ctx->device);
+    }
+    if (resident) {
+        std::atomic<int> &n = ctas[ctx->device & 63];
+        int r = n.load(std::memory_order_relaxed);
+        if (!r) {
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r, K, threads, bytes) != cudaSuccess || r < 1) { cudaGetLastError(); r = 1; }
+            n.store(r, std::memory_order_relaxed);
+        }
+        *resident = r;
+    }
+    return B2S_OK;
+}
 
 // Ownership: every buffer and sub-plan an object allocates is freed by its owner's destructor.  A Buf owns device
 // (or pinned host) memory and counts it in its context's bytes_held; a plan under construction lives in a PlanPtr

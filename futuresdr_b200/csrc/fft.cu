@@ -82,14 +82,8 @@ int32_t launch_fft(b2s_fft *p, const FftArgs &a, cudaStream_t stream) {
     constexpr int TH = fft_cta_threads(LOG2N);
     constexpr FftGeom G = fft_geom(LOG2N, TH);
     constexpr size_t smem = (size_t)G.fpb * G.np * sizeof(float2);
-    auto kern = fft_kernel<LOG2N, TH, fft_min_blocks(LOG2N)>;
-    if (smem > 48 * 1024) {
-        static PerDeviceOnce optin;              // per template instantiation, per device
-        if (optin.need(p->ctx->device)) {
-            B2S_CUDA(p->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            optin.done(p->ctx->device);
-        }
-    }
+    constexpr auto kern = fft_kernel<LOG2N, TH, fft_min_blocks(LOG2N)>;
+    B2S_TRY(smem_optin<kern>(p->ctx, smem));
     const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)G.fpb);
     kern<<<grid, TH, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);
@@ -153,14 +147,8 @@ template <int LOG2M>
 int32_t launch_bluestein(b2s_fft *p, const BsArgs &a, cudaStream_t stream) {
     constexpr FftGeom G = fft_geom(LOG2M, kFftThreads);
     constexpr size_t smem = (size_t)G.fpb * G.np * sizeof(float2);
-    auto kern = bluestein_kernel<LOG2M>;
-    if (smem > 48 * 1024) {
-        static PerDeviceOnce optin;              // per template instantiation, per device
-        if (optin.need(p->ctx->device)) {
-            B2S_CUDA(p->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            optin.done(p->ctx->device);
-        }
-    }
+    constexpr auto kern = bluestein_kernel<LOG2M>;
+    B2S_TRY(smem_optin<kern>(p->ctx, smem));
     const unsigned grid = (unsigned)ceil_div((size_t)a.nfft, (size_t)G.fpb);
     kern<<<grid, kFftThreads, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);

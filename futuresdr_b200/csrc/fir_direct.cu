@@ -391,12 +391,8 @@ SlideLayout slide_layout(size_t L, size_t M, size_t Upad, size_t isz, size_t tsz
 template <typename S, typename T, int LT>
 int32_t slide_launch(b2s_ctx *ctx, const T *d_tab, int L, int M, int Upad, const SlideLayout &lay, const void *d_in,
                      size_t n_in, void *d_out, size_t n_out, cudaStream_t stream) {
-    auto kern = fir_direct_kernel<S, T, LT>;
-    static PerDeviceOnce optin;                  // per template instantiation, per device
-    if (optin.need(ctx->device)) {
-        B2S_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax));
-        optin.done(ctx->device);
-    }
+    constexpr auto kern = fir_direct_kernel<S, T, LT>;
+    B2S_TRY(smem_optin<kern>(ctx, kSmemMax));
     const int vec_ok = ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) & 15) == 0;
     const unsigned grid = (unsigned)ceil_div(n_out, (size_t)L * kTK);
     kern<<<grid, kThreads, lay.smem, stream>>>((const S *)d_in, (S *)d_out, d_tab, M, Upad, lay.pitch,

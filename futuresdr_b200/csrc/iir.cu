@@ -414,12 +414,8 @@ int32_t scan_launch(b2s_iir *f, const void *d_in, void *d_out, size_t n) {
 
 template <typename T>
 int32_t seq_launch(b2s_iir *f, const void *d_in, void *d_out, size_t n) {
-    static PerDeviceOnce once;
     constexpr size_t max_smem = (kSeqMaxTaps + 2 * kSeqMaxTaps + kSeqTile + kSeqMaxTaps - 1 + kSeqTile) * sizeof(T);
-    if (once.need(f->ctx->device)) {
-        B2S_CUDA(f->ctx, cudaFuncSetAttribute(iir_seq_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
-        once.done(f->ctx->device);
-    }
+    B2S_TRY(smem_optin<iir_seq_kernel<T>>(f->ctx, max_smem));
     const size_t smem = (f->n_b + 2 * f->n_a + kSeqTile + f->n_b - 1 + kSeqTile) * sizeof(T);
     iir_seq_kernel<T><<<1, kSeqThreads, smem, f->ctx->stream>>>((const T *)d_in, (T *)d_out, (long long)n,
                                                                (const T *)f->d_a.get(), (int)f->n_a, (const T *)f->d_b.get(),

@@ -19,14 +19,12 @@
 // is uploaded once (16 bytes per record), and a call only needs its position in the cycle: no per-call host replay,
 // no per-call record upload, output counts still bit-identical.  Rates whose trajectory has a pre-period or a cycle
 // longer than 2^25 samples keep the per-call host replay above.
-// The input history (the reference's WindowBuffer) is a T-sample device buffer carried between
-// calls, including the reference's start-up behaviour: while the window fills, push() writes
-// sample j at slot (start_idx - missing) mod T (window_buffer.rs:24-32), which scatters the
-// first T samples (it is not a plain append); this is reproduced so the first outputs match.
+// The input history (the reference's WindowBuffer) is the shared window buffer of pfb_common.cuh
+// with one window, carried between calls, including the scattered start-up fill.
 #include <cmath>
 #include <cstdlib>
 
-#include "common.cuh"
+#include "pfb_common.cuh"
 
 namespace {
 constexpr int kSB = 32;            // input samples per recorded sub-block
@@ -48,10 +46,7 @@ struct b2s_pfbarb {
     float rate = 1.f, delay = 1.f;
     Buf<float2> d_arms;            // [num_filters][T] PAIRS (arm_b[T-1-j], arm_{(b+1) % N}[T-1-j]), time-reversed: an output blends
                                    // arm b and its successor (arm 0 after the last one: the Boundary state), one 8-byte load per tap
-    Buf<float2> d_circ;            // 2*T, the reference's circular buffer (only used while filling)
-    Buf<float2> d_hist;            // T samples of history once filled
-    // WindowBuffer bookkeeping (host)
-    size_t start_idx = 0, missing = 0;
+    PfbWindows win;                // one window of T samples: the input history
     // State (host): arb_resampler.rs:40-52
     float tau = 0.f, bf = 0.f, mu = 0.f;
     size_t base_index = 0;
@@ -67,35 +62,6 @@ struct b2s_pfbarb {
 };
 
 namespace {
-
-// ---- window fill: the reference's push() while num_samples_missing > 0 ------------------------
-__global__ void pfb_fill_kernel(const float2 *__restrict__ in, float2 *circ, int L, int start_idx, int missing,
-                                int count) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    for (int c = 0; c < count; c++) {
-        int idx = (start_idx - missing) % L;
-        if (idx < 0) idx += L;                                   // rem_euclid
-        circ[idx] = in[c];
-        circ[idx + L] = in[c];
-        if (missing > 0) missing--;
-        start_idx = (start_idx + 1) % L;
-    }
-}
-
-__global__ void pfb_hist_from_circ(const float2 *__restrict__ circ, float2 *hist, int L, int start_idx) {
-    for (int j = threadIdx.x; j < L; j += blockDim.x) hist[j] = circ[start_idx + j];
-}
-
-// hist <- last L samples of [hist | in[0..n))
-__global__ void pfb_hist_update(float2 *hist, const float2 *__restrict__ in, int L, long long n) {
-    extern __shared__ float2 tmp[];
-    for (int j = threadIdx.x; j < L; j += blockDim.x) {
-        const long long idx = n + j;                             // position in [hist | in]
-        tmp[j] = (idx < L) ? hist[idx] : in[idx - L];
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < L; j += blockDim.x) hist[j] = tmp[j];
-}
 
 __device__ __forceinline__ float2 pfb_x(const float2 *__restrict__ hist, const float2 *__restrict__ in, int L,
                                         long long idx) {
@@ -385,23 +351,18 @@ int32_t b2s_pfbarb_plan_c32(b2s_ctx *ctx, const float *taps, size_t ntaps, size_
     PlanPtr<b2s_pfbarb> p(new b2s_pfbarb());
     p->ctx = ctx; p->num_filters = num_filters; p->ntaps = ntaps; p->rate = rate;
     p->delay = 1.0f / rate;
-    // partition_filter_taps (utilities.rs:9-19): T = ceil(len as f32 / n as f32); arm i = taps[i::n] zero padded
-    const size_t T = (size_t)std::ceil((float)ntaps / (float)num_filters);
+    std::vector<float> arms;
+    const size_t T = pfb_partition(taps, ntaps, num_filters, arms);
     p->T = T;
-    std::vector<float> arms(num_filters * T, 0.0f);
-    for (size_t i = 0; i < num_filters; i++) {
-        size_t j = 0;
-        for (size_t idx = i; idx < ntaps; idx += num_filters, j++) arms[i * T + (T - 1 - j)] = taps[idx];   // reversed
-    }
-    std::vector<float2> pairs(num_filters * T);
+    std::vector<float2> pairs(num_filters * T);      // time-reversed
     for (size_t b = 0; b < num_filters; b++)
-        for (size_t j = 0; j < T; j++) pairs[b * T + j] = make_float2(arms[b * T + j], arms[((b + 1) % num_filters) * T + j]);
+        for (size_t j = 0; j < T; j++)
+            pairs[b * T + j] = make_float2(arms[b * T + T - 1 - j], arms[((b + 1) % num_filters) * T + T - 1 - j]);
     B2S_TRY(p->d_arms.upload(ctx, pairs.data(), pairs.size(), "pfbarb arms"));
-    B2S_TRY(p->d_circ.alloc(ctx, 2 * T, "pfbarb window"));
-    B2S_TRY(p->d_hist.alloc(ctx, T, "pfbarb history"));
+    B2S_TRY(p->win.init(ctx, 1, (int)T, false, "pfbarb history"));
     p->periodic = getenv("B2S_PFBARB_NO_PERIODIC") ? false : build_periodic_schedule(p.get());
     if (p->periodic) B2S_TRY(p->d_tab.upload(ctx, p->tab.data(), p->tab.size(), "pfbarb schedule table"));
-    B2S_CUDA(ctx, cudaFuncSetAttribute(pfb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPaSmemMax));
+    B2S_TRY(smem_optin<pfb_kernel>(ctx, kPaSmemMax));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     B2S_TRY(b2s_pfbarb_reset(p.get()));
     *out = p.release();
@@ -413,12 +374,9 @@ void b2s_pfbarb_destroy(b2s_pfbarb *p) { PlanDeleter<b2s_pfbarb>()(p); }
 int32_t b2s_pfbarb_reset(b2s_pfbarb *p) {
     if (!p) return b2s_fail(nullptr, B2S_EINVAL, "pfbarb is NULL");
     DeviceGuard g(p->ctx->device);
-    p->start_idx = 0; p->missing = p->T;                           // WindowBuffer::new(len, pad_start=false)
     p->tau = 0.f; p->bf = 0.f; p->mu = 0.f; p->base_index = 0; p->boundary = false;
     p->gpos = 0;
-    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_circ.get(), 0, 2 * p->T * sizeof(float2), p->ctx->stream));
-    B2S_CUDA(p->ctx, cudaMemsetAsync(p->d_hist.get(), 0, p->T * sizeof(float2), p->ctx->stream));
-    return B2S_OK;
+    return p->win.reset(p->ctx);                                   // WindowBuffer::new(len, pad_start=false)
 }
 
 int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
@@ -430,18 +388,9 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
     const int T = (int)p->T;
     const float2 *in = (const float2 *)d_in;
     // fill filter history (arb_resampler.rs:199-215)
-    if (p->missing != 0) {
-        const size_t c = std::min(p->missing, n_in);
-        if (c) {
-            pfb_fill_kernel<<<1, 32, 0, ctx->stream>>>(in, p->d_circ.get(), T, (int)p->start_idx, (int)p->missing, (int)c);
-            B2S_CHECK_LAUNCH(ctx);
-            p->missing -= c;
-            p->start_idx = (p->start_idx + c) % p->T;
-            if (p->missing == 0) {
-                pfb_hist_from_circ<<<1, 256, 0, ctx->stream>>>(p->d_circ.get(), p->d_hist.get(), T, (int)p->start_idx);
-                B2S_CHECK_LAUNCH(ctx);
-            }
-        }
+    if (!p->win.full()) {
+        const size_t c = std::min(p->win.missing(), n_in);
+        B2S_TRY(p->win.push(ctx, in, c));
         *consumed = c;
         if (n_in - c > 0) *call_again = 1;
         return B2S_OK;
@@ -454,7 +403,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
     if (n >= (1ull << 31)) return b2s_fail(ctx, B2S_EUNSUPPORTED, "b2s_pfbarb_exec: more than 2^31 items per call");
     NvtxRange nvtx("b2s_pfbarb_exec");
     PaParams P{};
-    P.in = in; P.hist = p->d_hist.get(); P.out = (float2 *)d_out; P.arms = p->d_arms.get();
+    P.in = in; P.hist = p->win.hist.get(); P.out = (float2 *)d_out; P.arms = p->d_arms.get();
     P.n_in = (long long)n; P.N = (int)p->num_filters; P.T = T; P.delay = p->delay;
     size_t nout;
     Timing after;                                  // fallback path: the state to commit once the call is accepted
@@ -514,8 +463,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
                         (P.arms_in_smem ? arms_smem_bytes : 0);
     pfb_kernel<<<grid, kPaThreads, smem, ctx->stream>>>(P);
     B2S_CHECK_LAUNCH(ctx);
-    pfb_hist_update<<<1, 256, T * sizeof(float2), ctx->stream>>>(p->d_hist.get(), in, T, (long long)n);
-    B2S_CHECK_LAUNCH(ctx);
+    B2S_TRY(p->win.slide(ctx, in, 0, (long long)n));
     // the call is on the stream: commit the timing state
     if (p->periodic) p->gpos = (p->gpos + n) % p->lambda;
     else { p->tau = after.tau; p->mu = after.mu; p->base_index = after.base; p->boundary = after.boundary; }

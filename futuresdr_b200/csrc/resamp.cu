@@ -172,12 +172,8 @@ int32_t b2s_resamp_exec(b2s_resamp *r, const void *d_in, size_t n_in, void *d_ou
     const unsigned grid = (unsigned)ceil_div(p, tile_out);
 #define RS_LAUNCH(S, TS)                                                                                     \
     do {                                                                                                     \
-        auto kern = resamp_kernel<S, TS>;                                                                    \
-        static PerDeviceOnce optin;                           /* the opt-in is the tile ceiling, not this plan's size */ \
-        if (smem > 48 * 1024 && optin.need(ctx->device)) {                                                   \
-            B2S_CUDA(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024)); \
-            optin.done(ctx->device);                                                                         \
-        }                                                                                                    \
+        constexpr auto kern = resamp_kernel<S, TS>;                                                          \
+        if (smem > 48 * 1024) B2S_TRY(smem_optin<kern>(ctx, 216 * 1024));   /* the tile ceiling, not this plan's size */ \
         kern<<<grid, kRsThreads, smem, ctx->stream>>>((const S *)d_in, (S *)d_out, r->d_banks.get(), (int)L, (int)M, \
                                                       (int)T, r->pitch, (long long)p, G, (int)(xs_bytes / isz)); \
     } while (0)

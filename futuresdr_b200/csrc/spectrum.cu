@@ -190,25 +190,11 @@ constexpr size_t spectrum_smem(int log2n) {           // per transform slot: the
 template <int LOG2N>
 int32_t launch_spectrum(b2s_spectrum *p, const SpArgs &a, cudaStream_t stream) {
     constexpr size_t smem = spectrum_smem(LOG2N);
-    auto kern = spectrum_kernel<LOG2N>;
-    static PerDeviceOnce optin;                  // per template instantiation, per device
-    if (smem > 48 * 1024 && optin.need(p->ctx->device)) {
-        B2S_CUDA(p->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        optin.done(p->ctx->device);
-    }
+    B2S_TRY(smem_optin<spectrum_kernel<LOG2N>>(p->ctx, smem));
     const unsigned grid = (unsigned)ceil_div((size_t)a.groups, (size_t)fft_geom(LOG2N, kSpThreads).fpb);
-    kern<<<grid, kSpThreads, smem, stream>>>(a);
+    spectrum_kernel<LOG2N><<<grid, kSpThreads, smem, stream>>>(a);
     B2S_CHECK_LAUNCH(p->ctx);
     return B2S_OK;
-}
-
-template <int LOG2N> int spectrum_resident() {         // CTAs of this instantiation that fit one SM
-    constexpr size_t smem = spectrum_smem(LOG2N);
-    auto kern = spectrum_kernel<LOG2N>;
-    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int nb = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kSpThreads, smem) != cudaSuccess) { cudaGetLastError(); nb = 1; }
-    return nb > 0 ? nb : 1;
 }
 
 }  // namespace
@@ -273,7 +259,10 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     cudaStream_t st = ctx->stream;
     // thread groups: one wave of resident CTAs when the call is long enough, never fewer than 4 frames per group
     const int FPB = fft_geom(p->log2n, kSpThreads).fpb;
-    if (!p->resident) p->resident = with_log2n<5, 13>(p->log2n, 0, [](auto L) { return spectrum_resident<L>(); });
+    if (!p->resident)                                        // CTAs of this size's kernel that fit one SM
+        B2S_TRY((with_log2n<5, 13>(p->log2n, B2S_OK, [&](auto L) {
+            return smem_optin<spectrum_kernel<L>>(ctx, spectrum_smem(L), kSpThreads, &p->resident);
+        })));
     const size_t resident = (size_t)std::max(1, p->resident);
     const size_t g_target = (size_t)ctx->sm_count * resident * FPB;
     const size_t C = std::max<size_t>(4, ceil_div(frames, g_target));

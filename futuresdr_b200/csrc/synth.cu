@@ -7,69 +7,23 @@
 // Device form: (1) gather the channel-major inputs into vectors and run the batched inverse FFT of
 // fft.cu; (2) one thread per (vector, arm) dots the T newest spun samples of its slot (history
 // buffer + this call) with its arm and writes out[(v - v0) * N + w] -- coalesced in w.
-// All windows move in lockstep, so the WindowBuffer bookkeeping (including the scattered start-up
-// order of window_buffer.rs:24-32) is two host scalars; the loop condition of :95-97
+// The windows are the shared window buffer of pfb_common.cuh (spun sample w of vector v is item v*N + w
+// of its stream, so all windows move in lockstep); the loop condition of :95-97
 // (`out.len() - produced > N || !all_windows_filled`) is evaluated in closed form.
-#include <cmath>
 #include <cstdlib>
 
-#include "common.cuh"
-#include "fft_common.cuh"
-
-const float2 *b2s_fft_twiddles(const b2s_fft *p);   // fft.cu
-int b2s_fft_log2n(const b2s_fft *p);
+#include "pfb_common.cuh"
 
 struct b2s_synth {
     b2s_ctx *ctx = nullptr;
     size_t N = 0, T = 0;
-    Buf<float> d_arms;              // [T][N] tap-major: d_arms[j*N + w] = arm_w[j] = taps[w + j*N]; newest sample <-> j = 0
-    Buf<float2> d_circ;             // [N][T] window positions while filling
-    Buf<float2> d_hist;             // [N][T] FIFO order once filled
-    size_t start_idx = 0, missing = 0;
-    bool all_filled = false;
+    PfbBankTaps taps;               // arm w filters window w
+    PfbWindows win;                 // N windows: spun sample w of every vector goes to window w
     PlanPtr<b2s_fft> ifft;
     Buf<float2> d_tmp;              // two halves: gathered vectors, spun vectors
-    Buf<float> d_arms_pad;          // [TPAD][N]: d_arms zero-padded to the fused kernel's tap count
-    int tpad = 0;
 };
 
 namespace {
-
-// vec[v * N + w] = in[w * stride + v]
-__global__ void synth_gather_kernel(const float2 *__restrict__ in, float2 *__restrict__ vec, int N, long long nv,
-                                    long long stride) {
-    __shared__ float2 tile[32][33];
-    const long long v0 = (long long)blockIdx.x * 32;
-    const int w0 = blockIdx.y * 32;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int w = w0 + i; const long long v = v0 + threadIdx.x;
-        if (w < N && v < nv) tile[i][threadIdx.x] = in[(long long)w * stride + v];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const long long v = v0 + i; const int w = w0 + threadIdx.x;
-        if (w < N && v < nv) vec[v * N + w] = tile[threadIdx.x][i];
-    }
-}
-
-// replay of the fill pushes: window position of push #k is pos[k] (same for every window)
-__global__ void synth_fill_kernel(const float2 *__restrict__ spun, float2 *circ, int N, int T, int start_idx,
-                                  int missing, int count) {
-    const int w = blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= N) return;
-    for (int k = 0; k < count; k++) {
-        int idx = (start_idx - missing) % T;
-        if (idx < 0) idx += T;
-        circ[(size_t)w * T + idx] = spun[(size_t)k * N + w];
-        if (missing > 0) missing--;
-        start_idx = (start_idx + 1) % T;
-    }
-}
-
-__global__ void synth_hist_from_circ(const float2 *__restrict__ circ, float2 *hist, int N, int T, int start_idx) {
-    const int w = blockIdx.x;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) hist[(size_t)w * T + t] = circ[(size_t)w * T + (start_idx + t) % T];
-}
 
 // outputs for steady vectors u in [u0, k2): u = -1 is the vector that completed the fill (history only)
 __global__ void synth_bank_kernel(const float2 *__restrict__ spun /* steady vectors, u = 0 first */,
@@ -90,17 +44,6 @@ __global__ void synth_bank_kernel(const float2 *__restrict__ spun /* steady vect
         }
         out[g] = make_float2(re, im);
     }
-}
-
-__global__ void synth_hist_update(float2 *hist, const float2 *__restrict__ spun, int N, int T, long long k2) {
-    extern __shared__ float2 tmp[];
-    const int w = blockIdx.x;
-    for (int t = threadIdx.x; t < T; t += blockDim.x) {
-        const long long up = k2 - T + t;                          // new hist[t] = S(k2 - T + t)
-        tmp[t] = up >= 0 ? spun[up * N + w] : hist[(size_t)w * T + (T + up)];
-    }
-    __syncthreads();
-    for (int t = threadIdx.x; t < T; t += blockDim.x) hist[(size_t)w * T + t] = tmp[t];
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -163,18 +106,8 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
         if (t >= t0) {
             // ---- C: FIR bank
             float2 acc[RL];
-#pragma unroll
-            for (int u = 0; u < RL; u++) acc[u] = make_float2(0.f, 0.f);
-            const float2 *col = Sb + (size_t)(run * RL) * N + w;   // ring row (run*RL + k) <-> vector v0 + run*RL + k - (TPAD-1)
-#pragma unroll
-            for (int k = 0; k < RL + TPAD - 1; k++) {
-                const float2 x = col[(size_t)k * N];
-#pragma unroll
-                for (int u = 0; u < RL; u++) {
-                    const int j = u + TPAD - 1 - k;          // output u sees this row as its j-th newest spun sample
-                    if (j >= 0 && j < TPAD) mac(acc[u], x, tap[j]);
-                }
-            }
+            // ring row (run*RL + k) <-> vector v0 + run*RL + k - (TPAD-1)
+            pfb_bank_column<N, RL, TPAD>(Sb + (size_t)(run * RL) * N + w, tap, acc);
 #pragma unroll
             for (int u = 0; u < RL; u++) {
                 const long long uu = v0 + run * RL + u;
@@ -219,38 +152,19 @@ template <int LOG2N, int TPAD>
 int32_t synth_fused_launch(b2s_synth *s, const float2 *in, long long in_stride, float2 *out, long long k2) {
     constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = synth_fused_smem<LOG2N, TPAD>();
-    auto kern = synth_fused_kernel<LOG2N, TPAD>;
-    static PerDeviceOnce optin;
-    if (smem > 48 * 1024 && optin.need(s->ctx->device)) {
-        B2S_CUDA(s->ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        optin.done(s->ctx->device);
-    }
-    static int resident = 0;
-    if (!resident) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern, 256, smem) != cudaSuccess || resident < 1) { cudaGetLastError(); resident = 1; }
-    }
+    constexpr auto kern = synth_fused_kernel<LOG2N, TPAD>;
+    int resident = 1;
+    B2S_TRY(smem_optin<kern>(s->ctx, smem, 256, &resident));
     constexpr int WARM = (TPAD - 1 + OB - 1) / OB;
     const long long ntiles = (k2 - (long long)WARM * OB + OB - 1) / OB;   // tiles over vectors [WARM*OB, k2)
     if (ntiles > 0x7fffff00ll) return b2s_fail(s->ctx, B2S_EUNSUPPORTED, "synthesizer: too many vectors in one call");
     const long long grid = std::min<long long>(ntiles, (long long)s->ctx->sm_count * resident);
     const long long tpc = (ntiles + grid - 1) / grid;
     const long long grid2 = (ntiles + tpc - 1) / tpc;         // no empty CTAs (the last tile must be owned by the last CTA)
-    kern<<<(unsigned)grid2, 256, smem, s->ctx->stream>>>(in, in_stride, s->d_arms_pad.get(), b2s_fft_twiddles(s->ifft.get()), out, s->d_hist.get(),
-                                                          (int)s->T, k2, (int)ntiles, (int)tpc);
+    kern<<<(unsigned)grid2, 256, smem, s->ctx->stream>>>(in, in_stride, s->taps.arms_pad.get(), b2s_fft_twiddles(s->ifft.get()), out,
+                                                          s->win.hist.get(), (int)s->T, k2, (int)ntiles, (int)tpc);
     B2S_CHECK_LAUNCH(s->ctx);
     return B2S_OK;
-}
-
-template <int TPAD>
-int32_t synth_fused_dispatch(b2s_synth *s, int log2n, const float2 *in, long long in_stride, float2 *out, long long k2) {
-    return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN, [&](auto L) { return synth_fused_launch<L, TPAD>(s, in, in_stride, out, k2); });
-}
-
-int synth_fused_tpad(const b2s_synth *s) {
-    const int l2 = b2s_fft_log2n(s->ifft.get());
-    if (getenv("B2S_SYNTH_NO_FUSED")) return 0;
-    if (l2 < 2 || l2 > 8 || s->T > 32) return 0;
-    return s->T <= 8 ? 8 : (s->T <= 16 ? 16 : 32);
 }
 
 int synth_fused_ob(int log2n) { return fftk::fft_geom(log2n, 256).fpb; }
@@ -268,24 +182,16 @@ int32_t b2s_synth_plan_c32(b2s_ctx *ctx, size_t num_channels, const float *taps,
     DeviceGuard g(ctx->device);
     PlanPtr<b2s_synth> s(new b2s_synth());
     s->ctx = ctx; s->N = num_channels;
-    const size_t N = s->N, T = (size_t)std::ceil((float)ntaps / (float)N);     // utilities.rs:9
-    s->T = T; s->missing = T;
-    std::vector<float> arms(N * T, 0.0f);
-    for (size_t i = 0; i < N; i++) { size_t j = 0; for (size_t idx = i; idx < ntaps; idx += N) arms[(j++) * N + i] = taps[idx]; }
+    const size_t N = s->N;
+    std::vector<float> arms;
+    const size_t T = pfb_partition(taps, ntaps, N, arms);
+    s->T = T;
     b2s_fft *ifft = nullptr;
     B2S_TRY(b2s_fft_plan_c32(ctx, N, 1, 0, 0, 1.0f, &ifft));                  // plan_fft(n, Inverse) (synthesizer.rs:65)
     s->ifft.reset(ifft);
-    B2S_TRY(s->d_arms.upload(ctx, arms.data(), arms.size(), "synthesizer arms"));
-    B2S_TRY(s->d_circ.alloc(ctx, N * T, "synthesizer windows"));
-    B2S_TRY(s->d_hist.alloc(ctx, N * T, "synthesizer history"));
-    B2S_CUDA(ctx, cudaMemsetAsync(s->d_circ.get(), 0, N * T * sizeof(float2), ctx->stream));
-    s->tpad = synth_fused_tpad(s.get());
-    std::vector<float> apad;
-    if (s->tpad) {
-        apad.assign((size_t)s->tpad * N, 0.0f);                                  // taps beyond T are zero (older samples)
-        std::copy(arms.begin(), arms.end(), apad.begin());
-        B2S_TRY(s->d_arms_pad.upload(ctx, apad.data(), apad.size(), "synthesizer padded arms"));
-    }
+    const int tpad = getenv("B2S_SYNTH_NO_FUSED") ? 0 : pfb_fused_tpad(b2s_fft_log2n(ifft), T);
+    B2S_TRY(s->taps.upload(ctx, arms, N, T, tpad, "synthesizer arms"));
+    B2S_TRY(s->win.init(ctx, (int)N, (int)T, false, "synthesizer windows"));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *out = s.release();
     return B2S_OK;
@@ -304,12 +210,14 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
     // closed form of `while n_in - c > 0 && (cap - p > N || !all_filled)`
     size_t k1 = 0, k2 = 0, p = 0;
     bool completes = false;
-    if (!s->all_filled) {
-        k1 = std::min(n_in, s->missing);
-        completes = (k1 == s->missing) && k1 > 0;
+    const bool all_filled = s->win.full();
+    if (!all_filled) {
+        const size_t missing = s->win.missing() / N;          // vectors
+        k1 = std::min(n_in, missing);
+        completes = (k1 == missing) && k1 > 0;
         if (completes) p = N;                       // the completing vector writes its N outputs unconditionally
     }
-    if (s->all_filled || completes) {
+    if (all_filled || completes) {
         const size_t remaining = n_in - k1;
         if (n_out_cap > p + N) {
             const size_t room = n_out_cap - N - p;  // vectors while cap - p > N  <=>  p < cap - N
@@ -327,51 +235,37 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
     // steady calls long enough for two tiles: the first OB vectors (their windows reach into the previous call's
     // history) through the three kernels below, everything after them through the fused kernel
     const int l2n = b2s_fft_log2n(s->ifft.get());
-    const size_t ob = s->tpad ? (size_t)synth_fused_ob(l2n) : 0;
-    const size_t lead = s->tpad ? synth_fused_lead(l2n, s->tpad) : 0;
-    const bool fused = s->tpad && s->all_filled && k1 == 0 && k2 >= lead + ob && k2 >= lead + T;
+    const int tpad = s->taps.tpad;
+    const size_t ob = tpad ? (size_t)synth_fused_ob(l2n) : 0;
+    const size_t lead = tpad ? synth_fused_lead(l2n, tpad) : 0;
+    const bool fused = tpad && all_filled && k1 == 0 && k2 >= lead + ob && k2 >= lead + T;
     const size_t k2_all = k2;
     if (fused) k2 = lead;                                 // the generic part
     const size_t items = (k1 + k2) * N;
     if (s->d_tmp.size() < 2 * items) B2S_TRY(s->d_tmp.reserve(ctx, 2 * (items * 5 / 4 + 1024), "synthesizer workspace"));
     float2 *vec = s->d_tmp.get(), *spun = s->d_tmp.get() + s->d_tmp.size() / 2;
     const size_t nvg = k1 + k2;                           // vectors of the generic part
-    dim3 gg((unsigned)ceil_div(nvg, (size_t)32), (unsigned)ceil_div(N, (size_t)32));
-    synth_gather_kernel<<<gg, dim3(32, 8), 0, ctx->stream>>>((const float2 *)d_in, vec, (int)N, (long long)nvg, (long long)in_stride);
-    B2S_CHECK_LAUNCH(ctx);
+    B2S_TRY(pfb_transpose(ctx, (const float2 *)d_in, vec, N, nvg, in_stride, N));   // vec[v * N + w] = in[w * in_stride + v]
     size_t fc = 0, fp = 0;
     int32_t rc = b2s_fft_exec(s->ifft.get(), vec, items, spun, items, &fc, &fp);
     if (rc != B2S_OK) return rc;
-    if (k1) {
-        synth_fill_kernel<<<(unsigned)ceil_div(N, (size_t)128), 128, 0, ctx->stream>>>(spun, s->d_circ.get(), (int)N, (int)T,
-                                                                                         (int)s->start_idx, (int)s->missing, (int)k1);
-        B2S_CHECK_LAUNCH(ctx);
-        s->missing -= k1;
-        s->start_idx = (s->start_idx + k1) % T;
-        if (completes) {
-            synth_hist_from_circ<<<(unsigned)N, 64, 0, ctx->stream>>>(s->d_circ.get(), s->d_hist.get(), (int)N, (int)T, (int)s->start_idx);
-            B2S_CHECK_LAUNCH(ctx);
-            s->all_filled = true;
-        }
-    }
+    B2S_TRY(s->win.push(ctx, spun, k1 * N));
     if (p) {
         const int u0 = completes ? -1 : 0;
         const size_t total = (k2 - (long long)u0) * N;
         const unsigned grid = (unsigned)std::min<size_t>(ceil_div(total, (size_t)256), (size_t)ctx->sm_count * 32);
-        synth_bank_kernel<<<grid, 256, 0, ctx->stream>>>(spun + k1 * N, s->d_hist.get(), s->d_arms.get(), (float2 *)d_out, (int)N, (int)T,
+        synth_bank_kernel<<<grid, 256, 0, ctx->stream>>>(spun + k1 * N, s->win.hist.get(), s->taps.arms.get(), (float2 *)d_out, (int)N, (int)T,
                                                          u0, (long long)k2);
         B2S_CHECK_LAUNCH(ctx);
     }
     if (fused) {
         // (the generic bank kernel above has read the old history; the fused kernel writes the new one)
-        int32_t frc = B2S_EAGAIN;
-        if (s->tpad == 8) frc = synth_fused_dispatch<8>(s, l2n, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
-        else if (s->tpad == 16) frc = synth_fused_dispatch<16>(s, l2n, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
-        else if (s->tpad == 32) frc = synth_fused_dispatch<32>(s, l2n, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
+        const int32_t frc = pfb_fused_dispatch(l2n, tpad, [&](auto L, auto P) {
+            return synth_fused_launch<L, P>(s, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
+        });
         if (frc != B2S_OK) return frc == B2S_EAGAIN ? b2s_fail(ctx, B2S_ESTATE, "synthesizer: fused shape mismatch") : frc;
     } else if (k2) {
-        synth_hist_update<<<(unsigned)N, 64, T * sizeof(float2), ctx->stream>>>(s->d_hist.get(), spun + k1 * N, (int)N, (int)T, (long long)k2);
-        B2S_CHECK_LAUNCH(ctx);
+        B2S_TRY(s->win.slide(ctx, spun + k1 * N, 0, (long long)(k2 * N)));
     }
     *consumed_per_channel = nv; *produced = p;
     return B2S_OK;
