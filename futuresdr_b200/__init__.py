@@ -1,10 +1,11 @@
 """futuresdr_b200 -- H100-native (sm_90a) backend for FutureSDR's FIR / decimator / resampler /
-FFT / Apply / PfbArbResampler hot path.
+FFT / Apply / PfbArbResampler hot path, and the stream plumbing of branching flowgraphs.
 
 Python host layer above the C ABI (include/b200sdr.h).  Class and method names mirror the
 reference's Rust API for this path (futuredsp::{FirFilter, DecimatingFirFilter,
-PolyphaseResamplingFir}, futuresdr::blocks::{Fir, FirBuilder, Fft, Apply, PfbArbResampler,
-SignalSource, SignalSourceBuilder, FixedPointPhase, Head},
+PolyphaseResamplingFir}, futuredsp::{firdes::hilbert, windows::hamming}, futuresdr::blocks::{Fir,
+FirBuilder, Fft, Apply, PfbArbResampler, SignalSource, SignalSourceBuilder, FixedPointPhase, Head,
+Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver},
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -19,6 +20,7 @@ from .filters import (  # noqa: F401
 )
 from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
+    Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator,
 )
-from . import firdes  # noqa: F401
-# host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain): futuresdr_b200.edges
+from . import firdes, windows  # noqa: F401
+# host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

@@ -20,6 +20,10 @@ ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
  OP_MAG_C32, OP_LOG10_F32) = range(8)
 WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
+(COMBINE_ADD_F32, COMBINE_SUB_F32, COMBINE_MUL_F32, COMBINE_CONJ_MUL_C32, COMBINE_MAG_DIV_C32_F32, COMBINE_TO_C32,
+ COMBINE_TO_C32_NEG_Q) = range(7)
+SPLIT_RE_IM, SPLIT_DUP_F32 = 0, 1
+FANOUT_MAX_OUTPUTS = 256
 
 _vp, _sz, _i32, _f32 = C.c_void_p, C.c_size_t, C.c_int32, C.c_float
 _szp, _i32p, _vpp, _f32p = C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_float)
@@ -134,6 +138,11 @@ SIGNATURES = {
     "b2s_memset": (_i32, [_vp, _vp, _i32, _sz]),
     "b2s_firdes_kaiser_lowpass": (_sz, [C.c_double, C.c_double, C.c_double, _f32p, _sz]),
     "b2s_firdes_kaiser_multirate": (_sz, [_sz, _sz, _sz, C.c_double, _f32p, _sz]),
+    "b2s_combine_exec": (_i32, [_vp, C.c_int, _vp, _sz, _vp, _sz, _vp, _sz, _szp, _szp]),
+    "b2s_split_exec": (_i32, [_vp, C.c_int, _vp, _sz, _vp, _vp, _sz, _szp, _szp]),
+    "b2s_fanout_exec": (_i32, [_vp, _i32, _sz, _vp, _sz, _vpp, _sz, _sz, _szp, _szp]),
+    "b2s_window_hamming": (_sz, [_sz, _i32, C.POINTER(C.c_double), _sz]),
+    "b2s_firdes_hilbert": (_sz, [C.POINTER(C.c_double), _sz, _f32p, _sz]),
 }
 
 

@@ -8,6 +8,9 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``Fft`` / ``FftDirection``    src/blocks/fft.rs:30-221
   * ``Apply``                     src/blocks/apply.rs:100-131 (closed catalogue of closures)
   * ``PfbArbResampler``           src/blocks/pfb/arb_resampler.rs:72-231
+  * ``Combine`` / ``Split``       src/blocks/combine.rs:31-137, split.rs:31-127 (closed catalogues of closures)
+  * ``Delay``                     src/blocks/delay.rs:31-169
+  * ``StreamDuplicator`` / ``StreamDeinterleaver``   src/blocks/stream_duplicator.rs, stream_deinterleaver.rs
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
 
@@ -115,6 +118,18 @@ class Writer:
 class Block:
     in_dtype = np.complex64
     out_dtype = np.complex64
+
+    # Stream ports, as the graph driver (edges.Flowgraph) addresses them: a port is an attribute name, or
+    # (attribute name, index) for one port of a list of ports.  Single-input / single-output blocks keep the defaults.
+    def stream_inputs(self) -> list:
+        return ["input"] if self.in_dtype is not None else []
+
+    def stream_outputs(self) -> list:
+        return ["output"] if self.out_dtype is not None else []
+
+    def port_dtype(self, port) -> np.dtype:
+        name = port[0] if isinstance(port, tuple) else port
+        return np.dtype(self.in_dtype if name == "input" else self.out_dtype)
 
     def _ports(self):
         ctx = getattr(self, "ctx", None) or getattr(getattr(self, "filter", None), "ctx", None)
@@ -687,6 +702,241 @@ class PfbChannelizer(Block, Handle):
         if ca.value:
             io.call_again = True
         elif n_in - c.value < self.decimation_factor and self.input.finished():      # :214-218
+            io.finished = True
+
+
+def _ptr(t: torch.Tensor) -> C.c_void_p:
+    return C.c_void_p(t.data_ptr())
+
+
+class CombineOp(enum.IntEnum):
+    """The Combine closures of the reference graphs that exist as device ops (b2s_combine_op)."""
+    AddF32 = _lib.COMBINE_ADD_F32                # a + b                 (tests/combine.rs)
+    SubF32 = _lib.COMBINE_SUB_F32                # i1 - i2               (m17 rx)
+    MulF32 = _lib.COMBINE_MUL_F32                # a * b                 (cw)
+    ConjMulC32 = _lib.COMBINE_CONJ_MUL_C32       # a * b.conj()          (wlan rx)
+    MagDivC32F32 = _lib.COMBINE_MAG_DIV_C32_F32  # a.norm() / b          (wlan rx)
+    ToC32 = _lib.COMBINE_TO_C32                  # Complex32::new(i, q)  (ssb USB)
+    ToC32NegQ = _lib.COMBINE_TO_C32_NEG_Q        # Complex32::new(i, q * -1.0) (ssb LSB)
+
+
+_F32, _C32 = np.dtype(np.float32), np.dtype(np.complex64)
+_COMBINE_TYPES = {                               # (in0, in1, output)
+    CombineOp.AddF32: (_F32, _F32, _F32), CombineOp.SubF32: (_F32, _F32, _F32), CombineOp.MulF32: (_F32, _F32, _F32),
+    CombineOp.ConjMulC32: (_C32, _C32, _C32), CombineOp.MagDivC32F32: (_C32, _F32, _F32),
+    CombineOp.ToC32: (_F32, _F32, _C32), CombineOp.ToC32NegQ: (_F32, _F32, _C32),
+}
+
+
+class Combine(Block):
+    """blocks::Combine (src/blocks/combine.rs:31-137): two input streams ``in0``, ``in1`` -> ``output`` through one
+    closure of CombineOp.  Finishes when an input has finished and everything on it was processed (:127-133)."""
+    in_dtype = None
+
+    def __init__(self, op: CombineOp, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.op = CombineOp(op)
+        a, b, self.out_dtype = _COMBINE_TYPES[self.op]
+        dev = _ctx_device(self.ctx)
+        self.in0, self.in1, self.output = Reader(a, dev), Reader(b, dev), Writer(self.out_dtype, dev)
+
+    def stream_inputs(self):
+        return ["in0", "in1"]
+
+    def port_dtype(self, port):
+        return {"in0": self.in0.dtype, "in1": self.in1.dtype, "output": np.dtype(self.out_dtype)}[port]
+
+    def combine(self, i0: torch.Tensor, i1: torch.Tensor, o: torch.Tensor) -> int:
+        """The closure over min(len) items of device slices (asynchronous); returns that count."""
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_combine_exec(self.ctx.handle, int(self.op), _ptr(i0), i0.numel(), _ptr(i1), i1.numel(), _ptr(o),
+                                   o.numel(), C.byref(c), C.byref(p)), self.ctx.handle)
+        return p.value
+
+    def work(self, io: WorkIo):
+        i0, i1, o = self.in0.slice(), self.in1.slice(), self.output.slice()       # combine.rs:108-115
+        i0_len, i1_len = i0.numel(), i1.numel()
+        m = min(i0_len, i1_len, o.numel())
+        if m > 0:
+            self.combine(i0, i1, o)
+            self.in0.consume(m)
+            self.in1.consume(m)
+            self.output.produce(m)
+        if self.in0.finished() and m == i0_len:                                 # :127-133
+            io.finished = True
+        if self.in1.finished() and m == i1_len:
+            io.finished = True
+
+
+class SplitOp(enum.IntEnum):
+    """The Split closures that exist as device ops (b2s_split_op)."""
+    ReIm = _lib.SPLIT_RE_IM                      # |a: &Complex32| (a.re, a.im)   (tests/split.rs)
+    DupF32 = _lib.SPLIT_DUP_F32                  # |v: &f32| (*v, *v)             (ssb)
+
+
+class Split(Block):
+    """blocks::Split (src/blocks/split.rs:31-127): ``input`` -> ``output0``, ``output1`` through one closure."""
+
+    def __init__(self, op: SplitOp, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.op = SplitOp(op)
+        self.in_dtype = _C32 if self.op == SplitOp.ReIm else _F32
+        self.out_dtype = None
+        dev = _ctx_device(self.ctx)
+        self.input = Reader(self.in_dtype, dev)
+        self.output0, self.output1 = Writer(_F32, dev), Writer(_F32, dev)
+
+    def stream_outputs(self):
+        return ["output0", "output1"]
+
+    def port_dtype(self, port):
+        return np.dtype(self.in_dtype) if port == "input" else _F32
+
+    def split(self, i: torch.Tensor, o0: torch.Tensor, o1: torch.Tensor) -> int:
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_split_exec(self.ctx.handle, int(self.op), _ptr(i), i.numel(), _ptr(o0), _ptr(o1),
+                                 min(o0.numel(), o1.numel()), C.byref(c), C.byref(p)), self.ctx.handle)
+        return p.value
+
+    def work(self, io: WorkIo):
+        i0, o0, o1 = self.input.slice(), self.output0.slice(), self.output1.slice()   # split.rs:101-107
+        i0_len = i0.numel()
+        m = min(i0_len, o0.numel(), o1.numel())
+        if m > 0:
+            self.split(i0, o0, o1)
+            self.input.consume(m)
+            self.output0.produce(m)
+            self.output1.produce(m)
+        if self.input.finished() and m == i0_len:                               # :121-123
+            io.finished = True
+
+
+class Delay(Block):
+    """blocks::Delay (src/blocks/delay.rs:31-169): ``n > 0`` pads n zero items in front of the stream, ``n <= 0`` skips
+    -n items.  The pad is a device memset and the copy a device-to-device copy; a skip only moves the read cursor.
+    ``state`` is ("pad", n), ("skip", n) or ("copy", 0)."""
+
+    def __init__(self, dtype, n: int, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.in_dtype = self.out_dtype = np.dtype(dtype)
+        n = int(n)
+        self.state = ("pad", n) if n > 0 else ("skip", -n)                      # delay.rs:55-60
+        self._ports()
+
+    def new_value(self, pad: bool, value: int):
+        """The ``new_value`` message handler (delay.rs:68-105): shifts the delay by +value (pad) or -value (skip)."""
+        val = int(value) if pad else -int(value)
+        kind, n = self.state
+        new_val = (n if kind == "pad" else -n if kind == "skip" else 0) + val
+        self.state = ("pad", new_val) if new_val > 0 else ("copy", 0) if new_val == 0 else ("skip", -new_val)
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()                          # delay.rs:120-123
+        i_len, o_len = i.numel(), o.numel()
+        isz = self.in_dtype.itemsize
+        kind, n = self.state
+        if kind == "pad":
+            m = min(o_len, n)
+            if m:
+                check(lib.b2s_memset(self.ctx.handle, _ptr(o), 0, m * isz), self.ctx.handle)
+            self.output.produce(m)
+            if m == n:
+                self.state = ("copy", 0)
+                io.call_again = True
+                if self.input.finished():
+                    io.finished = True
+            else:
+                self.state = ("pad", n - m)
+        elif kind == "skip":
+            m = min(i_len, n)
+            self.input.consume(m)
+            if n == m:
+                self.state = ("copy", 0)
+                io.call_again = True
+            else:
+                self.state = ("skip", n - m)
+            if self.input.finished() and m == i_len:
+                io.finished = True
+        else:
+            m = min(i_len, o_len)
+            if m > 0:
+                check(lib.b2s_memcpy_d2d(self.ctx.handle, _ptr(o), _ptr(i), m * isz), self.ctx.handle)
+            self.input.consume(m)
+            self.output.produce(m)
+            if self.input.finished() and m == i_len:
+                io.finished = True
+
+
+class _FanOut(Block):
+    """One input, ``n`` outputs in the list attribute ``self._list``, moved by one b2s_fanout_exec launch."""
+    _list = ""
+    _deinterleave = 0
+
+    def __init__(self, dtype, n: int, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.in_dtype = self.out_dtype = np.dtype(dtype)
+        if self.in_dtype.itemsize not in (4, 8):
+            raise ValueError(f"{type(self).__name__}: items of 4 or 8 bytes, not {self.in_dtype}")
+        self.n = int(n)
+        if self.n < 1:
+            raise ValueError(f"{type(self).__name__}: at least one output")
+        if self.n > _lib.FANOUT_MAX_OUTPUTS:
+            raise _lib.B200SdrError(_lib.EUNSUPPORTED, f"{type(self).__name__}: {self.n} outputs "
+                                    f"(at most {_lib.FANOUT_MAX_OUTPUTS} in one launch)")
+        dev = _ctx_device(self.ctx)
+        self.input = Reader(self.in_dtype, dev)
+        setattr(self, self._list, [Writer(self.in_dtype, dev) for _ in range(self.n)])
+
+    def stream_outputs(self):
+        return [(self._list, k) for k in range(self.n)]
+
+    def port_dtype(self, port):
+        return self.in_dtype
+
+    def fanout(self, i: torch.Tensor, outs) -> tuple[int, int]:
+        """(consumed, produced per output) of one launch over device slices."""
+        ptrs = (C.c_void_p * len(outs))(*[o.data_ptr() for o in outs])
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_fanout_exec(self.ctx.handle, self._deinterleave, self.in_dtype.itemsize, _ptr(i), i.numel(), ptrs,
+                                  len(outs), min(o.numel() for o in outs), C.byref(c), C.byref(p)), self.ctx.handle)
+        return c.value, p.value
+
+
+class StreamDuplicator(_FanOut):
+    """blocks::StreamDuplicator<T, N> (src/blocks/stream_duplicator.rs:20-94): ``input`` copied to ``outputs[k]``."""
+    _list = "outputs"
+
+    def work(self, io: WorkIo):
+        outs = [w.slice() for w in self.outputs]                                # stream_duplicator.rs:72-80
+        i = self.input.slice()
+        nitem_to_consume = i.numel()
+        m = min(min(o.numel() for o in outs), nitem_to_consume)
+        if m > 0:
+            self.fanout(i, outs)
+            for w in self.outputs:
+                w.produce(m)
+            self.input.consume(m)
+        if nitem_to_consume - m == 0 and self.input.finished():                 # :89-91
+            io.finished = True
+
+
+class StreamDeinterleaver(_FanOut):
+    """blocks::StreamDeinterleaver<T> (src/blocks/stream_deinterleaver.rs:25-98): item j N + k of ``input`` goes to
+    ``output[k]``; only whole groups of N are moved, and the block finishes once fewer than N items are left."""
+    _list = "output"
+    _deinterleave = 1
+
+    def work(self, io: WorkIo):
+        outs = [w.slice() for w in self.output]                                 # stream_deinterleaver.rs:67-75
+        i = self.input.slice()
+        n_items_to_consume = i.numel()
+        m = min(min(o.numel() for o in outs), n_items_to_consume // self.n)
+        if m > 0:
+            self.fanout(i, outs)
+            for w in self.output:
+                w.produce(m)
+            self.input.consume(m * self.n)
+        if n_items_to_consume - m * self.n < self.n and self.input.finished():   # :91-95
             io.finished = True
 
 

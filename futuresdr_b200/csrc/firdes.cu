@@ -96,4 +96,43 @@ size_t b2s_firdes_kaiser_multirate(size_t interp, size_t decim, size_t half_poly
     return n;
 }
 
+// windows::gen_cos (windows.rs:68-94) with coeffs {0.54, 0.46}, literally: alpha is computed in f32 and widened, pi is
+// f32::consts::PI widened to f64, and the terms (-1)^k c_k cos(pi (k n) / alpha) are summed in k order.
+size_t b2s_window_hamming(size_t len, int32_t periodic, double *out, size_t cap) {
+    if (len == 0) return 0;
+    if (!out || cap < len) return len;
+    static const double coeffs[2] = {0.54, 0.46};
+    const size_t npts = periodic ? len + 1 : len;
+    const double alpha = (double)((float)(npts - 1) / 2.0f);
+    const double pi = (double)3.14159265358979323846f;
+    for (size_t n = 0; n < len; n++) {               // the periodic window's extra last point is dropped
+        double s = -0.0;
+        for (int k = 0; k < 2; k++) {
+            const double sign = (k & 1) ? -1.0 : 1.0;  // (-1.0).powi(k)
+            s += sign * coeffs[k] * std::cos(pi * (double)(k * n) / alpha);
+        }
+        out[n] = s;
+    }
+    return len;
+}
+
+// firdes::hilbert (basic.rs:202-222), literally: the odd taps h +- i for i in (1..h).step_by(2), the gain recurrence,
+// then x / gain cast to f32.
+size_t b2s_firdes_hilbert(const double *window, size_t len, float *taps, size_t cap) {
+    if (len == 0 || len % 2 == 0) return 0;
+    if (!window || !taps || cap < len) return len;
+    std::vector<double> t(len, 0.0);
+    const size_t h = (len - 1) / 2;
+    double gain = 0.0;
+    for (size_t i = 1; i < h; i += 2) {
+        const double x = 1.0 / (double)i;
+        t[h + i] = x * window[h + i];
+        t[h - i] = -x * window[h - i];
+        gain = t[h + i] - gain;
+    }
+    gain = 2.0 * std::fabs(gain);
+    for (size_t i = 0; i < len; i++) taps[i] = (float)(t[i] / gain);
+    return len;
+}
+
 }  // extern "C"

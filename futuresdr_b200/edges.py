@@ -14,7 +14,9 @@ What the reference has, and what mirrors it here:
 
 ``run_chain`` is NOT a scheduler (the reference's runtime is out of scope, SURVEY.md §8): it is the
 Mocker idea (src/runtime/mocker.rs) extended to a linear chain -- call ``work`` on every stage in turn
-until all report finished -- so the edges and the finish rules can be tested end to end.
+until all report finished -- so the edges and the finish rules can be tested end to end.  ``Flowgraph``
+does the same for branching graphs (fan-out through ``MultiStreamBuffer``, fan-in through multi-input
+blocks such as Combine) with the reference's StreamInputDone / StreamOutputDone finish rules.
 """
 from __future__ import annotations
 
@@ -101,6 +103,79 @@ class _WriterPort:
 
     def produce(self, n):
         self.buf.produce(n)
+
+    def set_min_items(self, n):
+        self.min_items = max(self.min_items, n)
+
+
+class MultiStreamBuffer:
+    """Linear device buffer with one writer and ``n_readers`` readers, each with its own read cursor (the reference's
+    buffers let one output feed several inputs).  The writer's free space is bounded by the slowest reader that is
+    still running: unconsumed items from the smallest live read cursor on are moved to the front when the free tail
+    gets short.  A reader whose block has finished no longer holds items back."""
+
+    def __init__(self, dtype, capacity_items: int, n_readers: int, device="cuda"):
+        self.dtype = np.dtype(dtype)
+        self.data = torch.empty(int(capacity_items), dtype=_tdtype(dtype), device=device)
+        self.rd = [0] * int(n_readers)
+        self.live = [True] * int(n_readers)
+        self.wr = 0
+        self.shift = 0                              # items dropped from the front by compaction so far
+        self.writer_finished = False
+
+    def _low(self) -> int:
+        live = [r for r, a in zip(self.rd, self.live) if a]
+        return min(live) if live else self.wr
+
+    def _compact(self):
+        lo = self._low()
+        if lo == 0:
+            return
+        rem = self.wr - lo
+        if rem:
+            src = self.data[lo:self.wr]
+            if rem > lo:                            # source and destination overlap
+                src = src.clone()
+            self.data[:rem].copy_(src)
+        self.rd = [max(r - lo, 0) for r in self.rd]
+        self.wr = rem
+        self.shift += lo
+
+    # writer side
+    def write_slice(self) -> torch.Tensor:
+        if self._low() and (self.data.numel() - self.wr) < self.data.numel() // 2:
+            self._compact()
+        return self.data[self.wr:]
+
+    def produce(self, n: int):
+        assert self.wr + n <= self.data.numel()
+        self.wr += n
+
+    # reader side
+    def read_slice(self, k: int) -> torch.Tensor:
+        return self.data[self.rd[k]:self.wr]
+
+    def consume(self, k: int, n: int):
+        assert self.rd[k] + n <= self.wr
+        self.rd[k] += n
+
+    def cursors(self) -> tuple:
+        """Stream positions of the write and read cursors (unchanged by compaction)."""
+        return (self.wr + self.shift, *(r + self.shift for r in self.rd))
+
+
+class _MultiReaderPort:
+    def __init__(self, buf: MultiStreamBuffer, k: int):
+        self.buf, self.k, self.dtype, self.min_items = buf, k, buf.dtype, 1
+
+    def slice(self):
+        return self.buf.read_slice(self.k)
+
+    def consume(self, n):
+        self.buf.consume(self.k, n)
+
+    def finished(self):
+        return self.buf.writer_finished
 
     def set_min_items(self, n):
         self.min_items = max(self.min_items, n)
@@ -358,3 +433,126 @@ def run_chain(stages: Sequence[Block], buffer_items: int = 4 << 20, max_rounds: 
     if torch.device(device).type == "cuda":
         torch.cuda.synchronize()
     return calls
+
+
+# ---------------------------------------------------------------------------------------------------
+# fan-out / fan-in graph driver
+# ---------------------------------------------------------------------------------------------------
+def _port_key(p):
+    return tuple(p) if isinstance(p, (tuple, list)) else p
+
+
+def _set_port(blk: Block, port, obj):
+    if isinstance(port, tuple):
+        getattr(blk, port[0])[port[1]] = obj
+    else:
+        setattr(blk, port, obj)
+
+
+class Flowgraph:
+    """A graph of blocks joined by device stream buffers, driven like ``run_chain`` (the Mocker idea, not a scheduler:
+    the reference's runtime is out of scope, SURVEY.md §8) but with any topology:
+
+      * ``connect(src, "port", dst, "port")``; ports default to ``"output"`` / ``"input"`` (``connect(src, dst)``),
+        a port of a list of ports is ``("outputs", k)``.  Item types must agree on every edge.
+      * one output port may feed several inputs (``MultiStreamBuffer``); an input port has exactly one writer.
+      * finish rules of the reference's block loop (runtime/wrapped_kernel.rs:133-138, :188-191): a block that finishes
+        marks each of its output streams finished for the readers (StreamInputDone) and finishes every block writing
+        to one of its inputs (StreamOutputDone), even when that writer has other readers.  The run ends when every
+        block has finished; a round in which no block moves a cursor, changes state or finishes raises.
+
+    Blocks run round-robin in the order they first appear in ``connect`` calls."""
+
+    def __init__(self):
+        self.blocks: List[Block] = []
+        self.edges: List[tuple] = []                 # (src, src_port, dst, dst_port)
+
+    def add(self, blk: Block) -> Block:
+        if not any(b is blk for b in self.blocks):
+            self.blocks.append(blk)
+        return blk
+
+    def connect(self, src: Block, *args):
+        """connect(src, dst) | connect(src, src_port, dst) | connect(src, dst, dst_port) |
+        connect(src, src_port, dst, dst_port)."""
+        a = list(args)
+        src_port = _port_key(a.pop(0)) if a and not isinstance(a[0], Block) else "output"
+        if not a or not isinstance(a[0], Block):
+            raise TypeError("Flowgraph.connect: the destination block is missing")
+        dst = a.pop(0)
+        dst_port = _port_key(a.pop(0)) if a else "input"
+        if a:
+            raise TypeError("Flowgraph.connect: too many arguments")
+        if src_port not in src.stream_outputs():
+            raise ValueError(f"{type(src).__name__} has no stream output {src_port!r}")
+        if dst_port not in dst.stream_inputs():
+            raise ValueError(f"{type(dst).__name__} has no stream input {dst_port!r}")
+        if any(d is dst and dp == dst_port for _, _, d, dp in self.edges):
+            raise ValueError(f"{type(dst).__name__}.{dst_port} is already connected")
+        st, dt = np.dtype(src.port_dtype(src_port)), np.dtype(dst.port_dtype(dst_port))
+        if st != dt:
+            raise TypeError(f"{type(src).__name__}.{src_port} ({st}) -> {type(dst).__name__}.{dst_port} ({dt}): "
+                            "item types differ")
+        self.add(src)
+        self.add(dst)
+        self.edges.append((src, src_port, dst, dst_port))
+
+    def run(self, buffer_items: int = 4 << 20, max_rounds: int = 1 << 24, device="cuda") -> int:
+        """Run until every block has finished; returns the number of work() calls made."""
+        idx = {id(b): k for k, b in enumerate(self.blocks)}
+        for b in self.blocks:
+            for p in b.stream_inputs():
+                if not any(d is b and dp == p for _, _, d, dp in self.edges):
+                    raise ValueError(f"{type(b).__name__}.{p} is not connected")
+            for p in b.stream_outputs():
+                if not any(s is b and sp == p for s, sp, _, _ in self.edges):
+                    raise ValueError(f"{type(b).__name__}.{p} is not connected")
+        writers = {}                                 # (src index, port) -> [(dst, dst_port), ...]
+        for s, sp, d, dp in self.edges:
+            writers.setdefault((idx[id(s)], sp), []).append((d, dp))
+        out_bufs = [[] for _ in self.blocks]         # block -> buffers it writes
+        in_bufs = [[] for _ in self.blocks]          # block -> (buffer, reader index, writer block index)
+        bufs = []
+        for (si, sp), readers in writers.items():
+            src = self.blocks[si]
+            b = MultiStreamBuffer(src.port_dtype(sp), buffer_items, len(readers), device)
+            _set_port(src, sp, _WriterPort(b))
+            for k, (d, dp) in enumerate(readers):
+                _set_port(d, dp, _MultiReaderPort(b, k))
+                in_bufs[idx[id(d)]].append((b, k, si))
+            out_bufs[si].append(b)
+            bufs.append(b)
+        done = [False] * len(self.blocks)
+
+        def finish(k):
+            if done[k]:
+                return
+            done[k] = True
+            for b in out_bufs[k]:                    # StreamInputDone to every reader
+                b.writer_finished = True
+            for b, r, w in in_bufs[k]:               # StreamOutputDone to every writer
+                b.live[r] = False
+                finish(w)
+
+        calls = 0
+        for _ in range(max_rounds):
+            progressed = False
+            for k, blk in enumerate(self.blocks):
+                if done[k]:
+                    continue
+                before = tuple(b.cursors() for b in bufs)
+                io = WorkIo()
+                blk.work(io)
+                calls += 1
+                if io.finished:
+                    finish(k)
+                    progressed = True
+                progressed |= io.call_again or before != tuple(b.cursors() for b in bufs)
+            if all(done):
+                break
+            if not progressed:
+                stuck = [type(b).__name__ for k, b in enumerate(self.blocks) if not done[k]]
+                raise RuntimeError(f"Flowgraph.run: no block can make progress (still running: {stuck})")
+        if torch.device(device).type == "cuda":
+            torch.cuda.synchronize()
+        return calls

@@ -1,4 +1,4 @@
-"""Tap design (host, f64): futuredsp::firdes::kaiser (crates/futuredsp/src/firdes/basic.rs:310-459)."""
+"""Tap design (host, f64): futuredsp::firdes::kaiser and firdes::hilbert (crates/futuredsp/src/firdes/basic.rs)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -30,3 +30,13 @@ class kaiser:
         lib.b2s_firdes_kaiser_multirate(interp, decim, half_polyphase_len, max_ripple,
                                         t.ctypes.data_as(C.POINTER(C.c_float)), n)
         return t
+
+
+def hilbert(window) -> np.ndarray:
+    """firdes::hilbert::<f32> (basic.rs:202-222): a 90-degree phase shifter with the window's (odd) length."""
+    w = np.ascontiguousarray(window, dtype=np.float64)
+    assert w.size % 2 == 1, "Must be an odd number"                          # basic.rs:204
+    t = np.zeros(w.size, np.float32)
+    lib.b2s_firdes_hilbert(w.ctypes.data_as(C.POINTER(C.c_double)), w.size, t.ctypes.data_as(C.POINTER(C.c_float)),
+                           w.size)
+    return t

@@ -400,12 +400,55 @@ int32_t b2s_flag_read(b2s_ctx *ctx, const uint32_t *d_flag, uint32_t *value);
 int32_t b2s_memcpy_d2d(b2s_ctx *ctx, void *dst, const void *src, size_t bytes); /* async, any two devices */
 int32_t b2s_memset(b2s_ctx *ctx, void *dst, int32_t byte, size_t bytes);         /* async */
 
+/* ---- stream plumbing of branching flowgraphs: Combine (src/blocks/combine.rs:102-136), Split (split.rs:95-126),
+ * StreamDuplicator (stream_duplicator.rs:66-93) and StreamDeinterleaver (stream_deinterleaver.rs:61-97).  Stateless
+ * context-level calls: (consumed, produced) is a pure function of the sizes, returned immediately; the kernels run
+ * asynchronously on the context's stream and allocate nothing.  The reference's closures are a closed catalogue here,
+ * each evaluated with un-fused IEEE f32 operations in the Rust expression's order: outputs are bit-identical to the
+ * reference (NaN payloads aside).  Slices need 4-byte alignment only; any offset and any length (0 and 1 included)
+ * work.  An output may coincide exactly with an input of the same item size (in place) or be disjoint from it;
+ * any other overlap is B2S_EINVAL.  A NULL slice is B2S_EINVAL when the call would process an item. */
+typedef enum {
+    B2S_COMBINE_ADD_F32 = 0,       /* f32, f32 -> f32: a + b                      (tests/combine.rs)   */
+    B2S_COMBINE_SUB_F32 = 1,       /* f32, f32 -> f32: i1 - i2                    (examples/m17)       */
+    B2S_COMBINE_MUL_F32 = 2,       /* f32, f32 -> f32: a * b                      (examples/cw)        */
+    B2S_COMBINE_CONJ_MUL_C32 = 3,  /* c32, c32 -> c32: a * b.conj()               (examples/wlan rx)   */
+    B2S_COMBINE_MAG_DIV_C32_F32 = 4, /* c32, f32 -> f32: a.norm() / b; norm = glibc hypotf (wlan rx)   */
+    B2S_COMBINE_TO_C32 = 5,        /* f32, f32 -> c32: Complex32::new(i, q)       (examples/ssb USB)   */
+    B2S_COMBINE_TO_C32_NEG_Q = 6   /* f32, f32 -> c32: Complex32::new(i, q * -1.0) (examples/ssb LSB)  */
+} b2s_combine_op;
+/* m = min(n_in0, n_in1, n_out_cap) items of each input are consumed and m produced (combine.rs:114-125) */
+int32_t b2s_combine_exec(b2s_ctx *ctx, b2s_combine_op op, const void *d_in0, size_t n_in0, const void *d_in1,
+                         size_t n_in1, void *d_out, size_t n_out_cap, size_t *consumed, size_t *produced);
+typedef enum {
+    B2S_SPLIT_RE_IM = 0,           /* c32 -> (f32 re, f32 im)                     (tests/split.rs)     */
+    B2S_SPLIT_DUP_F32 = 1          /* f32 -> (v, v)                               (examples/ssb)       */
+} b2s_split_op;
+/* m = min(n_in, n_out_cap) (split.rs:106-119); n_out_cap is the smaller of the two output slices */
+int32_t b2s_split_exec(b2s_ctx *ctx, b2s_split_op op, const void *d_in, size_t n_in, void *d_out0, void *d_out1,
+                       size_t n_out_cap, size_t *consumed, size_t *produced);
+/* One launch, the input read once, items of item_bytes = 4 or 8 (f32, Complex32, f64).  d_outs is a HOST array of
+ * n_outs device pointers; n_out_cap is the smallest free space over the outputs.
+ *   deinterleave == 0  StreamDuplicator: out_k[j] = in[j], m = min(n_in, n_out_cap), consumed = produced = m.
+ *   deinterleave != 0  StreamDeinterleaver: out_k[j] = in[j n_outs + k] over whole groups only,
+ *                      m = min(n_out_cap, n_in / n_outs), consumed = m n_outs, produced = m (per output).
+ * The output pointers travel in the kernel's parameter block: n_outs > 256 is B2S_EUNSUPPORTED.  Outputs must not
+ * overlap the input or each other. */
+int32_t b2s_fanout_exec(b2s_ctx *ctx, int32_t deinterleave, size_t item_bytes, const void *d_in, size_t n_in,
+                        void *const *d_outs, size_t n_outs, size_t n_out_cap, size_t *consumed, size_t *produced);
+
 /* ---- tap design, host side, f64 then cast (≙ futuredsp::firdes::kaiser, firdes/basic.rs:310-459)
  * Return the tap count; write taps only if cap is large enough (call with taps=NULL to size). */
 size_t b2s_firdes_kaiser_lowpass(double cutoff, double transition_bw, double max_ripple,
                                  float *taps, size_t cap);
 size_t b2s_firdes_kaiser_multirate(size_t interp, size_t decim, size_t half_polyphase_len,
                                    double max_ripple, float *taps, size_t cap);
+/* ≙ futuredsp::windows::hamming (windows.rs:68-120, gen_cos with {0.54, 0.46}): len f64 points, periodic != 0 computes
+ * len + 1 and drops the last.  Same count / cap convention; len == 0 returns 0. */
+size_t b2s_window_hamming(size_t len, int32_t periodic, double *out, size_t cap);
+/* ≙ futuredsp::firdes::hilbert (firdes/basic.rs:202-222): taps of the window's length, f64 then cast to f32.
+ * The reference asserts an odd length: an even (or zero) length returns 0 taps. */
+size_t b2s_firdes_hilbert(const double *window, size_t len, float *taps, size_t cap);
 
 #ifdef __cplusplus
 }

@@ -5,7 +5,9 @@
 //                                     (crates/futuredsp/src/lib.rs:48-68)
 //   futuredsp::{FirFilter, DecimatingFirFilter, PolyphaseResamplingFir, IirFilter}
 //   futuresdr::blocks::{Fir, FirBuilder, Iir, IirBuilder, Fft, Apply, PfbArbResampler, SignalSource,
-//                       SignalSourceBuilder, FixedPointPhase, Head}                       (src/blocks/*.rs)
+//                       SignalSourceBuilder, FixedPointPhase, Head, Combine, Split, Delay,
+//                       StreamDuplicator, StreamDeinterleaver}                          (src/blocks/*.rs)
+//   futuredsp::{firdes::hilbert, windows::hamming}
 //   futuresdr::runtime::{WorkIo, mocker::Mocker}                        (work_io.rs, mocker.rs)
 //
 // The reference is Rust; no Rust toolchain exists in this image, so this header is the
@@ -562,6 +564,145 @@ public:
 private:
     const Instance &inst_; size_t n_; Handle<b2s_spectrum, b2s_spectrum_destroy> h_;
 };
+
+// ---- stream plumbing of branching graphs (b2s_combine_exec / b2s_split_exec / b2s_fanout_exec) --------------------
+// ≙ blocks::Combine (src/blocks/combine.rs:31-137) for the b2s_combine_op catalogue; A, B, Out are the op's item types
+template <typename A, typename B, typename Out> class Combine {
+public:
+    Combine(const Instance &inst, b2s_combine_op op) : in0(inst), in1(inst), output(inst), inst_(inst), op_(op) {}
+    void work(WorkIo &io) {                                                        // combine.rs:102-136
+        const size_t i0_len = in0.len(), i1_len = in1.len();
+        size_t c = 0, m = 0;
+        check(b2s_combine_exec(inst_.get(), op_, in0.slice(), i0_len, in1.slice(), i1_len, output.slice(), output.capacity(),
+                               &c, &m), inst_.get());
+        if (m > 0) { in0.consume(m); in1.consume(m); output.produce(m); }
+        if (in0.finished() && m == i0_len) io.finished = true;
+        if (in1.finished() && m == i1_len) io.finished = true;
+    }
+    Reader<A> in0;
+    Reader<B> in1;
+    Writer<Out> output;
+private:
+    const Instance &inst_; b2s_combine_op op_;
+};
+
+// ≙ blocks::Split (src/blocks/split.rs:31-127): RE_IM (In = Complex32) or DUP_F32 (In = float), two f32 outputs
+template <typename In> class Split {
+public:
+    Split(const Instance &inst, b2s_split_op op) : input(inst), output0(inst), output1(inst), inst_(inst), op_(op) {}
+    void work(WorkIo &io) {                                                        // split.rs:95-126
+        const size_t i_len = input.len();
+        size_t c = 0, m = 0;
+        check(b2s_split_exec(inst_.get(), op_, input.slice(), i_len, output0.slice(), output1.slice(),
+                             std::min(output0.capacity(), output1.capacity()), &c, &m), inst_.get());
+        if (m > 0) { input.consume(m); output0.produce(m); output1.produce(m); }
+        if (input.finished() && m == i_len) io.finished = true;
+    }
+    Reader<In> input;
+    Writer<float> output0, output1;
+private:
+    const Instance &inst_; b2s_split_op op_;
+};
+
+// ≙ blocks::Delay (src/blocks/delay.rs:31-169): n > 0 pads n zero items, n <= 0 skips -n items, then copies
+template <typename T> class Delay {
+public:
+    enum class State { Pad, Skip, Copy };
+    Delay(const Instance &inst, int64_t n) : input(inst), output(inst), inst_(inst) {
+        if (n > 0) { state_ = State::Pad; n_ = (size_t)n; } else { state_ = State::Skip; n_ = (size_t)(-n); }
+    }
+    State state() const { return state_; }
+    size_t count() const { return n_; }
+    // the new_value message handler (delay.rs:68-105)
+    void new_value(bool pad, size_t value) {
+        const int64_t val = pad ? (int64_t)value : -(int64_t)value;
+        const int64_t cur = state_ == State::Pad ? (int64_t)n_ : state_ == State::Skip ? -(int64_t)n_ : 0;
+        const int64_t nv = cur + val;
+        if (nv > 0) { state_ = State::Pad; n_ = (size_t)nv; }
+        else if (nv == 0) { state_ = State::Copy; n_ = 0; }
+        else { state_ = State::Skip; n_ = (size_t)(-nv); }
+    }
+    void work(WorkIo &io) {                                                        // delay.rs:114-168
+        const size_t i_len = input.len(), o_len = output.capacity();
+        if (state_ == State::Pad) {
+            const size_t m = std::min(o_len, n_);
+            if (m) check(b2s_memset(inst_.get(), output.slice(), 0, m * sizeof(T)), inst_.get());
+            output.produce(m);
+            if (m == n_) {
+                state_ = State::Copy; n_ = 0;
+                io.call_again = true;
+                if (input.finished()) io.finished = true;
+            } else n_ -= m;
+        } else if (state_ == State::Skip) {
+            const size_t m = std::min(i_len, n_);
+            input.consume(m);
+            if (m == n_) { state_ = State::Copy; n_ = 0; io.call_again = true; }
+            else n_ -= m;
+            if (input.finished() && m == i_len) io.finished = true;
+        } else {
+            const size_t m = std::min(i_len, o_len);
+            if (m) check(b2s_memcpy_d2d(inst_.get(), output.slice(), input.slice(), m * sizeof(T)), inst_.get());
+            input.consume(m);
+            output.produce(m);
+            if (input.finished() && m == i_len) io.finished = true;
+        }
+    }
+    Reader<T> input;
+    Writer<T> output;
+private:
+    const Instance &inst_; State state_; size_t n_ = 0;
+};
+
+// One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
+template <typename T, int32_t Deinterleave> class FanOut {
+    static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");
+public:
+    FanOut(const Instance &inst, size_t n) : input(inst), inst_(inst), n_(n) {
+        if (n == 0) throw Error(B2S_EINVAL, "stream fan-out: at least one output");
+        if (n > 256) throw Error(B2S_EUNSUPPORTED, "stream fan-out: at most 256 outputs in one launch");
+        for (size_t k = 0; k < n; k++) outs_.push_back(std::make_unique<Writer<T>>(inst));
+    }
+    Writer<T> &out(size_t k) { return *outs_.at(k); }
+    size_t num_outputs() const { return n_; }
+    void work(WorkIo &io) {                           // stream_duplicator.rs:66-93, stream_deinterleaver.rs:61-97
+        const size_t n_in = input.len();
+        size_t cap = SIZE_MAX;
+        std::vector<void *> ptrs(n_);
+        for (size_t k = 0; k < n_; k++) { cap = std::min(cap, outs_[k]->capacity()); ptrs[k] = outs_[k]->slice(); }
+        size_t c = 0, m = 0;
+        check(b2s_fanout_exec(inst_.get(), Deinterleave, sizeof(T), input.slice(), n_in, ptrs.data(), n_, cap, &c, &m),
+              inst_.get());
+        if (m > 0) {
+            for (auto &o : outs_) o->produce(m);
+            input.consume(c);
+        }
+        if (Deinterleave ? (n_in - c < n_ && input.finished()) : (n_in - m == 0 && input.finished())) io.finished = true;
+    }
+    Reader<T> input;
+private:
+    const Instance &inst_; size_t n_; std::vector<std::unique_ptr<Writer<T>>> outs_;
+};
+// ≙ blocks::StreamDuplicator<T, N> (stream_duplicator.rs:20-94): outputs[k] = input
+template <typename T> using StreamDuplicator = FanOut<T, 0>;
+// ≙ blocks::StreamDeinterleaver<T> (stream_deinterleaver.rs:25-98): output[k][j] = input[j N + k], whole groups only
+template <typename T> using StreamDeinterleaver = FanOut<T, 1>;
+
+// ---- firdes::hilbert (firdes/basic.rs:202-222) and windows::hamming (windows.rs:109-120) ---------------------------
+namespace windows {
+inline std::vector<double> hamming(size_t len, bool periodic) {
+    std::vector<double> w(len);
+    if (len) b2s_window_hamming(len, periodic ? 1 : 0, w.data(), len);
+    return w;
+}
+}  // namespace windows
+namespace firdes {
+inline std::vector<float> hilbert(const std::vector<double> &window) {
+    if (window.size() % 2 == 0) throw Error(B2S_EINVAL, "firdes::hilbert: Must be an odd number");   // basic.rs:204
+    std::vector<float> t(window.size());
+    b2s_firdes_hilbert(window.data(), window.size(), t.data(), t.size());
+    return t;
+}
+}  // namespace firdes
 
 // ≙ runtime::mocker::Mocker (mocker.rs:33-190): run one block without a scheduler
 template <typename Block> class Mocker {

@@ -44,7 +44,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 
 def want(section):
-    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, scale)."""
+    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -126,6 +126,109 @@ def sigsrc_section(quick):
         sec = time.perf_counter() - t0
         print(json.dumps({"kernel": f"sigsrc_oracle_1thread_{name}", "items": nc,
                           "Gsamples_s": round(nc / sec / 1e9, 4), "note": "CPU, one thread"}), flush=True)
+
+
+def stream_section(quick):
+    """Combine / Split / StreamDuplicator / StreamDeinterleaver kernels on 64 Mi items per call, as fractions of the
+    3.35 TB/s data-sheet figure computed from algorithmic bytes; the numpy restatement on one CPU thread beside each;
+    and the WLAN receiver front end (rx.rs:73-93) as an end-to-end graph rate through edges.Flowgraph."""
+    import subprocess
+    import ctypes as C
+    from futuresdr_b200 import _lib
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({"kernel": "stream_device", "gpu": q[torch.cuda.current_device()] if q else "unknown"}), flush=True)
+    n = (16 if quick else 64) << 20
+    nc = 4 << 20
+    g = torch.Generator(device="cuda").manual_seed(5)
+    ctx = fb.default_context().handle
+
+    def line(name, nbytes, sec, cpu_sec):
+        gbs = nbytes / sec / 1e9
+        print(json.dumps({"kernel": name, "items": n, "ms": round(sec * 1e3, 4), "Gitems_s": round(n / sec / 1e9, 2),
+                          "alg_GBs": round(gbs, 1), "frac_3350GBs": round(gbs / 3350.0, 4),
+                          "cpu_1thread_Gitems_s": round(nc / cpu_sec / 1e9, 4)}), flush=True)
+
+    def cpu_time(fn):
+        fn()
+        t0 = time.perf_counter()
+        fn()
+        return time.perf_counter() - t0
+
+    c64 = lambda m: torch.view_as_complex(torch.randn(m, 2, generator=g, device="cuda"))  # noqa: E731
+    a, b = c64(n), c64(n)
+    bf = torch.rand(n, generator=g, device="cuda") + 0.5
+    oc = torch.empty(n, dtype=torch.complex64, device="cuda")
+    of = torch.empty(n, device="cuda")
+    ha, hb, hf = a[:nc].cpu().numpy(), b[:nc].cpu().numpy(), bf[:nc].cpu().numpy()
+    cb, cp = C.c_size_t(0), C.c_size_t(0)
+
+    def comb(op, x, y, o):
+        return lambda: _lib.lib.b2s_combine_exec(ctx, op, C.c_void_p(x.data_ptr()), n, C.c_void_p(y.data_ptr()), n,
+                                                 C.c_void_p(o.data_ptr()), n, C.byref(cb), C.byref(cp))
+
+    def np_conj_mul():
+        r = np.empty(nc, np.complex64)
+        r.real = ha.real * hb.real - ha.imag * (-hb.imag)
+        r.imag = ha.real * (-hb.imag) + ha.imag * hb.real
+    sec = timeit(comb(_lib.COMBINE_CONJ_MUL_C32, a, b, oc), iters=20, warm=3)
+    line("combine_conj_mul_c32", 24 * n, sec, cpu_time(np_conj_mul))
+    sec = timeit(comb(_lib.COMBINE_MAG_DIV_C32_F32, a, bf, of), iters=20, warm=3)
+    line("combine_mag_div_c32_f32", 16 * n, sec, cpu_time(lambda: np.hypot(ha.real, ha.imag) / hf))
+    o1 = torch.empty(n, device="cuda")
+    sec = timeit(lambda: _lib.lib.b2s_split_exec(ctx, _lib.SPLIT_RE_IM, C.c_void_p(a.data_ptr()), n,
+                                                 C.c_void_p(of.data_ptr()), C.c_void_p(o1.data_ptr()), n, C.byref(cb),
+                                                 C.byref(cp)), iters=20, warm=3)
+    line("split_re_im", 16 * n, sec, cpu_time(lambda: (ha.real.copy(), ha.imag.copy())))
+    del o1
+    for dt, s in ((torch.float32, 4), (torch.complex64, 8)):
+        src = (torch.randn(n, generator=g, device="cuda") if dt == torch.float32 else a)
+        hsrc = src[:nc].cpu().numpy()
+        for N in (2, 4):
+            outs = [torch.empty(n, dtype=dt, device="cuda") for _ in range(N)]
+            ptrs = (C.c_void_p * N)(*[o.data_ptr() for o in outs])
+            sec = timeit(lambda: _lib.lib.b2s_fanout_exec(ctx, 0, s, C.c_void_p(src.data_ptr()), n, ptrs, N, n,
+                                                          C.byref(cb), C.byref(cp)), iters=10, warm=2)
+            line(f"duplicate_{'f32' if s == 4 else 'c32'}_N{N}", (1 + N) * s * n, sec,
+                 cpu_time(lambda: [hsrc.copy() for _ in range(N)]))
+            del outs
+        for N in (2, 4, 16, 256):
+            per = n // N
+            outs = [torch.empty(per, dtype=dt, device="cuda") for _ in range(N)]
+            ptrs = (C.c_void_p * N)(*[o.data_ptr() for o in outs])
+            sec = timeit(lambda: _lib.lib.b2s_fanout_exec(ctx, 1, s, C.c_void_p(src.data_ptr()), per * N, ptrs, N, per,
+                                                          C.byref(cb), C.byref(cp)), iters=10, warm=2)
+            line(f"deinterleave_{'f32' if s == 4 else 'c32'}_N{N}", 2 * s * per * N, sec,
+                 cpu_time(lambda: [hsrc[k::N].copy() for k in range(N)]))
+            del outs
+    del a, b, bf, oc, of
+    torch.cuda.empty_cache()
+    # whole graph, end to end: source stream already on the device is not possible through VectorSource, so the rate
+    # includes the host -> device copy of the source and the device -> host copies of the sink
+    from futuresdr_b200.blocks import Apply, ApplyOp, Fir
+    from futuresdr_b200.edges import Flowgraph, VectorSink, VectorSource
+    ns = (4 if quick else 16) << 20
+    x = (np.random.default_rng(0).standard_normal(2 * ns).astype(np.float32).view(np.complex64))
+    best = None
+    for _ in range(3):
+        fg = Flowgraph()
+        src, delay = VectorSource(x), fb.Delay(np.complex64, 16)
+        mag2, mult = Apply(ApplyOp.NormSqr), fb.Combine(fb.CombineOp.ConjMulC32)
+        favg = Fir(fb.FirFilter(np.ones(64, np.float32), sample_dtype=np.float32))
+        cavg = Fir(fb.FirFilter(np.ones(48, np.float32), sample_dtype=np.complex64))
+        div, snk = fb.Combine(fb.CombineOp.MagDivC32F32), VectorSink(np.float32)
+        for args in ((src, delay), (src, mag2), (src, mult, "in0"), (delay, mult, "in1"), (mag2, favg),
+                     (mult, cavg), (cavg, div, "in0"), (favg, div, "in1"), (div, snk)):
+            fg.connect(*args)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "wlan_rx_front_end_graph", "items": ns, "s": round(best, 4),
+                      "Gsamples_s_end_to_end": round(ns / best / 1e9, 4),
+                      "note": "whole graph, end to end: VectorSource H2D + Delay + NormSqr + 2 FIR + 2 Combine + "
+                              "VectorSink D2H, driven by edges.Flowgraph from Python"}), flush=True)
 
 
 def main():
@@ -309,6 +412,8 @@ def main():
         iir_section(quick)
     if want("sigsrc"):
         sigsrc_section(quick)
+    if want("stream"):
+        stream_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
