@@ -175,10 +175,11 @@ __device__ __forceinline__ void chan_cp_async16(void *dst_smem, const void *src,
 // Persistent: a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... and the input tile of the NEXT one is fetched
 // with cp.async into the other half of a double buffer while the current one is filtered, transformed and stored
 // (a load, wait, compute sequence leaves the CTA stalled on its global loads).
-template <int LOG2N, int TPAD>
+template <int LOG2N, int TPAD, bool PADDED>
 __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restrict__ in, const float *__restrict__ arms_pad,
-                                                         const float2 *__restrict__ tw, float2 *__restrict__ out, int base0,
-                                                         long long o_first, long long nprod, long long out_stride, int ntiles) {
+                                                         const float2 *__restrict__ tw, float2 *__restrict__ out, int T,
+                                                         int base0, long long o_first, long long nprod, long long out_stride,
+                                                         int ntiles) {
     using namespace fftk;
     constexpr FftGeom G = fft_geom(LOG2N, 256);
     constexpr int N = G.n, TT = G.t, NP = G.np;              // TT threads per transform
@@ -230,7 +231,7 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
         {
             float2 acc[RL];
             // tile row (run*RL + k) <-> sample row o_run - TPAD + 1 + k
-            pfb_bank_column<N, RL, TPAD>(X + (size_t)(run * RL) * N + r, tap, acc);
+            pfb_bank_column<N, RL, TPAD, PADDED>(X + (size_t)(run * RL) * N + r, tap, T, acc);
 #pragma unroll
             for (int u = 0; u < RL; u++)                      // conjugated: the inverse transform is conj(FFT(conj(.)))
                 V[(size_t)(run * RL + u) * NP + pad(b)] = make_float2(acc[u].x, -acc[u].y);
@@ -261,18 +262,18 @@ template <int LOG2N, int TPAD> constexpr size_t chan_fused_smem() {
 
 static inline bool ntiles_overflow(long long nprod, long long o_first, int ob) { return (nprod - o_first) / ob > 0x7fffff00ll; }
 
-template <int LOG2N, int TPAD>
+template <int LOG2N, int TPAD, bool PADDED>
 int32_t chan_fused_launch(b2s_chan *c, const float2 *in, float2 *out, long long o_first, long long nprod, long long out_stride) {
     constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = chan_fused_smem<LOG2N, TPAD>();
     if (ntiles_overflow(nprod, o_first, OB)) return b2s_fail(c->ctx, B2S_EUNSUPPORTED, "channelizer: too many output vectors in one call");
-    constexpr auto kern = chan_fused_kernel<LOG2N, TPAD>;
+    constexpr auto kern = chan_fused_kernel<LOG2N, TPAD, PADDED>;
     int resident = 1;
     B2S_TRY(smem_optin<kern>(c->ctx, smem, 256, &resident));
     const size_t ntiles = ceil_div((size_t)(nprod - o_first), (size_t)OB);
     const unsigned grid = (unsigned)std::min<size_t>(ntiles, (size_t)c->ctx->sm_count * resident);
-    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->taps.arms_pad.get(), b2s_fft_twiddles(c->ifft.get()), out, (int)c->base_index, o_first,
-                                             nprod, out_stride, (int)ntiles);
+    kern<<<grid, 256, smem, c->ctx->stream>>>(in, c->taps.arms_pad.get(), b2s_fft_twiddles(c->ifft.get()), out, (int)c->T,
+                                             (int)c->base_index, o_first, nprod, out_stride, (int)ntiles);
     B2S_CHECK_LAUNCH(c->ctx);
     return B2S_OK;
 }
@@ -344,8 +345,8 @@ int32_t b2s_chan_exec(b2s_chan *c, const void *d_in, size_t n_in, void *d_out, s
     const size_t n_generic = fused_ok ? std::min<size_t>(nprod, (size_t)T - 1) : nprod;
     NvtxRange nvtx("b2s_chan_exec");
     if (n_generic < nprod) {
-        const int32_t rc = pfb_fused_dispatch(b2s_fft_log2n(c->ifft.get()), c->taps.tpad, [&](auto L, auto P) {
-            return chan_fused_launch<L, P>(c, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
+        const int32_t rc = pfb_fused_dispatch(b2s_fft_log2n(c->ifft.get()), c->taps.tpad, c->T, [&](auto L, auto P, auto D) {
+            return chan_fused_launch<L, P, D>(c, in, (float2 *)d_out, (long long)n_generic, (long long)nprod, (long long)out_stride);
         });
         if (rc != B2S_OK) return rc == B2S_EAGAIN ? b2s_fail(ctx, B2S_ESTATE, "channelizer: fused shape mismatch") : rc;
     }

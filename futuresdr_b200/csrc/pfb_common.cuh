@@ -39,6 +39,9 @@ struct PfbWindows {
 
     int32_t init(b2s_ctx *ctx, int w, int t, bool mir, const char *what) {
         W = w; T = t; mirror = mir;
+        if ((size_t)T * sizeof(float2) > ctx->smem_optin)      // slide() stages one window in shared memory
+            return b2s_fail(ctx, B2S_EUNSUPPORTED, "%s: %d taps per window exceed the %zu bytes of shared memory a CTA can have",
+                            what, T, ctx->smem_optin);
         B2S_TRY(hist.alloc(ctx, (size_t)W * T, what));
         return reset(ctx);
     }
@@ -117,7 +120,9 @@ inline int32_t PfbWindows::push(b2s_ctx *ctx, const float2 *in, size_t n) {
 }
 
 inline int32_t PfbWindows::slide(b2s_ctx *ctx, const float2 *in, long long c0, long long n) {
-    pfb_slide_kernel<<<(unsigned)W, 64, T * sizeof(float2), ctx->stream>>>(hist.get(), in, W, T, mirror, c0, n);
+    const size_t bytes = (size_t)T * sizeof(float2);   // one window in shared memory: above 48 KiB (T > 6144) only opted in
+    if (bytes > 48 * 1024) B2S_TRY(smem_optin<pfb_slide_kernel>(ctx, ctx->smem_optin));
+    pfb_slide_kernel<<<(unsigned)W, 64, bytes, ctx->stream>>>(hist.get(), in, W, T, mirror, c0, n);
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }
@@ -138,10 +143,14 @@ inline int pfb_fused_tpad(int log2n, size_t T) {
     return T <= 8 ? 8 : (T <= 16 ? 16 : 32);
 }
 
-// f(L, P) with L = log2n and P = tpad as std::integral_constant: the instantiations of a fused kernel; B2S_EAGAIN for a
-// shape outside them
-template <typename F> int32_t pfb_fused_dispatch(int log2n, int tpad, F &&f) {
-    auto at = [&](auto P) { return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN, [&](auto L) { return f(L, P); }); };
+// f(L, P, D) with L = log2n, P = tpad and D = (T < tpad) as std::integral_constant: the instantiations of a fused kernel;
+// B2S_EAGAIN for a shape outside them
+template <typename F> int32_t pfb_fused_dispatch(int log2n, int tpad, size_t T, F &&f) {
+    auto at = [&](auto P) {
+        return fftk::with_log2n<2, 8>(log2n, B2S_EAGAIN, [&](auto L) {
+            return T < (size_t)tpad ? f(L, P, std::true_type{}) : f(L, P, std::false_type{});
+        });
+    };
     switch (tpad) {
         case 8: return at(std::integral_constant<int, 8>{});
         case 16: return at(std::integral_constant<int, 16>{});
@@ -174,8 +183,10 @@ struct PfbBankTaps {
 // first; output u of the run is the window ending at row u + TPAD - 1 with tap j on its j-th newest sample.  The column
 // is streamed through registers once and every sample is multiplied into each output that contains it (taps in
 // registers, static indices after unrolling), so every output accumulates oldest sample first like the reference.
-template <int N, int RL, int TPAD>
-__device__ __forceinline__ void pfb_bank_column(const float2 *col, const float (&tap)[TPAD], float2 (&acc)[RL]) {
+// PADDED (T < TPAD): the padded taps j >= T are skipped, not multiplied -- 0 * inf is NaN, and a non-finite sample must
+// reach exactly the T outputs it reaches in the reference.  Unpadded banks (T == TPAD) are compiled without the guard.
+template <int N, int RL, int TPAD, bool PADDED>
+__device__ __forceinline__ void pfb_bank_column(const float2 *col, const float (&tap)[TPAD], int T, float2 (&acc)[RL]) {
 #pragma unroll
     for (int u = 0; u < RL; u++) acc[u] = make_float2(0.f, 0.f);
 #pragma unroll
@@ -184,7 +195,7 @@ __device__ __forceinline__ void pfb_bank_column(const float2 *col, const float (
 #pragma unroll
         for (int u = 0; u < RL; u++) {
             const int j = u + TPAD - 1 - k;          // output u sees this row as its j-th newest sample
-            if (j >= 0 && j < TPAD) mac(acc[u], x, tap[j]);
+            if (j >= 0 && j < TPAD && (!PADDED || j < T)) mac(acc[u], x, tap[j]);
         }
     }
 }

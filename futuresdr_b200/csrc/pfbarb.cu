@@ -63,6 +63,23 @@ struct b2s_pfbarb {
 
 namespace {
 
+// `bf.floor() as usize` (arb_resampler.rs:136): Rust's float -> integer cast saturates -- negative and NaN give 0.  With
+// rate > num_filters, tau is still negative when the output after a Boundary state advances it, so bf < 0 does occur; a
+// plain C cast of a negative float to an unsigned type is undefined (it wraps to 0xFFFFFFFF on x86-64) and would stop
+// the timing loop for good.
+__host__ __device__ __forceinline__ uint32_t pfb_arm_index(float bf) {
+    const float f = floorf(bf);
+    return f > 0.f ? (f < 4294967296.f ? (uint32_t)f : 0xffffffffu) : 0u;
+}
+
+// Outputs one input sample can produce, at most.  A sample starts with tau >= -1/N (tau >= (N-1)/N when the Boundary
+// state is entered, then tau -= 1) and emits one output per step of `delay` until tau >= 1: at most
+// ceil(rate * (1 + 1/N)) outputs.  For rate <= N that is ceil(rate) + 1; above it, 2 more for f32 rounding.
+inline size_t pfbarb_per_sample_max(float rate, size_t num_filters) {
+    if (rate <= (float)num_filters) return (size_t)std::ceil(rate) + 1;
+    return (size_t)std::ceil((double)rate * (1.0 + 1.0 / (double)num_filters)) + 2;
+}
+
 __device__ __forceinline__ float2 pfb_x(const float2 *__restrict__ hist, const float2 *__restrict__ in, int L,
                                         long long idx) {
     return idx < L ? hist[idx] : __ldg(in + (idx - L));
@@ -154,7 +171,7 @@ __global__ void __launch_bounds__(kPaThreads) pfb_kernel(const PaParams P) {
                     o++;
                     tau = __fadd_rn(tau, delay);
                     const float bf = __fmul_rn(tau, fN);
-                    base = (uint32_t)floorf(bf);
+                    base = pfb_arm_index(bf);
                     mu = __fsub_rn(bf, (float)base);
                     boundary = false;
                 } else if (base == (uint32_t)(N - 1)) {
@@ -165,7 +182,7 @@ __global__ void __launch_bounds__(kPaThreads) pfb_kernel(const PaParams P) {
                     o++;
                     tau = __fadd_rn(tau, delay);
                     const float bf = __fmul_rn(tau, fN);
-                    base = (uint32_t)floorf(bf);
+                    base = pfb_arm_index(bf);
                     mu = __fsub_rn(bf, (float)base);
                 }
             }
@@ -257,14 +274,14 @@ struct Timing {
         while (base < N) {
             if (boundary) {
                 o++;
-                tau = tau + delay; const float bf = tau * fN; base = (uint32_t)floorf(bf); mu = bf - (float)base;
+                tau = tau + delay; const float bf = tau * fN; base = pfb_arm_index(bf); mu = bf - (float)base;
                 boundary = false;
             } else if (base == N - 1) {
                 boundary = true;
                 base = N;
             } else {
                 o++;
-                tau = tau + delay; const float bf = tau * fN; base = (uint32_t)floorf(bf); mu = bf - (float)base;
+                tau = tau + delay; const float bf = tau * fN; base = pfb_arm_index(bf); mu = bf - (float)base;
             }
         }
         tau = tau - 1.0f;
@@ -345,8 +362,10 @@ int32_t b2s_pfbarb_plan_c32(b2s_ctx *ctx, const float *taps, size_t ntaps, size_
     if (!(rate > 0.f)) return b2s_fail(ctx, B2S_EINVAL, "PfbArbResampler: resampling rate must be greater than zero");
     if (num_filters == 0) return b2s_fail(ctx, B2S_EINVAL, "PfbArbResampler: number of filter banks must be greater than zero");
     if (ntaps < num_filters) return b2s_fail(ctx, B2S_EINVAL, "PfbArbResampler: prototype filter length must be at least num_filters");
-    // a 32-sample sub-block must fit the descriptor tile of a CTA: (ceil(rate) + 1) * 32 <= kDescCap
-    if (num_filters > (1u << 20) || rate > 126.f) return b2s_fail(ctx, B2S_EUNSUPPORTED, "PfbArbResampler: num_filters / rate too large (rate <= 126)");
+    // a 32-sample sub-block must fit the descriptor tile of a CTA: pfbarb_per_sample_max * 32 <= kDescCap (rate <= 126
+    // with at least as many arms as the rate, less above it)
+    if (num_filters > (1u << 20) || rate > 126.f || pfbarb_per_sample_max(rate, num_filters) * kSB > (size_t)kDescCap)
+        return b2s_fail(ctx, B2S_EUNSUPPORTED, "PfbArbResampler: rate %f too large for %zu arms (a sample may produce more outputs than one CTA holds)", (double)rate, num_filters);
     DeviceGuard g(ctx->device);
     PlanPtr<b2s_pfbarb> p(new b2s_pfbarb());
     p->ctx = ctx; p->num_filters = num_filters; p->ntaps = ntaps; p->rate = rate;
@@ -448,7 +467,7 @@ int32_t b2s_pfbarb_exec(b2s_pfbarb *p, const void *d_in, size_t n_in, void *d_ou
     }
     P.nout = (long long)nout;
     // CTA tiling: sub-blocks per CTA so that a CTA never exceeds kDescCap outputs
-    const size_t per_sample_max = (size_t)std::ceil(p->rate) + 1;
+    const size_t per_sample_max = pfbarb_per_sample_max(p->rate, p->num_filters);
     size_t sub_per_cta = kDescCap / (per_sample_max * P.sb_len);
     if (sub_per_cta == 0) return b2s_fail(ctx, B2S_EUNSUPPORTED, "pfbarb: rate %f too high for the descriptor tile", (double)p->rate);
     sub_per_cta = std::min<size_t>(sub_per_cta, kPaThreads);

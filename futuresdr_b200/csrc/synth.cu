@@ -63,7 +63,7 @@ __global__ void synth_bank_kernel(const float2 *__restrict__ spun /* steady vect
 // The first vectors of a call (windows still reaching into the previous call's history; one tile, more when a tile is
 // shorter than the history), the window fill and other bank shapes take the three-kernel path.
 // ---------------------------------------------------------------------------------------------------------------
-template <int LOG2N, int TPAD>
+template <int LOG2N, int TPAD, bool PADDED>
 __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restrict__ in, long long in_stride,
                                                           const float *__restrict__ arms_pad, const float2 *__restrict__ tw,
                                                           float2 *__restrict__ out, float2 *__restrict__ hist, int T,
@@ -107,7 +107,7 @@ __global__ void __launch_bounds__(256) synth_fused_kernel(const float2 *__restri
             // ---- C: FIR bank
             float2 acc[RL];
             // ring row (run*RL + k) <-> vector v0 + run*RL + k - (TPAD-1)
-            pfb_bank_column<N, RL, TPAD>(Sb + (size_t)(run * RL) * N + w, tap, acc);
+            pfb_bank_column<N, RL, TPAD, PADDED>(Sb + (size_t)(run * RL) * N + w, tap, T, acc);
 #pragma unroll
             for (int u = 0; u < RL; u++) {
                 const long long uu = v0 + run * RL + u;
@@ -148,11 +148,11 @@ template <int LOG2N, int TPAD> constexpr size_t synth_fused_smem() {
     return ((size_t)G.n * (G.fpb + 1) + (size_t)G.fpb * G.np + (size_t)(TPAD - 1 + G.fpb) * G.n) * sizeof(float2);
 }
 
-template <int LOG2N, int TPAD>
+template <int LOG2N, int TPAD, bool PADDED>
 int32_t synth_fused_launch(b2s_synth *s, const float2 *in, long long in_stride, float2 *out, long long k2) {
     constexpr int OB = fftk::fft_geom(LOG2N, 256).fpb;
     constexpr size_t smem = synth_fused_smem<LOG2N, TPAD>();
-    constexpr auto kern = synth_fused_kernel<LOG2N, TPAD>;
+    constexpr auto kern = synth_fused_kernel<LOG2N, TPAD, PADDED>;
     int resident = 1;
     B2S_TRY(smem_optin<kern>(s->ctx, smem, 256, &resident));
     constexpr int WARM = (TPAD - 1 + OB - 1) / OB;
@@ -260,8 +260,8 @@ int32_t b2s_synth_exec(b2s_synth *s, const void *d_in, size_t in_stride, size_t 
     }
     if (fused) {
         // (the generic bank kernel above has read the old history; the fused kernel writes the new one)
-        const int32_t frc = pfb_fused_dispatch(l2n, tpad, [&](auto L, auto P) {
-            return synth_fused_launch<L, P>(s, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
+        const int32_t frc = pfb_fused_dispatch(l2n, tpad, T, [&](auto L, auto P, auto D) {
+            return synth_fused_launch<L, P, D>(s, (const float2 *)d_in, (long long)in_stride, (float2 *)d_out, (long long)k2_all);
         });
         if (frc != B2S_OK) return frc == B2S_EAGAIN ? b2s_fail(ctx, B2S_ESTATE, "synthesizer: fused shape mismatch") : frc;
     } else if (k2) {

@@ -281,7 +281,7 @@ def main():
             po = torch.empty(n // 3 + 2 * N, dtype=torch.float32, device="cuda")
             sec = timeit(lambda: sp.process(x[:n], po), iters=5, warm=2)
             report(f"spectrum_pipe_fused_{N}", n, 8 * n + 4 * (n // 3), sec, extra="FFT + |x|^2 + MovingAvg(0.1, 3): spectrum_kernel + scan + fixup")
-        for N, T in ((64, 16), (16, 16), (256, 8)):
+        for N, T in ((64, 16), (16, 16), (256, 8), (64, 12)):         # 64 x 12: padded to 16 taps
             ctaps = (orc.kaiser_lowpass(0.4 / N, 0.1 / N, 1e-3)).astype(np.float32)
             ctaps = np.resize(ctaps, N * T)
             ch = B.PfbChannelizer(N, ctaps, 1.0)
@@ -295,7 +295,7 @@ def main():
             sec = timeit(run_ch, iters=5, warm=1)
             report(f"pfb_channelizer_fused_{N}ch_{T}taps", n, 16 * n, sec, extra="FIR bank + IFFT + transposed store in one launch")
     if want("synth"):
-        for N, T in ((64, 16), (16, 16)):
+        for N, T in ((64, 16), (16, 16), (64, 12)):                    # 64 x 12: padded to 16 taps
             staps = np.resize((orc.kaiser_lowpass(0.4 / N, 0.1 / N, 1e-3)).astype(np.float32), N * T)
             syn = B.PfbSynthesizer(N, staps)
             nv = n // N
