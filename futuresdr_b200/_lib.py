@@ -141,6 +141,10 @@ SIGNATURES = {
     "b2s_combine_exec": (_i32, [_vp, C.c_int, _vp, _sz, _vp, _sz, _vp, _sz, _szp, _szp]),
     "b2s_split_exec": (_i32, [_vp, C.c_int, _vp, _sz, _vp, _vp, _sz, _szp, _szp]),
     "b2s_fanout_exec": (_i32, [_vp, _i32, _sz, _vp, _sz, _vpp, _sz, _sz, _szp, _szp]),
+    "b2s_boxavg_create": (_i32, [_vp, _i32, _sz, _i32, _f32, _vpp]),
+    "b2s_boxavg_destroy": (None, [_vp]),
+    "b2s_boxavg_reset": (_i32, [_vp]),
+    "b2s_boxavg_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _sz, _szp, _szp, _szp, _i32p, _i32p]),
     "b2s_window_hamming": (_sz, [_sz, _i32, C.POINTER(C.c_double), _sz]),
     "b2s_firdes_hilbert": (_sz, [C.POINTER(C.c_double), _sz, _f32p, _sz]),
 }

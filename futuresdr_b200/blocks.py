@@ -10,6 +10,7 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``PfbArbResampler``           src/blocks/pfb/arb_resampler.rs:72-231
   * ``Combine`` / ``Split``       src/blocks/combine.rs:31-137, split.rs:31-127 (closed catalogues of closures)
   * ``Delay``                     src/blocks/delay.rs:31-169
+  * ``MovingAverage``             examples/wlan/src/moving_average.rs:27-107, examples/m17/src/moving_average.rs:5-81
   * ``StreamDuplicator`` / ``StreamDeinterleaver``   src/blocks/stream_duplicator.rs, stream_deinterleaver.rs
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
@@ -865,6 +866,56 @@ class Delay(Block):
             self.output.produce(m)
             if self.input.finished() and m == i_len:
                 io.finished = True
+
+
+class MovingAverage(Block, Handle):
+    """The WLAN and M17 receivers' MovingAverage (examples/wlan/src/moving_average.rs:27-107, f32 and Complex32;
+    examples/m17/src/moving_average.rs:5-81, f32 with ``divisor=4800.0``): a box-car sum over ``len`` items, emitted
+    after ``len - 1`` leading zeros, so output k is the window that ENDS at input k.  Not ``MovingAvg`` (an
+    exponential average per bin over fixed-width chunks).
+
+    Each reference work() call restarts a strict-order f32 running sum and produces at most 4000 outputs, so the
+    rounding depends on where the calls fall; the device reproduces it bit for bit given the same calls.  One
+    ``work()`` runs the calls the reference would make back to back on the current slices until one makes no progress
+    (``max_calls=0``), or at most ``max_calls`` of them (``max_calls=1`` is exactly one reference work() call).
+    ``io.call_again`` and the finish rule (:103-105) are those of the last of these calls."""
+    _destroy = lib.b2s_boxavg_destroy
+
+    def __init__(self, dtype, len: int, divisor: Optional[float] = None, max_calls: int = 0,
+                 ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.in_dtype = self.out_dtype = np.dtype(dtype)
+        if self.in_dtype not in (_F32, _C32):
+            raise TypeError(f"MovingAverage: f32 or Complex32 items, not {self.in_dtype}")
+        self.len = int(len)
+        self.divisor = None if divisor is None else float(np.float32(divisor))
+        self.max_calls = int(max_calls)
+        self._h = C.c_void_p()
+        check(lib.b2s_boxavg_create(self.ctx.handle, int(self.in_dtype == _C32), self.len, int(divisor is not None),
+                                    float(self.divisor or 0.0), C.byref(self._h)), self.ctx.handle)
+        self._ports()
+
+    def average(self, i: torch.Tensor, o: torch.Tensor, max_calls: Optional[int] = None):
+        """One exec over device slices (asynchronous) -> (consumed, produced, calls, call_again, done)."""
+        c, p, n = C.c_size_t(0), C.c_size_t(0), C.c_size_t(0)
+        ca, dn = C.c_int32(0), C.c_int32(0)
+        check(lib.b2s_boxavg_exec(self._h, _ptr(i), i.numel(), _ptr(o), o.numel(),
+                                  self.max_calls if max_calls is None else int(max_calls), C.byref(c), C.byref(p),
+                                  C.byref(n), C.byref(ca), C.byref(dn)), self.ctx.handle)
+        return c.value, p.value, n.value, bool(ca.value), bool(dn.value)
+
+    def reset(self):
+        check(lib.b2s_boxavg_reset(self._h), self.ctx.handle)
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()
+        c, p, _, call_again, done = self.average(i, o)
+        self.input.consume(c)
+        self.output.produce(p)
+        if call_again:                                                          # :82-84
+            io.call_again = True
+        if self.input.finished() and done:                                      # :103-105
+            io.finished = True
 
 
 class _FanOut(Block):

@@ -437,6 +437,32 @@ int32_t b2s_split_exec(b2s_ctx *ctx, b2s_split_op op, const void *d_in, size_t n
 int32_t b2s_fanout_exec(b2s_ctx *ctx, int32_t deinterleave, size_t item_bytes, const void *d_in, size_t n_in,
                         void *const *d_outs, size_t n_outs, size_t n_out_cap, size_t *consumed, size_t *produced);
 
+/* ---- the WLAN and M17 receivers' MovingAverage (≙ examples/wlan/src/moving_average.rs:44-107, f32 and Complex32,
+ * output = sum; examples/m17/src/moving_average.rs:20-81, f32, output = sum / 4800.0).  Not MovingAvg (b2s_mavg).
+ * One reference work() call: while pad > 0 (pad starts at len - 1) it writes m = min(pad, n_out) zeros and consumes
+ * nothing, with call_again = m < n_out; afterwards it produces m = min(4000, (n_in + 1) - len (saturating), n_out)
+ * window sums, each a strict-order f32 running sum that restarts at the call (sum = fold of x[0 .. len-1] from -0.0
+ * for f32, from (+0, +0) for Complex32; then sum += x[i+len-1], out[i] = sum [/ divisor], sum -= x[i]), consumes m,
+ * and is finished iff the input is finished and m == (n_in + 1) - len (saturating).  The outputs depend on where the
+ * calls fall, so the device reproduces them bit for bit given the same sequence of calls (NaN payloads aside).
+ *   create: complex_items as in b2s_sigsrc_create; len == 0 and a divisor with complex_items are B2S_EINVAL.
+ *   exec:   emulates the calls the reference makes back to back on what is left of the slices -- the remaining pad,
+ *           then runs of up to 4000 outputs -- until a call makes no progress or max_calls calls have run
+ *           (max_calls == 0: no limit; 1: exactly one work() call).  *calls counts the emulated calls, the last
+ *           one included; *call_again and *done are that call's call_again and its m == (rem_in + 1) - len, which
+ *           the caller ANDs with input.finished().  The only state is pad, kept on the host: calls are
+ *           stream-ordered and never synchronise.  Slices need 4-byte alignment only; an output overlapping the
+ *           input it reads is B2S_EINVAL.
+ *   reset:  pad back to len - 1. */
+typedef struct b2s_boxavg b2s_boxavg;
+int32_t b2s_boxavg_create(b2s_ctx *ctx, int32_t complex_items, size_t len, int32_t has_divisor, float divisor,
+                          b2s_boxavg **out);
+void    b2s_boxavg_destroy(b2s_boxavg *p);
+int32_t b2s_boxavg_reset(b2s_boxavg *p);
+int32_t b2s_boxavg_exec(b2s_boxavg *p, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
+                        size_t max_calls, size_t *consumed, size_t *produced, size_t *calls, int32_t *call_again,
+                        int32_t *done);
+
 /* ---- tap design, host side, f64 then cast (≙ futuredsp::firdes::kaiser, firdes/basic.rs:310-459)
  * Return the tap count; write taps only if cap is large enough (call with taps=NULL to size). */
 size_t b2s_firdes_kaiser_lowpass(double cutoff, double transition_bw, double max_ripple,

@@ -20,6 +20,7 @@
 #include <cstdint>
 #include <cstring>
 #include <memory>
+#include <optional>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -651,6 +652,35 @@ public:
     Writer<T> output;
 private:
     const Instance &inst_; State state_; size_t n_ = 0;
+};
+
+// ≙ the WLAN and M17 receivers' MovingAverage (examples/wlan/src/moving_average.rs:27-107, T = float or Complex32;
+// examples/m17/src/moving_average.rs:5-81, float with divisor 4800).  Not MovingAvg.  One work() runs the reference's
+// work() calls back to back on the current slices until one makes no progress, or at most max_calls of them
+// (1: exactly one reference call); call_again and the finish rule are those of the last call (b2s_boxavg_exec).
+template <typename T> class MovingAverage {
+    static_assert(std::is_same_v<T, float> || std::is_same_v<T, Complex32>, "MovingAverage: f32 or Complex32 items");
+public:
+    MovingAverage(const Instance &inst, size_t len, std::optional<float> divisor = std::nullopt, size_t max_calls = 0)
+        : input(inst), output(inst), inst_(inst), max_calls_(max_calls) {
+        check(b2s_boxavg_create(inst.get(), std::is_same_v<T, Complex32> ? 1 : 0, len, divisor.has_value(),
+                                divisor.value_or(0.0f), out_ptr(h_)), inst.get());
+    }
+    void reset() { check(b2s_boxavg_reset(h_.get()), inst_.get()); }
+    void work(WorkIo &io) {
+        size_t c = 0, p = 0, calls = 0;
+        int32_t again = 0, done = 0;
+        check(b2s_boxavg_exec(h_.get(), input.slice(), input.len(), output.slice(), output.capacity(), max_calls_, &c,
+                              &p, &calls, &again, &done), inst_.get());
+        input.consume(c);
+        output.produce(p);
+        if (again) io.call_again = true;                                            // :82-84
+        if (input.finished() && done) io.finished = true;                           // :103-105
+    }
+    Reader<T> input;
+    Writer<T> output;
+private:
+    const Instance &inst_; size_t max_calls_; Handle<b2s_boxavg, b2s_boxavg_destroy> h_;
 };
 
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)

@@ -44,7 +44,8 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 
 def want(section):
-    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, scale)."""
+    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg,
+    scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -231,6 +232,70 @@ def stream_section(quick):
                               "VectorSink D2H, driven by edges.Flowgraph from Python"}), flush=True)
 
 
+def boxavg_section(quick):
+    """The WLAN / M17 MovingAverage (csrc/boxavg.cu) on 64 Mi items per exec: f32 len 64, c32 len 48 (the WLAN rx
+    shapes) and f32 len 4800 / 4800 (M17), as fractions of the 3.35 TB/s data-sheet figure computed from algorithmic
+    bytes (input + output once each); the C oracle on one thread beside each; and the WLAN receiver front end with the
+    real MovingAverage blocks as an end-to-end graph rate through edges.Flowgraph."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from boxavg_oracle import BoxAvgRef
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({"kernel": "boxavg_device", "gpu": q[torch.cuda.current_device()] if q else "unknown"}), flush=True)
+    n = (16 if quick else 64) << 20
+    nc = 4 << 20
+    g = torch.Generator(device="cuda").manual_seed(7)
+    for dt, length, div in ((np.float32, 64, None), (np.complex64, 48, None), (np.float32, 4800, 4800.0)):
+        cplx = dt == np.complex64
+        x = (torch.view_as_complex(torch.randn(n, 2, generator=g, device="cuda")) if cplx
+             else torch.randn(n, generator=g, device="cuda"))
+        o = torch.empty_like(x)
+        blk = fb.MovingAverage(dt, length, div)
+        blk.average(x, o)                                        # the pad: later execs are all sums
+
+        def run():
+            blk.average(x, o)
+        sec = timeit(run, iters=20, warm=3)
+        nbytes = 2 * x.element_size() * (n + 1 - length)
+        gbs = nbytes / sec / 1e9
+        hx = x[:nc].cpu().numpy()
+        ref = BoxAvgRef(dt, length, div)
+        ref.pad = 0
+        t0 = time.perf_counter()
+        ref.run(hx, nc)
+        cpu = time.perf_counter() - t0
+        name = f"boxavg_{'c32' if cplx else 'f32'}_len{length}" + ("_div" if div else "")
+        print(json.dumps({"kernel": name, "items": n, "ms": round(sec * 1e3, 4), "Gitems_s": round(n / sec / 1e9, 2),
+                          "alg_GBs": round(gbs, 1), "frac_3350GBs": round(gbs / 3350.0, 4),
+                          "cpu_oracle_1thread_Gitems_s": round(nc / cpu / 1e9, 4)}), flush=True)
+        del x, o, blk
+        torch.cuda.empty_cache()
+    from futuresdr_b200.blocks import Apply, ApplyOp
+    from futuresdr_b200.edges import Flowgraph, VectorSink, VectorSource
+    ns = (4 if quick else 16) << 20
+    x = (np.random.default_rng(0).standard_normal(2 * ns).astype(np.float32).view(np.complex64))
+    best = None
+    for _ in range(3):
+        fg = Flowgraph()
+        src, delay = VectorSource(x), fb.Delay(np.complex64, 16)
+        mag2, mult = Apply(ApplyOp.NormSqr), fb.Combine(fb.CombineOp.ConjMulC32)
+        favg, cavg = fb.MovingAverage(np.float32, 64), fb.MovingAverage(np.complex64, 48)
+        div, snk = fb.Combine(fb.CombineOp.MagDivC32F32), VectorSink(np.float32)
+        for args in ((src, delay), (src, mag2), (src, mult, "in0"), (delay, mult, "in1"), (mag2, favg),
+                     (mult, cavg), (cavg, div, "in0"), (favg, div, "in1"), (div, snk)):
+            fg.connect(*args)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "wlan_rx_front_end_graph_moving_average", "items": ns, "s": round(best, 4),
+                      "Gsamples_s_end_to_end": round(ns / best / 1e9, 4),
+                      "note": "whole graph, end to end: VectorSource H2D + Delay + NormSqr + 2 MovingAverage + "
+                              "2 Combine + VectorSink D2H, driven by edges.Flowgraph from Python"}), flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -414,6 +479,8 @@ def main():
         sigsrc_section(quick)
     if want("stream"):
         stream_section(quick)
+    if want("boxavg"):
+        boxavg_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
