@@ -7,7 +7,7 @@
 // (examples/fm-receiver/src/main.rs:99-104) is the previous input item, so item j reads
 // in[j-1] and item 0 reads the carried sample; after the launch the carry is refreshed from
 // in[m-1] on the same stream.
-#include "common.cuh"
+#include "chunks.cuh"
 
 struct b2s_apply {
     b2s_ctx *ctx = nullptr;
@@ -87,10 +87,8 @@ __global__ void apply_kernel(const void *__restrict__ vin, void *__restrict__ vo
 template <int OP>
 int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
     b2s_ctx *ctx = a->ctx;
-    const int th = 256;
-    const size_t want = ceil_div(n, (size_t)th);
-    const unsigned grid = (unsigned)std::min<size_t>(want, (size_t)ctx->sm_count * 16);
-    apply_kernel<OP><<<grid, th, 0, ctx->stream>>>(in, out, (long long)n, a->param, a->d_carry.get());
+    apply_kernel<OP><<<grid_for(ctx, n, 16), kThreads, 0, ctx->stream>>>(in, out, (long long)n, a->param,
+                                                                         a->d_carry.get());
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }
@@ -137,9 +135,7 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
     // the demodulators read in[j-1] while a neighbour thread writes out[j-1]: the slices must not overlap
     // (the element-wise ops may run in place)
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {
-        const char *i0 = (const char *)d_in, *i1 = i0 + m * sizeof(float2);
-        const char *o0 = (const char *)d_out, *o1 = o0 + m * (a->op == B2S_OP_QUAD_DEMOD ? sizeof(float) : sizeof(float2));
-        if (i0 < o1 && o0 < i1)
+        if (overlap(d_in, m * sizeof(float2), d_out, m * (a->op == B2S_OP_QUAD_DEMOD ? sizeof(float) : sizeof(float2))))
             return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the quadrature demodulator cannot run in place (input and output overlap)");
     }
     DeviceGuard g(a->ctx->device);

@@ -47,15 +47,6 @@ template <int W> struct Geo {
     static constexpr int tile = rows * P;         // floats per tile (1056 for both item widths)
 };
 
-__device__ __forceinline__ void cp_async4(float *smem, const float *gmem) {
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(s), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory");
-}
-
 // n_seg segments; all hold 4000 outputs but the last, which holds m_last.  c0 = len - 1.  ring: lead tiles resident
 // (RING) or in flight (otherwise).  Shared memory: `ring` lead tiles, kStages trailing tiles (not RING), 1 output tile.
 template <int W, bool RING, bool DIV>
@@ -91,12 +82,12 @@ boxavg_kernel(const float *__restrict__ in, float *__restrict__ out, unsigned lo
                     const unsigned m = rr == last_row ? m_last : (unsigned)kMaxIter;
                     const unsigned it = t * kK + w / W;
                     const float *src = in0 + (size_t)rr * kMaxIter * W + (size_t)t * G::KW + w;
-                    if (it < c0 + m) cp_async4(L + rr * G::P + w, src);
-                    if (!RING && it >= c0 && it - c0 < m) cp_async4(Tr + rr * G::P + w, src - (size_t)c0 * W);
+                    if (it < c0 + m) cp_async::ca4(L + rr * G::P + w, src);
+                    if (!RING && it >= c0 && it - c0 < m) cp_async::ca4(Tr + rr * G::P + w, src - (size_t)c0 * W);
                 }
             }
         }
-        cp_async_commit();                     // one group per tile, empty ones included, so wait_group counts tiles
+        cp_async::commit();                    // one group per tile, empty ones included, so wait_group counts tiles
     };
 
 #pragma unroll
@@ -106,7 +97,7 @@ boxavg_kernel(const float *__restrict__ in, float *__restrict__ out, unsigned lo
     float s = W == 1 ? -0.0f : 0.0f;
     for (unsigned t = 0; t < T; t++) {
         issue(t + kStages - 1);
-        cp_async_wait<kStages - 1>();          // tile t has landed (this lane's copies) ...
+        cp_async::wait<kStages - 1>();         // tile t has landed (this lane's copies) ...
         __syncwarp();                          // ... and every lane's
         const float *Lr = lead + (t % ring) * G::tile + r * G::P + c;
         const float *pA, *pB;                  // trailing item of step jj: pA[jj W] for jj < rem, else pB[jj W]
@@ -152,7 +143,7 @@ boxavg_kernel(const float *__restrict__ in, float *__restrict__ out, unsigned lo
         }
         __syncwarp();                          // the output tile and tile t's slots are free again
     }
-    cp_async_wait<0>();
+    cp_async::wait<0>();
 }
 
 template <int W, bool RING, bool DIV>
@@ -167,11 +158,6 @@ int32_t launch(b2s_ctx *ctx, const float *in, float *out, size_t n_seg, unsigned
     kernel<<<(unsigned)grid, 32, smem, ctx->stream>>>(in, out, n_seg, m_last, c0, div, ring);
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
-}
-
-bool overlap(const void *p, size_t pb, const void *q, size_t qb) {
-    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
-    return pb && qb && a < b + qb && b < a + pb;
 }
 
 }  // namespace
@@ -252,7 +238,7 @@ int32_t b2s_boxavg_exec(b2s_boxavg *p, const void *d_in, size_t n_in, void *d_ou
     const size_t isz = p->cplx ? 8 : 4;
     if (pad_items || n_seg) {
         if (!d_out || (n_seg && !d_in)) return b2s_fail(ctx, B2S_EINVAL, "b2s_boxavg_exec: NULL slice");
-        if (((uintptr_t)d_out & 3) || (n_seg && ((uintptr_t)d_in & 3)))
+        if (!word_aligned(d_out) || (n_seg && !word_aligned(d_in)))
             return b2s_fail(ctx, B2S_EINVAL, "b2s_boxavg_exec: a slice is not 4-byte aligned");
     }
     if (n_seg && overlap(d_in, (c + p->len - 1) * isz, d_out, prod * isz))

@@ -166,12 +166,6 @@ constexpr size_t chan_xcap(int log2n, int tpad) {
     return rows > staging ? rows : staging;
 }
 
-__device__ __forceinline__ void chan_cp_async16(void *dst_smem, const void *src, bool valid) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-    const int sz = valid ? 16 : 0;                       // src-size 0: the 16 bytes are zero-filled
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(sz) : "memory");
-}
-
 // Persistent: a CTA walks tiles blockIdx.x, blockIdx.x + gridDim.x, ... and the input tile of the NEXT one is fetched
 // with cp.async into the other half of a double buffer while the current one is filtered, transformed and stored
 // (a load, wait, compute sequence leaves the CTA stalled on its global loads).
@@ -208,9 +202,9 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
         for (int e = tid; e < TOT4; e += 256) {
             const long long it = base + 2ll * e;             // even, and n_items is even: both samples valid or none
             const bool ok = it >= 0 && it + 1 < n_items;
-            chan_cp_async16(reinterpret_cast<float4 *>(X) + e, in + (ok ? it : 0), ok);
+            cp_async::cg16(reinterpret_cast<float4 *>(X) + e, in + (ok ? it : 0), ok);
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async::commit();
     };
 
     int it_n = 0;
@@ -220,9 +214,9 @@ __global__ void __launch_bounds__(256) chan_fused_kernel(const float2 *__restric
         const int nxt = tile + gridDim.x;
         if (nxt < ntiles) {
             fetch(nxt, Xbuf + (size_t)((it_n & 1) ^ 1) * XCAP);
-            asm volatile("cp.async.wait_group 1;" ::: "memory");
+            cp_async::wait<1>();
         } else {
-            asm volatile("cp.async.wait_group 0;" ::: "memory");
+            cp_async::wait<0>();
         }
         __syncthreads();
         const long long o0 = o_first + (long long)tile * OB;

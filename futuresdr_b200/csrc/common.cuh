@@ -65,6 +65,31 @@ __device__ __forceinline__ void mac(float2 &acc, float2 x, float2 t) {
 template <typename S> __device__ __forceinline__ S zero_of();
 template <> __device__ __forceinline__ float zero_of<float>() { return 0.0f; }
 template <> __device__ __forceinline__ float2 zero_of<float2>() { return make_float2(0.f, 0.f); }
+
+// cp.async (LDGSTS): global -> shared copies that hold no registers while in flight.  .ca also caches the line in L1,
+// .cg only in L2.  The forms with `valid` zero-fill the destination when it is false (src-size 0); src must then still
+// be a mapped address.  commit() closes a group of the thread's copies; wait<N>() returns when at most N groups are
+// still in flight (the thread's own copies only: a barrier publishes them to the CTA).
+namespace cp_async {
+__device__ __forceinline__ void ca4(float *dst_smem, const float *src) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst_smem);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(d), "l"(src) : "memory");
+}
+__device__ __forceinline__ void ca4(float *dst_smem, const float *src, bool valid) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst_smem);
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(src), "r"(valid ? 4 : 0) : "memory");
+}
+__device__ __forceinline__ void cg16(void *dst_smem, const void *src) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst_smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cg16(void *dst_smem, const void *src, bool valid) {
+    const unsigned d = (unsigned)__cvta_generic_to_shared(dst_smem);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+}  // namespace cp_async
 #endif
 
 extern thread_local std::string g_b2s_last_error;
@@ -212,6 +237,18 @@ int32_t peer_flag_wait_launch(b2s_ctx *ctx, const unsigned *flag, unsigned value
 static inline size_t sat_sub(size_t a, size_t b) { return a > b ? a - b : 0; }
 static inline size_t ceil_div(size_t a, size_t b) { return (a + b - 1) / b; }
 static inline size_t round_up(size_t a, size_t b) { return ceil_div(a, b) * b; }
+
+// slice checks of the exec calls: byte ranges [p, p + pb) and [q, q + qb) share a byte (empty ranges share none)
+static inline bool overlap(const void *p, size_t pb, const void *q, size_t qb) {
+    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
+    return pb && qb && a < b + qb && b < a + pb;
+}
+// an output may be disjoint from an input, or lie exactly on it with the same item size (in place)
+static inline bool bad_alias(const void *out, size_t ob, size_t oi, const void *in, size_t ib, size_t ii) {
+    if (!overlap(out, ob, in, ib)) return false;
+    return !(out == in && oi == ii);
+}
+static inline bool word_aligned(const void *p) { return ((uintptr_t)p & 3) == 0; }
 
 static inline size_t kind_in_bytes(b2s_kind k) { return k == B2S_F32_F32 ? 4 : 8; }   // F64_F64: 8 as well
 static inline size_t kind_tap_floats(b2s_kind k) { return k == B2S_C32_C32 ? 2 : 1; }

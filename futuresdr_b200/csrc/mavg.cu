@@ -30,12 +30,6 @@ namespace {
 // per block.)
 constexpr int kMaBins = 32, kMaFrames = 64, kMaWarps = 8, kMaStages = 4;
 
-__device__ __forceinline__ void ma_cp_async4(float *dst_smem, const float *src, bool valid) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-    const int sz = valid ? 4 : 0;                        // src-size 0: the 4 bytes are zero-filled
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(d), "l"(src), "r"(sz) : "memory");
-}
-
 __global__ void __launch_bounds__(32 * kMaWarps)
 mavg_kernel(const float *__restrict__ in, float *__restrict__ out, float *avg, int width,
             long long nchunks, int history, int i0, float decay, long long max_out) {
@@ -53,10 +47,10 @@ mavg_kernel(const float *__restrict__ in, float *__restrict__ out, float *avg, i
                 const int f = warp + k * kMaWarps;
                 const long long c = blk * kMaFrames + f;
                 const bool ok = live && c < nchunks;
-                ma_cp_async4(&buf[stage][f][lane], ok ? in + c * width + b : in, ok);
+                cp_async::ca4(&buf[stage][f][lane], ok ? in + c * width + b : in, ok);
             }
         }
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        cp_async::commit();
     };
     float a = live ? avg[b] : 0.0f;
     const float keep = __fsub_rn(1.0f, decay);
@@ -66,7 +60,7 @@ mavg_kernel(const float *__restrict__ in, float *__restrict__ out, float *avg, i
     for (int s = 0; s < kMaStages - 1; s++) issue(s);
     for (long long blk = 0; blk < nblk; blk++) {
         issue(blk + kMaStages - 1);                      // refills the stage warp 0 finished in the previous iteration
-        asm volatile("cp.async.wait_group %0;" ::"n"(kMaStages - 1) : "memory");
+        cp_async::wait<kMaStages - 1>();
         __syncthreads();                                 // block blk has landed for every thread's copies
         if (warp == 0 && live) {
             const int stage = (int)(blk % kMaStages);

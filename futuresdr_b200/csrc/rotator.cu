@@ -15,7 +15,7 @@
 #include <condition_variable>
 #include <thread>
 
-#include "common.cuh"
+#include "chunks.cuh"
 
 namespace {
 constexpr int kRotSub = 8;                      // samples per recorded phase
@@ -200,10 +200,9 @@ int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_
             B2S_CUDA(ctx, cudaMemcpyAsync(drec + first, r->h_ring.get(), (cnt - first) * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
         B2S_CUDA(ctx, cudaEventRecord(r->ev[h], ctx->stream));
         r->span_end[h] = rec0;                                      // records below rec0 are never needed again
-        const int th = 256;
-        const unsigned grid = (unsigned)std::min<size_t>(ceil_div(m, (size_t)th), (size_t)ctx->sm_count * 16);
-        rotator_kernel<<<grid, th, 0, ctx->stream>>>((const float2 *)d_in + done, (float2 *)d_out + done, drec,
-                                                     make_float2(r->incr[0], r->incr[1]), (long long)m, (int)(a0 % kRotSub));
+        rotator_kernel<<<grid_for(ctx, m, 16), kThreads, 0, ctx->stream>>>(
+            (const float2 *)d_in + done, (float2 *)d_out + done, drec, make_float2(r->incr[0], r->incr[1]), (long long)m,
+            (int)(a0 % kRotSub));
         B2S_CHECK_LAUNCH(ctx);
         r->pos = a1; r->half ^= 1; done += m;
     }

@@ -13,14 +13,12 @@
 #include <cmath>
 #include <cstdint>
 
-#include "common.cuh"
+#include "chunks.cuh"
 
 namespace {
 
 constexpr int kTableN = 1024;
 constexpr int kTablePad = kTableN + kTableN / 32;    // one pad word per 32 entries, see tpos()
-constexpr int kThreads = 256;
-constexpr int kBlocksPerSm = 8;
 constexpr uint32_t kAccumMask = 0x3FFFFFu;           // ACCUM_MASK: 32 - 10 fraction bits (fxpt_phase.rs:70)
 
 struct SineTable { float slope[kTableN], offset[kTableN]; };
@@ -105,8 +103,8 @@ __device__ __forceinline__ float sample_float(unsigned long long j, uint32_t pha
     return r != r ? __uint_as_float(nan_bits) : r;
 }
 
-// Writes nf floats at out.  The first `head` floats (0..3) bring the pointer to 16 bytes; then float4 stores over
-// a grid-stride loop; the last (nf - head) % 4 floats are scalar.
+// Writes nf floats at out on the aligned-chunk loop (chunks.cuh), counted in floats; `head` brings out to 16 bytes,
+// so every chunk is one float4 store.
 template <int WAVE, bool CPLX>
 __global__ void __launch_bounds__(kThreads)
 sigsrc_kernel(float *__restrict__ out, unsigned long long nf, unsigned head, uint32_t phase0, uint32_t inc, float amp,
@@ -119,10 +117,8 @@ sigsrc_kernel(float *__restrict__ out, unsigned long long nf, unsigned head, uin
         }
         __syncthreads();
     }
-    const unsigned long long g = (unsigned long long)blockIdx.x * kThreads + threadIdx.x;
-    const unsigned long long nv = (nf - head) >> 2;
     float4 *ov = reinterpret_cast<float4 *>(out + head);
-    for (unsigned long long v = g; v < nv; v += (unsigned long long)gridDim.x * kThreads) {
+    chunk_loop(nf, head, [&](unsigned long long v) {
         const unsigned long long j = head + 4 * v;
         float4 r;
         r.x = sample_float<WAVE, CPLX>(j, phase0, inc, amp, nan_bits, sl, of);
@@ -130,10 +126,7 @@ sigsrc_kernel(float *__restrict__ out, unsigned long long nf, unsigned head, uin
         r.z = sample_float<WAVE, CPLX>(j + 2, phase0, inc, amp, nan_bits, sl, of);
         r.w = sample_float<WAVE, CPLX>(j + 3, phase0, inc, amp, nan_bits, sl, of);
         ov[v] = r;
-    }
-    const unsigned long long tail0 = head + 4 * nv;
-    if (g < head) out[g] = sample_float<WAVE, CPLX>(g, phase0, inc, amp, nan_bits, sl, of);
-    if (g < nf - tail0) out[tail0 + g] = sample_float<WAVE, CPLX>(tail0 + g, phase0, inc, amp, nan_bits, sl, of);
+    }, [&](unsigned long long j) { out[j] = sample_float<WAVE, CPLX>(j, phase0, inc, amp, nan_bits, sl, of); });
 }
 
 template <int WAVE, bool CPLX>
@@ -210,15 +203,12 @@ int32_t b2s_sigsrc_exec(b2s_sigsrc *s, void *d_out, size_t n_out_cap, size_t *pr
     *produced = 0;
     if (n_out_cap == 0) return B2S_OK;
     if (!d_out) return b2s_fail(s->ctx, B2S_EINVAL, "b2s_sigsrc_exec: NULL output");
-    const uintptr_t addr = (uintptr_t)d_out;
-    if (addr & 3) return b2s_fail(s->ctx, B2S_EINVAL, "b2s_sigsrc_exec: output is not 4-byte aligned");
+    if (!word_aligned(d_out)) return b2s_fail(s->ctx, B2S_EINVAL, "b2s_sigsrc_exec: output is not 4-byte aligned");
     DeviceGuard g(s->ctx->device);
     NvtxRange nvtx("b2s_sigsrc_exec");
     const unsigned long long nf = (unsigned long long)n_out_cap * (s->cplx ? 2 : 1);
-    const unsigned head = (unsigned)std::min<unsigned long long>(((16 - (addr & 15)) & 15) / 4, nf);
-    const unsigned long long nv = (nf - head) / 4;
-    const unsigned grid = (unsigned)std::max<unsigned long long>(
-        1, std::min<unsigned long long>(ceil_div(nv, (size_t)kThreads), (unsigned long long)s->ctx->sm_count * kBlocksPerSm));
+    const unsigned head = (unsigned)std::min<unsigned long long>(head_items(d_out, 4), nf);
+    const unsigned grid = grid_for(s->ctx, (nf - head) / 4);
     float *o = (float *)d_out;
     cudaStream_t st = s->ctx->stream;
     const uint32_t ph = s->phase, inc = s->inc;

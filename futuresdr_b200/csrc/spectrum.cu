@@ -53,11 +53,6 @@ struct SpArgs {
     float a, d;
 };
 
-__device__ __forceinline__ void sp_cp_async16(void *dst_smem, const void *src) {
-    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src) : "memory");
-}
-
 // The next frame of a group is fetched with cp.async into a raw staging row while the current one is being
 // transformed: the first FFT pass reads the staging row, and from the barrier that ends it the row is free again, so
 // the fetch of frame c+1 overlaps passes 2.. and the averaging of frame c.  (The first version read the frame with
@@ -81,13 +76,13 @@ __global__ void __launch_bounds__(kSpThreads, (LOG2N <= 12 ? 3 : 1)) spectrum_ke
     for (int k = 0; k < NB; k++) avg[k] = 0.0f;
     auto fetch = [&](long long c) {                          // frame c of this group -> raw (idle rounds re-fetch frame 0)
         const float4 *src = reinterpret_cast<const float4 *>(p.in + (f0 + (c < nf ? c : 0)) * N);
-        for (int i = t; i < N / 2; i += T) sp_cp_async16(reinterpret_cast<float4 *>(raw) + i, src + i);
-        asm volatile("cp.async.commit_group;" ::: "memory");
+        for (int i = t; i < N / 2; i += T) cp_async::cg16(reinterpret_cast<float4 *>(raw) + i, src + i);
+        cp_async::commit();
     };
     fetch(0);
     for (long long c = 0; c < p.C; c++) {                   // every group of the CTA runs C rounds (barriers inside)
         const bool act = c < nf;
-        asm volatile("cp.async.wait_group 0;" ::: "memory");
+        cp_async::wait<0>();
         __syncthreads();                                     // raw holds frame c; everyone is done with sP of frame c-1
         fft_passes<LOG2N, T, Tw::Ahead>([&](int idx) { return raw[idx]; },
                                         [&](int idx, float2 v) { sP[idx] = fmaf(v.x, v.x, v.y * v.y); },   // norm_sqr

@@ -3,9 +3,8 @@
 // (stream_deinterleaver.rs:61-97).  Delay (delay.rs) needs no kernel: pad is b2s_memset, copy b2s_memcpy_d2d.
 //
 // Every kernel is element-wise or a permutation, so each is bound by HBM traffic.  Items are handled as 32-bit
-// words (f32 = 1 word, Complex32 / f64 = 2 words), so any 4-byte-aligned slice works.  Element-wise kernels process
-// chunks of 4 items: a scalar head (0..3 items) brings the first output to 16 bytes, every stream whose chunks are
-// then 16-byte aligned is moved with float4 accesses, the others word by word; a scalar tail finishes the call.
+// words (f32 = 1 word, Complex32 / f64 = 2 words), so any 4-byte-aligned slice works.  Element-wise kernels run on
+// the aligned-chunk loop of chunks.cuh; Combine and Split take the head from output 0, the duplicator from its input.
 //
 // Bit-exactness: every closure is written with __fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn in the order of the
 // Rust expression (Rust does not contract to FMA; the library is also built with -ffp-contract=off).  norm() is
@@ -15,41 +14,12 @@
 #include <algorithm>
 #include <cstdint>
 
-#include "common.cuh"
+#include "chunks.cuh"
 
 namespace {
 
-constexpr int kThreads = 256;
-constexpr int kBlocksPerSm = 8;
 constexpr int kMaxOuts = 256;                // output pointers passed in the kernel parameter block (2 KiB)
 constexpr size_t kTileBytes = 16384;         // deinterleave: target shared-memory tile
-
-// ---- 4-item chunks of W-word items ---------------------------------------------------------------------------
-template <int W> __device__ __forceinline__ void ld_chunk(const float *__restrict__ p, bool wide, float (&r)[4 * W]) {
-    if (wide) {
-#pragma unroll
-        for (int j = 0; j < W; j++) {
-            const float4 q = __ldg(reinterpret_cast<const float4 *>(p) + j);
-            r[4 * j] = q.x; r[4 * j + 1] = q.y; r[4 * j + 2] = q.z; r[4 * j + 3] = q.w;
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < 4 * W; j++) r[j] = __ldg(p + j);
-    }
-}
-
-template <int W> __device__ __forceinline__ void st_chunk(float *__restrict__ p, bool wide, const float (&r)[4 * W]) {
-    if (wide) {
-#pragma unroll
-        for (int j = 0; j < W; j++)
-            reinterpret_cast<float4 *>(p)[j] = make_float4(r[4 * j], r[4 * j + 1], r[4 * j + 2], r[4 * j + 3]);
-    } else {
-#pragma unroll
-        for (int j = 0; j < 4 * W; j++) p[j] = r[j];
-    }
-}
-
-__device__ __forceinline__ bool aligned16(const void *p) { return ((uintptr_t)p & 15) == 0; }
 
 // ---- Combine closures: words per item of in0, in1, out and the closure itself ---------------------------------
 template <int OP> struct CombineOp;
@@ -99,30 +69,23 @@ combine_kernel(const float *__restrict__ a, const float *__restrict__ b, float *
                unsigned head) {
     using Op = CombineOp<OP>;
     constexpr int WA = Op::WA, WB = Op::WB, WO = Op::WO;
-    const unsigned long long g = (unsigned long long)blockIdx.x * kThreads + threadIdx.x;
-    const unsigned long long nv = (m - head) >> 2;
     const float *a0 = a + (size_t)head * WA, *b0 = b + (size_t)head * WB;
     float *o0 = o + (size_t)head * WO;
     const bool wa = aligned16(a0), wb = aligned16(b0), wo = aligned16(o0);
-    for (unsigned long long v = g; v < nv; v += (unsigned long long)gridDim.x * kThreads) {
+    chunk_loop(m, head, [&](unsigned long long v) {
         float ra[4 * WA], rb[4 * WB], ro[4 * WO];
         ld_chunk<WA>(a0 + 4 * WA * v, wa, ra);
         ld_chunk<WB>(b0 + 4 * WB * v, wb, rb);
 #pragma unroll
         for (int k = 0; k < 4; k++) Op::f(ra + k * WA, rb + k * WB, ro + k * WO);
         st_chunk<WO>(o0 + 4 * WO * v, wo, ro);
-    }
-    const unsigned long long tail0 = head + 4 * nv;
-    unsigned long long i = ~0ull;
-    if (g < head) i = g;
-    else if (g - head < m - tail0) i = tail0 + (g - head);
-    if (i != ~0ull) {
+    }, [&](unsigned long long i) {
         float ra[WA], rb[WB], ro[WO];
         for (int j = 0; j < WA; j++) ra[j] = a[i * WA + j];
         for (int j = 0; j < WB; j++) rb[j] = b[i * WB + j];
         Op::f(ra, rb, ro);
         for (int j = 0; j < WO; j++) o[i * WO + j] = ro[j];
-    }
+    });
 }
 
 // ---- Split closures -------------------------------------------------------------------------------------------
@@ -142,29 +105,22 @@ split_kernel(const float *__restrict__ in, float *__restrict__ o0, float *__rest
              unsigned head) {
     using Op = SplitOp<OP>;
     constexpr int WI = Op::WI;
-    const unsigned long long g = (unsigned long long)blockIdx.x * kThreads + threadIdx.x;
-    const unsigned long long nv = (m - head) >> 2;
     const float *i0 = in + (size_t)head * WI;
     float *p0 = o0 + head, *p1 = o1 + head;
     const bool wi = aligned16(i0), w0 = aligned16(p0), w1 = aligned16(p1);
-    for (unsigned long long v = g; v < nv; v += (unsigned long long)gridDim.x * kThreads) {
+    chunk_loop(m, head, [&](unsigned long long v) {
         float r[4 * WI], y0[4], y1[4];
         ld_chunk<WI>(i0 + 4 * WI * v, wi, r);
 #pragma unroll
         for (int k = 0; k < 4; k++) Op::f(r + k * WI, y0[k], y1[k]);
         st_chunk<1>(p0 + 4 * v, w0, y0);
         st_chunk<1>(p1 + 4 * v, w1, y1);
-    }
-    const unsigned long long tail0 = head + 4 * nv;
-    unsigned long long i = ~0ull;
-    if (g < head) i = g;
-    else if (g - head < m - tail0) i = tail0 + (g - head);
-    if (i != ~0ull) {
+    }, [&](unsigned long long i) {
         float y0, y1;
         Op::f(in + i * WI, y0, y1);
         o0[i] = y0;
         o1[i] = y1;
-    }
+    });
 }
 
 // ---- fan-out: N output pointers in the parameter block --------------------------------------------------------
@@ -174,26 +130,19 @@ struct OutPtrs { float *p[kMaxOuts]; };
 // the input once and stores it to all N outputs.
 __global__ void __launch_bounds__(kThreads)
 duplicate_kernel(const float *__restrict__ in, const OutPtrs outs, int n_outs, unsigned long long m, unsigned head) {
-    const unsigned long long g = (unsigned long long)blockIdx.x * kThreads + threadIdx.x;
-    const unsigned long long nv = (m - head) >> 2;
     const float *i0 = in + head;
     const bool wi = aligned16(i0);
-    for (unsigned long long v = g; v < nv; v += (unsigned long long)gridDim.x * kThreads) {
+    chunk_loop(m, head, [&](unsigned long long v) {
         float r[4];
         ld_chunk<1>(i0 + 4 * v, wi, r);
         for (int k = 0; k < n_outs; k++) {
             float *ok = outs.p[k] + head;
             st_chunk<1>(ok + 4 * v, aligned16(ok), r);
         }
-    }
-    const unsigned long long tail0 = head + 4 * nv;
-    unsigned long long i = ~0ull;
-    if (g < head) i = g;
-    else if (g - head < m - tail0) i = tail0 + (g - head);
-    if (i != ~0ull) {
+    }, [&](unsigned long long i) {
         const float r = in[i];
         for (int k = 0; k < n_outs; k++) outs.p[k][i] = r;
-    }
+    });
 }
 
 // StreamDeinterleaver: one CTA per tile of G groups of N items.  The tile is read contiguously (float4 when the input
@@ -230,32 +179,7 @@ deinterleave_kernel(const float *__restrict__ in, const OutPtrs outs, int n, int
     }
 }
 
-// ---- host helpers -----------------------------------------------------------------------------------------------
-// first item count (0..3) that brings `addr` to 16 bytes, 0 if no count does
-unsigned head_items(const void *addr, size_t item_bytes) {
-    for (unsigned h = 0; h < 4; h++)
-        if ((((uintptr_t)addr + h * item_bytes) & 15) == 0) return h;
-    return 0;
-}
-
-unsigned grid_for(b2s_ctx *ctx, unsigned long long chunks) {
-    return (unsigned)std::max<unsigned long long>(
-        1, std::min<unsigned long long>(ceil_div(chunks, (size_t)kThreads), (unsigned long long)ctx->sm_count * kBlocksPerSm));
-}
-
-bool overlap(const void *p, size_t pb, const void *q, size_t qb) {
-    const uintptr_t a = (uintptr_t)p, b = (uintptr_t)q;
-    return pb && qb && a < b + qb && b < a + pb;
-}
-
-// an output may be disjoint from an input, or lie exactly on it with the same item size (in place)
-bool bad_alias(const void *out, size_t ob, size_t oi, const void *in, size_t ib, size_t ii) {
-    if (!overlap(out, ob, in, ib)) return false;
-    return !(out == in && oi == ii);
-}
-
-bool word_aligned(const void *p) { return ((uintptr_t)p & 3) == 0; }
-
+// ---- host side ------------------------------------------------------------------------------------------------
 struct CombineTypes { size_t a, b, o; };
 CombineTypes combine_types(b2s_combine_op op) {
     switch (op) {

@@ -167,14 +167,19 @@ def test_channelizer_unaligned_input_leaves_the_fused_path(ctx, monkeypatch):
     x = px.int_samples(rng, N * T + 200 * N, True, lim=px.LIM)
     calls = px.chan_run(N, taps, 1.0, x, [(N * T, 1 << 40)])
     xd = _dev(x)
-    seen = {}
-    for ioff in (0, 1):
-        ch = _Chan(ctx, N, taps, 1.0, False, monkeypatch)
-        try:
-            _check_chan_call(0, calls[0], *ch.call(xd, *calls[0][:3], ioff=ioff))
-            seen[ioff] = _kernels(lambda: _check_chan_call(1, calls[1], *ch.call(xd, *calls[1][:3], ioff=ioff)))
-        finally:
-            ch.close()
+    seen = {0: set(), 1: set()}
+    for ioff, expect in ((0, "chan_fused_kernel"), (1, "chan_bank_kernel")):
+        # A profiler session now and then lacks the records of some kernels that ran, so the call is repeated on a
+        # fresh plan (up to three sessions) until the expected kernel shows; every session counts for the asserts.
+        for _ in range(3):
+            ch = _Chan(ctx, N, taps, 1.0, False, monkeypatch)
+            try:
+                _check_chan_call(0, calls[0], *ch.call(xd, *calls[0][:3], ioff=ioff))
+                seen[ioff] |= _kernels(lambda: _check_chan_call(1, calls[1], *ch.call(xd, *calls[1][:3], ioff=ioff)))
+            finally:
+                ch.close()
+            if any(expect in n for n in seen[ioff]):
+                break
     assert any("chan_fused_kernel" in n for n in seen[0])
     assert not any("chan_fused_kernel" in n for n in seen[1])
     assert any("chan_bank_kernel" in n for n in seen[1])

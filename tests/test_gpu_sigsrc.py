@@ -56,7 +56,8 @@ def test_one_big_call_bit_equal(wave, freq, dtype):
 @pytest.mark.parametrize("wave", list(WAVES))
 def test_ragged_calls_equal_one_call(wave, dtype):
     """Calls of 0, 1, 3, 4095 and 2^20 + 7 items into slices that start one item past an aligned address produce the
-    single call's items bit for bit; the NCO phase after every call is the oracle's."""
+    single call's items bit for bit; the NCO phase after every call is the oracle's.  The gap items around the slices
+    keep a guard pattern, so a head or tail item written one slot early or late is caught."""
     sizes = [0, 1, 3, 4095, (1 << 20) + 7, 5, 0, 2]
     total = sum(sizes)
     tdt = torch.complex64 if dtype == np.complex64 else torch.float32
@@ -65,17 +66,21 @@ def test_ragged_calls_equal_one_call(wave, dtype):
     one.generate(whole)
     src = make(WAVES[wave], 1000.0, 0.5, -1.0, dtype)
     ref = orc.Source(WAVES[wave], 1000.0, FS, 0.5, -1.0, dtype)
-    buf = torch.empty(total + len(sizes) + 1, dtype=tdt, device="cuda")
-    pos, pieces = 1, []
+    guard = np.uint32(0xA5A5A5A5)
+    words = (total + len(sizes) + 1) * (2 if dtype == np.complex64 else 1)
+    buf = torch.from_numpy(np.full(words, guard, np.uint32).view(dtype)).cuda()
+    pos, pieces, gaps = 1, [], [0]
     for n in sizes:
         assert src.generate(buf[pos:pos + n]) == n
         pieces.append(buf[pos:pos + n])
         ref.work(n)
         ph, _ = src.phase()
         assert ph.value == ref.phase.value, n
+        gaps.append(pos + n)
         pos += n + 1                                      # leave a gap: the next slice starts at another alignment
     got = torch.cat(pieces)
     assert np.array_equal(u32(got), u32(whole))
+    assert np.all(u32(buf[gaps]) == guard)
     want = orc.Source(WAVES[wave], 1000.0, FS, 0.5, -1.0, dtype).work(total)
     assert np.array_equal(u32(whole), want.view(np.uint32))
 

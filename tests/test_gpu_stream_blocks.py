@@ -72,19 +72,31 @@ _TYPES = {fb.CombineOp.AddF32: ("f", "f", np.float32), fb.CombineOp.SubF32: ("f"
 
 
 class _Raw:
-    """A device copy of ``host`` that starts ``off_bytes`` (a multiple of 4) past a 256-byte boundary."""
+    """A device copy of ``host`` that starts ``off_bytes`` (a multiple of 4) past a 64-byte boundary, with 64 bytes of
+    a guard pattern on either side."""
+
+    GUARD = 0xA5
 
     def __init__(self, host: np.ndarray, off_bytes: int):
-        raw = np.ascontiguousarray(host).view(np.uint8)
-        self.t = torch.zeros(raw.size + 64, dtype=torch.uint8, device="cuda")
-        self.off = off_bytes
-        if raw.size:
-            self.t[off_bytes:off_bytes + raw.size].copy_(torch.from_numpy(raw.copy()))
-        self.ptr = C.c_void_p(self.t.data_ptr() + off_bytes)
+        raw = np.ascontiguousarray(host).view(np.uint8).ravel()
+        self.off = 64 + off_bytes
+        self.init = np.full(raw.size + 128, self.GUARD, np.uint8)
+        self.init[self.off:self.off + raw.size] = raw
+        self.t = torch.from_numpy(self.init).cuda()
+        self.ptr = C.c_void_p(self.t.data_ptr() + self.off)
 
     def get(self, dtype, n):
         b = np.dtype(dtype).itemsize * n
         return self.t[self.off:self.off + b].cpu().numpy().view(dtype)
+
+    def assert_written_only(self, dtype, n):
+        """Every byte outside the first ``n`` items still holds what the constructor put there: the rest of the slice
+        and the guards on both sides.  A head or tail item written one slot early or late lands on one of them."""
+        b = np.dtype(dtype).itemsize * n
+        outside = np.ones(self.init.size, bool)
+        outside[self.off:self.off + b] = False
+        bad = np.flatnonzero((self.t.cpu().numpy() != self.init) & outside) - self.off
+        assert bad.size == 0, f"{bad.size} bytes outside the {n} items changed, first at slice byte offsets {bad[:8]}"
 
 
 def _ctx():
@@ -92,11 +104,11 @@ def _ctx():
 
 
 @pytest.mark.parametrize("op", list(fb.CombineOp), ids=[o.name for o in fb.CombineOp])
-@pytest.mark.parametrize("n", [0, 1, 2, 5, 67, 4099, (1 << 20) + 3])
+@pytest.mark.parametrize("n", list(range(10)) + [67, 4099, (1 << 20) + 3])
 def test_combine_bit_exact(op, n):
     rng = np.random.default_rng(int(op) * 1000 + n % 997)
     ta, tb, to = _TYPES[op]
-    for offs in ([(0, 0, 0), (4, 8, 12), (12, 0, 4), (8, 4, 0)] if n < 5000 else [(0, 0, 0), (4, 12, 8)]):
+    for offs in ([(0, 0, 0), (4, 8, 12), (12, 0, 4), (8, 4, 0), (4, 12, 8)] if n < 5000 else [(0, 0, 0), (4, 12, 8)]):
         a = _c32(n, rng) if ta == "c" else _f32(n, rng)
         b = _c32(n + 3, rng) if tb == "c" else _f32(n + 3, rng)
         da, db = _Raw(a, offs[0]), _Raw(b, offs[1])
@@ -108,6 +120,7 @@ def test_combine_bit_exact(op, n):
         assert (c.value, p.value) == (n, n)
         assert lib.b2s_ctx_bytes_held(_ctx()) == before
         _same(do.get(to, n), _restate(op, a, b[:n]))
+        do.assert_written_only(to, n)
 
 
 def test_combine_in_place_and_overlap():
@@ -131,11 +144,11 @@ def test_combine_in_place_and_overlap():
 
 
 @pytest.mark.parametrize("op", list(fb.SplitOp), ids=[o.name for o in fb.SplitOp])
-@pytest.mark.parametrize("n", [0, 1, 3, 7, 4101, (1 << 20) + 1])
+@pytest.mark.parametrize("n", list(range(10)) + [4101, (1 << 20) + 1])
 def test_split_bit_exact(op, n):
     rng = np.random.default_rng(n)
     x = _c32(n, rng) if op == fb.SplitOp.ReIm else _f32(n, rng)
-    for offs in [(0, 0, 0), (4, 8, 12), (8, 12, 4)]:
+    for offs in [(0, 0, 0), (4, 8, 12), (8, 12, 4), (12, 4, 0)]:
         di, d0, d1 = _Raw(x, offs[0]), _Raw(np.zeros(n, np.float32), offs[1]), _Raw(np.zeros(n, np.float32), offs[2])
         c, p = C.c_size_t(0), C.c_size_t(0)
         assert lib.b2s_split_exec(_ctx(), int(op), di.ptr, n, d0.ptr, d1.ptr, n + 5, C.byref(c), C.byref(p)) == 0
@@ -144,6 +157,8 @@ def test_split_bit_exact(op, n):
         w0, w1 = (x.real, x.imag) if op == fb.SplitOp.ReIm else (x, x)
         _same(d0.get(np.float32, n), w0)
         _same(d1.get(np.float32, n), w1)
+        d0.assert_written_only(np.float32, n)
+        d1.assert_written_only(np.float32, n)
 
 
 _DT = {"f32": np.float32, "c32": np.complex64, "f64": np.float64}
@@ -162,7 +177,8 @@ def test_fanout_bit_exact(deinterleave, dtn, N):
     dt = _DT[dtn]
     isz = np.dtype(dt).itemsize
     rng = np.random.default_rng(N * 7 + deinterleave)
-    for groups, cap, offs in [(0, 5, 0), (1, 1, 4), (37, 40, 12), (1029, 1000, 8), ((1 << 16) + 5, 1 << 17, 4)]:
+    short = [(g, g, off) for g in range(10) for off in (0, 4, 8, 12)]   # lengths 0..9, the input at every offset
+    for groups, cap, offs in [(0, 5, 0), (1, 1, 4), (37, 40, 12), (1029, 1000, 8), ((1 << 16) + 5, 1 << 17, 4), *short]:
         if N >= 64:                                             # keep 256 separate outputs small
             groups, cap = min(groups, 4099), min(cap, 4200)
         n_in = groups * N + (N - 1 if deinterleave else 0) if deinterleave else groups
@@ -180,6 +196,7 @@ def test_fanout_bit_exact(deinterleave, dtn, N):
         for k, o in enumerate(outs):
             want = x[k:m * N:N] if deinterleave else x[:m]
             _same(o.get(dt, m), want)
+            o.assert_written_only(dt, m)
 
 
 def test_fanout_limits():
