@@ -21,6 +21,7 @@ from .filters import (  # noqa: F401
 from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
     Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator, MovingAverage,
+    AdsbDemod,
 )
-from . import firdes, windows  # noqa: F401
+from . import adsb, firdes, windows  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

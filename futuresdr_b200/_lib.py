@@ -145,6 +145,12 @@ SIGNATURES = {
     "b2s_boxavg_destroy": (None, [_vp]),
     "b2s_boxavg_reset": (_i32, [_vp]),
     "b2s_boxavg_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _sz, _szp, _szp, _szp, _i32p, _i32p]),
+    "b2s_adsb_create": (_i32, [_vp, _f32, _i32, _vpp]),
+    "b2s_adsb_destroy": (None, [_vp]),
+    "b2s_adsb_reset": (_i32, [_vp]),
+    "b2s_adsb_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _i32, _szp, _i32p]),
+    "b2s_adsb_drain_packets": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_adsb_drain_detections": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_window_hamming": (_sz, [_sz, _i32, C.POINTER(C.c_double), _sz]),
     "b2s_firdes_hilbert": (_sz, [C.POINTER(C.c_double), _sz, _f32p, _sz]),
 }

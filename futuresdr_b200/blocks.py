@@ -12,6 +12,8 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``Delay``                     src/blocks/delay.rs:31-169
   * ``MovingAverage``             examples/wlan/src/moving_average.rs:27-107, examples/m17/src/moving_average.rs:5-81
   * ``StreamDuplicator`` / ``StreamDeinterleaver``   src/blocks/stream_duplicator.rs, stream_deinterleaver.rs
+  * ``AdsbDemod``                 examples/adsb/src/{preamble_detector,demodulator,decoder}.rs (PreambleDetector,
+                                  Demodulator and Decoder::check_crc fused; helpers in futuresdr_b200.adsb)
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
 
@@ -915,6 +917,89 @@ class MovingAverage(Block, Handle):
         if call_again:                                                          # :82-84
             io.call_again = True
         if self.input.finished() and done:                                      # :103-105
+            io.finished = True
+
+
+ADSB_PACKET = np.dtype([("preamble_index", np.uint64), ("preamble_correlation", np.float32),
+                        ("crc_passed", np.int32), ("bytes", np.uint8, 14)], align=True)   # b2s_adsb_packet
+ADSB_DETECTION = np.dtype([("index", np.uint64), ("value", np.float32)], align=True)      # b2s_adsb_detection
+
+
+class AdsbDemod(Block, Handle):
+    """The ADS-B receiver's PreambleDetector -> Demodulator -> Decoder::check_crc (examples/adsb/src/
+    preamble_detector.rs:65-146, demodulator.rs:49-113, decoder.rs:57-73) as one device block.  Stream inputs
+    ``in_samples`` (|x|^2), ``in_nf`` (noise floor) and ``in_preamble_cor`` (preamble correlation), all f32; no stream
+    output.  The detector's tags stay inside the block: ``detections()`` returns them (index, correlation ratio) and
+    ``packets()`` the demodulated 112-bit frames -- only those that pass the CRC unless ``forward_failed_crc``.  Both
+    are cumulative numpy structured arrays, and reading them synchronises.
+
+    Finish rule: the reference finishes as soon as any input is finished, which depends on its scheduler.  Here the
+    block finishes once some input is finished and the scan has reached the limit computed from that input's final
+    length (the smallest final length, if several are finished); that is the reference's result whenever the other
+    inputs hold at least as much data, as they do in the receiver's graph."""
+    _destroy = lib.b2s_adsb_destroy
+    in_dtype = None
+    out_dtype = None
+
+    def __init__(self, threshold: float = 10.0, forward_failed_crc: bool = False, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.threshold = float(np.float32(threshold))
+        self.forward_failed_crc = bool(forward_failed_crc)
+        self._h = C.c_void_p()
+        check(lib.b2s_adsb_create(self.ctx.handle, self.threshold, int(self.forward_failed_crc), C.byref(self._h)),
+              self.ctx.handle)
+        dev = _ctx_device(self.ctx)
+        self.in_samples, self.in_nf, self.in_preamble_cor = (Reader(_F32, dev) for _ in range(3))
+        self._pk, self._det = [], []
+
+    def stream_inputs(self):
+        return ["in_samples", "in_nf", "in_preamble_cor"]
+
+    def port_dtype(self, port):
+        return _F32
+
+    def exec(self, s: torch.Tensor, nf: torch.Tensor, corr: torch.Tensor, finished: bool = False) -> tuple[int, bool]:
+        """One exec over device slices (asynchronous) -> (consumed from each input, done)."""
+        c, dn = C.c_size_t(0), C.c_int32(0)
+        check(lib.b2s_adsb_exec(self._h, _ptr(s), s.numel(), _ptr(nf), nf.numel(), _ptr(corr), corr.numel(),
+                                int(finished), C.byref(c), C.byref(dn)), self.ctx.handle)
+        return c.value, bool(dn.value)
+
+    def reset(self):
+        check(lib.b2s_adsb_reset(self._h), self.ctx.handle)
+        self._pk, self._det = [], []
+
+    def _drain(self, fn, dtype, acc):
+        while True:
+            buf = np.zeros(1 << 16, dtype)
+            n = C.c_size_t(0)
+            check(fn(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)), self.ctx.handle)
+            acc.append(buf[:n.value])
+            if n.value < buf.size:
+                return np.concatenate(acc)
+
+    def packets(self) -> np.ndarray:
+        """Every packet so far (ADSB_PACKET records, in index order)."""
+        out = self._drain(lib.b2s_adsb_drain_packets, ADSB_PACKET, self._pk)
+        self._pk = [out]
+        return out
+
+    def detections(self) -> np.ndarray:
+        """Every detector tag so far (ADSB_DETECTION records, in index order; equal indices can repeat)."""
+        out = self._drain(lib.b2s_adsb_drain_detections, ADSB_DETECTION, self._det)
+        self._det = [out]
+        return out
+
+    def work(self, io: WorkIo):
+        ports = (self.in_samples, self.in_nf, self.in_preamble_cor)
+        sl = [p.slice() for p in ports]
+        L = min(t.numel() for t in sl)
+        fin = [t.numel() for p, t in zip(ports, sl) if p.finished()]
+        final = bool(fin) and L == min(fin)
+        c, done = self.exec(*(t[:L] for t in sl), finished=final)
+        for p in ports:
+            p.consume(c)
+        if done:
             io.finished = True
 
 

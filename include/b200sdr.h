@@ -463,6 +463,42 @@ int32_t b2s_boxavg_exec(b2s_boxavg *p, const void *d_in, size_t n_in, void *d_ou
                         size_t max_calls, size_t *consumed, size_t *produced, size_t *calls, int32_t *call_again,
                         int32_t *done);
 
+/* ---- the ADS-B receiver's PreambleDetector, Demodulator and Decoder::check_crc (≙ examples/adsb/src/
+ * preamble_detector.rs:65-146, demodulator.rs:49-113, decoder.rs:57-73) as one block over three aligned f32 streams:
+ * the samples |x|^2, the noise floor nf and the preamble correlation corr.  The detector's tags are not stream tags:
+ * they are the detection list (index, correlation ratio), and each detection whose 480-sample window is complete is
+ * demodulated into 112 PPM bits, CRC-checked and appended to the packet list (bytes MSB first).
+ *   create: threshold must be finite and >= 0 (B2S_EINVAL otherwise); forward_failed_crc != 0 makes
+ *           drain_packets return the frames that fail the CRC too (Decoder::new(true)).
+ *   exec:   L = min(n_samples, n_nf, n_corr) (at most 2^30 per exec).  Scans the positions below L - 64 from where the
+ *           last exec left off and consumes L - 544 (saturating) of every input: every detection below that already
+ *           has its window.  With finished != 0 it is the last exec: the pending detections g with g + 480 < D (D =
+ *           where the scan ended) are demodulated, the rest dropped, L is consumed and *done is set; later execs do
+ *           nothing.  Stream-ordered, no synchronisation, except when the exec's worst case (one detection per 31
+ *           positions) does not fit a list's capacity: the list then doubles, which synchronises.  The host bounds the
+ *           lists by their true lengths once a copy of the counts behind an earlier exec has landed, so an undrained
+ *           block grows its lists with what it detects, not with the positions it scans.  Slices need 4-byte alignment.
+ *   drain_*: synchronise, copy up to cap entries in stream order to `host` (*n of them), and remove them.
+ *   reset:  back to the stream's start, lists emptied. */
+typedef struct {
+    uint64_t preamble_index;       /* stream index of the preamble's start */
+    float    preamble_correlation; /* the largest corr / nf of the trigger's window */
+    int32_t  crc_passed;
+    uint8_t  bytes[14];            /* the 112 bits, MSB first */
+} b2s_adsb_packet;
+typedef struct {
+    uint64_t index;
+    float    value;
+} b2s_adsb_detection;
+typedef struct b2s_adsb b2s_adsb;
+int32_t b2s_adsb_create(b2s_ctx *ctx, float threshold, int32_t forward_failed_crc, b2s_adsb **out);
+void    b2s_adsb_destroy(b2s_adsb *p);
+int32_t b2s_adsb_reset(b2s_adsb *p);
+int32_t b2s_adsb_exec(b2s_adsb *p, const float *d_samples, size_t n_samples, const float *d_nf, size_t n_nf,
+                      const float *d_corr, size_t n_corr, int32_t finished, size_t *consumed, int32_t *done);
+int32_t b2s_adsb_drain_packets(b2s_adsb *p, b2s_adsb_packet *host, size_t cap, size_t *n);
+int32_t b2s_adsb_drain_detections(b2s_adsb *p, b2s_adsb_detection *host, size_t cap, size_t *n);
+
 /* ---- tap design, host side, f64 then cast (≙ futuredsp::firdes::kaiser, firdes/basic.rs:310-459)
  * Return the tap count; write taps only if cap is large enough (call with taps=NULL to size). */
 size_t b2s_firdes_kaiser_lowpass(double cutoff, double transition_bw, double max_ripple,

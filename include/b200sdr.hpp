@@ -683,6 +683,57 @@ private:
     const Instance &inst_; size_t max_calls_; Handle<b2s_boxavg, b2s_boxavg_destroy> h_;
 };
 
+// ≙ the ADS-B receiver's PreambleDetector -> Demodulator -> Decoder::check_crc (examples/adsb/src/preamble_detector.rs
+// :65-146, demodulator.rs:49-113, decoder.rs:57-73) as one block (b2s_adsb_*).  Three f32 stream inputs, no stream
+// output; the detector's tags and the demodulated frames are drained from the block.  work() runs one exec and
+// finishes once an input is finished and the scan has reached the limit set by the smallest finished input.
+class AdsbDemod {
+public:
+    AdsbDemod(const Instance &inst, float threshold = 10.0f, bool forward_failed_crc = false)
+        : in_samples(inst), in_nf(inst), in_preamble_cor(inst), inst_(inst) {
+        check(b2s_adsb_create(inst.get(), threshold, forward_failed_crc ? 1 : 0, out_ptr(h_)), inst.get());
+    }
+    void reset() { check(b2s_adsb_reset(h_.get()), inst_.get()); }
+    // one exec over device slices (asynchronous): (consumed from each input, done)
+    std::pair<size_t, bool> exec(const float *s, size_t n_s, const float *nf, size_t n_nf, const float *corr,
+                                 size_t n_corr, bool finished) {
+        size_t c = 0;
+        int32_t done = 0;
+        check(b2s_adsb_exec(h_.get(), s, n_s, nf, n_nf, corr, n_corr, finished ? 1 : 0, &c, &done), inst_.get());
+        return {c, done != 0};
+    }
+    void work(WorkIo &io) {
+        const size_t n = std::min({in_samples.len(), in_nf.len(), in_preamble_cor.len()});
+        // every mocker::Reader is finished: the final exec runs on the common length
+        auto [c, done] = exec(in_samples.slice(), n, in_nf.slice(), n, in_preamble_cor.slice(), n, true);
+        in_samples.consume(c);
+        in_nf.consume(c);
+        in_preamble_cor.consume(c);
+        if (done) io.finished = true;
+    }
+    // every packet / detection since the last drain, in stream order (synchronises)
+    std::vector<b2s_adsb_packet> drain_packets() {
+        return drain<b2s_adsb_packet>(b2s_adsb_drain_packets);
+    }
+    std::vector<b2s_adsb_detection> drain_detections() {
+        return drain<b2s_adsb_detection>(b2s_adsb_drain_detections);
+    }
+    Reader<float> in_samples, in_nf, in_preamble_cor;
+private:
+    template <typename E, typename F> std::vector<E> drain(F fn) {
+        std::vector<E> out;
+        for (;;) {
+            const size_t k = out.size();
+            out.resize(k + 4096);
+            size_t n = 0;
+            check(fn(h_.get(), out.data() + k, 4096, &n), inst_.get());
+            out.resize(k + n);
+            if (n < 4096) return out;
+        }
+    }
+    const Instance &inst_; Handle<b2s_adsb, b2s_adsb_destroy> h_;
+};
+
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
 template <typename T, int32_t Deinterleave> class FanOut {
     static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");

@@ -44,7 +44,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 
 def want(section):
-    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg,
+    """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
     scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
@@ -296,6 +296,56 @@ def boxavg_section(quick):
                               "2 Combine + VectorSink D2H, driven by edges.Flowgraph from Python"}), flush=True)
 
 
+def adsb_section(quick):
+    """The ADS-B detector / demodulator (csrc/adsb.cu) on 64 Mi positions per exec, with sparse triggers and with a
+    trigger at every position, as fractions of the 3.35 TB/s data-sheet figure from 12 B of algorithmic bytes per
+    position (three f32 reads); and the receive front end (listen_adsb.rs:85-120) end to end through edges.Flowgraph."""
+    import subprocess
+    from futuresdr_b200 import adsb
+    from futuresdr_b200.edges import Flowgraph, VectorSource
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    print(json.dumps({"kernel": "adsb_device", "gpu": q[torch.cuda.current_device()] if q else "unknown"}), flush=True)
+    n = (16 if quick else 64) << 20
+    g = torch.Generator(device="cuda").manual_seed(11)
+    s = torch.rand(n, generator=g, device="cuda")
+    nf = torch.rand(n, generator=g, device="cuda") + 0.25
+    for name, density in (("sparse", 1e-4), ("every_position", 1.0)):
+        hit = torch.rand(n, generator=g, device="cuda") < density
+        corr = torch.where(hit, nf * 20.0, nf * 5.0)
+        blk = fb.AdsbDemod(10.0)
+
+        def run():
+            blk.reset()                                          # lists restart: no growth inside the timing
+            blk.exec(s, nf, corr)
+        sec = timeit(run, iters=20, warm=3)
+        gbs = 12 * n / sec / 1e9
+        n_det = blk.detections().size
+        print(json.dumps({"kernel": f"adsb_{name}", "positions": n, "detections": int(n_det),
+                          "ms": round(sec * 1e3, 4), "alg_GBs": round(gbs, 1), "frac_3350GBs": round(gbs / 3350.0, 4)}),
+              flush=True)
+        del corr, blk
+    del s, nf
+    torch.cuda.empty_cache()
+    ns = (4 if quick else 16) << 20
+    x = (np.random.default_rng(0).standard_normal(2 * ns).astype(np.float32).view(np.complex64))
+    best = None
+    for _ in range(3):
+        fg = Flowgraph()
+        src = VectorSource(x)
+        fg.add(src)
+        adsb.front_end(fg, src, 4_000_000)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "adsb_rx_front_end_graph", "items": ns, "s": round(best, 4),
+                      "Gsamples_s_end_to_end": round(ns / best / 1e9, 4),
+                      "note": "whole graph, end to end: VectorSource H2D + resampler + NormSqr + 2 FIR + AdsbDemod, "
+                              "driven by edges.Flowgraph from Python"}), flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -481,6 +531,8 @@ def main():
         stream_section(quick)
     if want("boxavg"):
         boxavg_section(quick)
+    if want("adsb"):
+        adsb_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
