@@ -5,7 +5,8 @@ Python host layer above the C ABI (include/b200sdr.h).  Class and method names m
 reference's Rust API for this path (futuredsp::{FirFilter, DecimatingFirFilter,
 PolyphaseResamplingFir}, futuredsp::{firdes::hilbert, windows::hamming}, futuresdr::blocks::{Fir,
 FirBuilder, Fft, Apply, PfbArbResampler, SignalSource, SignalSourceBuilder, FixedPointPhase, Head,
-Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver}, the WLAN / M17 receivers' MovingAverage,
+Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver}, the WLAN / M17 receivers' MovingAverage, the ZigBee
+receiver's ClockRecoveryMm and Decoder,
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -21,7 +22,7 @@ from .filters import (  # noqa: F401
 from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
     Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator, MovingAverage,
-    AdsbDemod,
+    AdsbDemod, ClockRecoveryMm, ZigbeeDecoder,
 )
-from . import adsb, firdes, windows  # noqa: F401
+from . import adsb, firdes, windows, zigbee  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

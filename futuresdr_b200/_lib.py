@@ -18,7 +18,7 @@ INSUFFICIENT_INPUT, INSUFFICIENT_OUTPUT, BOTH_SUFFICIENT = 0, 1, 2
 F32_F32, C32_F32, C32_C32, F64_F64 = 0, 1, 2, 3
 ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
- OP_MAG_C32, OP_LOG10_F32) = range(8)
+ OP_MAG_C32, OP_LOG10_F32, OP_DC_BLOCK_F32) = range(9)
 WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
 (COMBINE_ADD_F32, COMBINE_SUB_F32, COMBINE_MUL_F32, COMBINE_CONJ_MUL_C32, COMBINE_MAG_DIV_C32_F32, COMBINE_TO_C32,
  COMBINE_TO_C32_NEG_Q) = range(7)
@@ -151,6 +151,16 @@ SIGNATURES = {
     "b2s_adsb_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _i32, _szp, _i32p]),
     "b2s_adsb_drain_packets": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_adsb_drain_detections": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_mmclock_create": (_i32, [_vp, _f32, _f32, _f32, _f32, _f32, _vpp]),
+    "b2s_mmclock_destroy": (None, [_vp]),
+    "b2s_mmclock_reset": (_i32, [_vp]),
+    "b2s_mmclock_look_ahead": (_sz, [_vp]),
+    "b2s_mmclock_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp]),
+    "b2s_zigbee_create": (_i32, [_vp, C.c_uint32, _vpp]),
+    "b2s_zigbee_destroy": (None, [_vp]),
+    "b2s_zigbee_reset": (_i32, [_vp]),
+    "b2s_zigbee_exec": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_zigbee_drain_frames": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_window_hamming": (_sz, [_sz, _i32, C.POINTER(C.c_double), _sz]),
     "b2s_firdes_hilbert": (_sz, [C.POINTER(C.c_double), _sz, _f32p, _sz]),
 }

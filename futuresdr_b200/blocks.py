@@ -14,6 +14,9 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``StreamDuplicator`` / ``StreamDeinterleaver``   src/blocks/stream_duplicator.rs, stream_deinterleaver.rs
   * ``AdsbDemod``                 examples/adsb/src/{preamble_detector,demodulator,decoder}.rs (PreambleDetector,
                                   Demodulator and Decoder::check_crc fused; helpers in futuresdr_b200.adsb)
+  * ``ClockRecoveryMm``           examples/zigbee/src/clock_recovery_mm.rs:28-97
+  * ``ZigbeeDecoder``             examples/zigbee/src/decoder.rs:78-183 with Mac::check_crc (mac.rs:62-85); helpers in
+                                  futuresdr_b200.zigbee
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
 
@@ -423,6 +426,7 @@ class ApplyOp(enum.IntEnum):
     ExpF32 = _lib.OP_EXP_F32
     MagC32 = _lib.OP_MAG_C32
     Log10F32 = _lib.OP_LOG10_F32
+    DcBlockF32 = _lib.OP_DC_BLOCK_F32      # param = alpha: s = (1 - alpha) * s + alpha * x; y = x - s
 
 
 _APPLY_TYPES = {
@@ -430,6 +434,7 @@ _APPLY_TYPES = {
     ApplyOp.QuadDemod: (np.complex64, np.float32), ApplyOp.NormSqr: (np.complex64, np.float32),
     ApplyOp.QuadDemodC32: (np.complex64, np.complex64), ApplyOp.ExpF32: (np.float32, np.float32),
     ApplyOp.MagC32: (np.complex64, np.float32), ApplyOp.Log10F32: (np.float32, np.float32),
+    ApplyOp.DcBlockF32: (np.float32, np.float32),
 }
 
 
@@ -1000,6 +1005,97 @@ class AdsbDemod(Block, Handle):
         for p in ports:
             p.consume(c)
         if done:
+            io.finished = True
+
+
+class ClockRecoveryMm(Block, Handle):
+    """examples/zigbee/src/clock_recovery_mm.rs:28-97 (Mueller & Muller), f32 -> f32, bit for bit.  Consumption depends
+    on the data, so every exec synchronises once to learn its counts.  A NaN latches mu (nothing is consumed from then
+    on); a step that would move past the slice raises B200SdrError (ESTATE) with the block left before that step.
+    Finish rule: the input is finished and what is left of it is within the look-ahead, or the call consumed nothing
+    while it produced (a latched mu).  This departs from clock_recovery_mm.rs:92-94, which finishes as soon as the
+    input is finished: here an input is reported finished as soon as its writer is, while it can still hold items, and
+    finishing then would drop them (and the outputs they give) whenever the output buffer had cut the call short."""
+    _destroy = lib.b2s_mmclock_destroy
+    in_dtype = out_dtype = np.float32
+
+    def __init__(self, omega: float, gain_omega: float, mu: float, gain_mu: float, omega_relative_limit: float,
+                 ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self._h = C.c_void_p()
+        check(lib.b2s_mmclock_create(self.ctx.handle, float(omega), float(gain_omega), float(mu), float(gain_mu),
+                                     float(omega_relative_limit), C.byref(self._h)), self.ctx.handle)
+        self.look_ahead = int(lib.b2s_mmclock_look_ahead(self._h))
+        self._ports()
+        self.input.set_min_items(self.look_ahead + 1)                           # :37
+
+    def exec(self, i: torch.Tensor, o: torch.Tensor) -> tuple[int, int]:
+        """One call of the reference's work loop over device slices -> (consumed, produced); synchronises."""
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_mmclock_exec(self._h, _ptr(i), i.numel(), _ptr(o), o.numel(), C.byref(c), C.byref(p)),
+              self.ctx.handle)
+        return c.value, p.value
+
+    def reset(self):
+        check(lib.b2s_mmclock_reset(self._h), self.ctx.handle)
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()
+        c, p = self.exec(i, o)
+        self.input.consume(c)
+        self.output.produce(p)
+        if self.input.finished() and (i.numel() - c <= self.look_ahead or (c == 0 and p > 0)):
+            io.finished = True
+
+
+ZIGBEE_FRAME = np.dtype([("index", np.uint64), ("len", np.uint32), ("crc_ok", np.int32), ("bytes", np.uint8, 128)],
+                        align=True)                                                          # b2s_zigbee_frame
+
+
+class ZigbeeDecoder(Block, Handle):
+    """examples/zigbee/src/decoder.rs:78-183 with Mac::check_crc (mac.rs:62-85) as a device block: one f32 stream
+    input, no stream output.  The frames the reference posts come out of ``frames()``, a cumulative numpy structured
+    array (ZIGBEE_FRAME: the stream index of the chip that completed the frame, its length, whether its FCS checks,
+    its bytes); reading it synchronises.  Every exec consumes its whole slice and never synchronises."""
+    _destroy = lib.b2s_zigbee_destroy
+    in_dtype = np.float32
+    out_dtype = None
+
+    def __init__(self, threshold: int = 6, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.threshold = int(threshold)
+        self._h = C.c_void_p()
+        check(lib.b2s_zigbee_create(self.ctx.handle, C.c_uint32(self.threshold), C.byref(self._h)), self.ctx.handle)
+        self.input = Reader(self.in_dtype, _ctx_device(self.ctx))
+        self._fr = []
+
+    def exec(self, i: torch.Tensor) -> int:
+        c = C.c_size_t(0)
+        check(lib.b2s_zigbee_exec(self._h, _ptr(i), i.numel(), C.byref(c)), self.ctx.handle)
+        return c.value
+
+    def reset(self):
+        check(lib.b2s_zigbee_reset(self._h), self.ctx.handle)
+        self._fr = []
+
+    def frames(self) -> np.ndarray:
+        """Every frame so far (ZIGBEE_FRAME records, in stream order)."""
+        while True:
+            buf = np.zeros(1 << 12, ZIGBEE_FRAME)
+            n = C.c_size_t(0)
+            check(lib.b2s_zigbee_drain_frames(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
+                  self.ctx.handle)
+            self._fr.append(buf[:n.value])
+            if n.value < buf.size:
+                break
+        out = np.concatenate(self._fr)
+        self._fr = [out]
+        return out
+
+    def work(self, io: WorkIo):
+        i = self.input.slice()
+        self.input.consume(self.exec(i))
+        if self.input.finished():                                               # decoder.rs:174-176
             io.finished = True
 
 

@@ -27,9 +27,8 @@
 // flushes).  NaN compares false, f32::min / f32::max are fminf / fmaxf (the non-NaN operand).
 #include <algorithm>
 #include <cstdint>
-#include <vector>
 
-#include "common.cuh"
+#include "lists.cuh"
 
 namespace {
 
@@ -339,18 +338,6 @@ demod_kernel(const float *__restrict__ s, const State *__restrict__ st, const De
     }
 }
 
-// a list that keeps its first `valid` entries when it grows (stream-ordered copy, then the old memory is freed)
-template <typename T> int32_t grow(b2s_ctx *ctx, Buf<T> &b, size_t need, size_t valid, const char *what) {
-    if (b.size() >= need) return B2S_OK;
-    Buf<T> nb;
-    B2S_TRY(nb.alloc(ctx, std::max<size_t>({need, 2 * b.size(), 1024}), what));
-    valid = std::min(valid, b.size());
-    if (valid) B2S_CUDA(ctx, cudaMemcpyAsync(nb.get(), b.get(), valid * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    b = std::move(nb);
-    return B2S_OK;
-}
-
 }  // namespace
 
 struct b2s_adsb {
@@ -364,16 +351,9 @@ struct b2s_adsb {
     Buf<uint2> tfun, gfun, gent, tent; // transfer functions of tiles / groups, entries of groups / tiles
     size_t det_bound = 0, pk_bound = 0;   // upper bounds of the device lists' lengths
     size_t det_rd = 0, pk_rd = 0;         // entries already drained
-    // (n_det, n_pk) as the last exec left them, copied to pinned memory behind it; once `counted` has completed the
-    // host takes them as exact bounds, so the lists only grow with what was detected, not with the worst case
-    Buf<unsigned long long, Mem::Pinned> counts;
-    cudaEvent_t counted = nullptr;
-    bool counts_pending = false;
+    ListCounts<2> counts;                 // (n_det, n_pk) as the last exec left them
     int par = 0;
     bool done = false;
-    ~b2s_adsb() {
-        if (counted) cudaEventDestroy(counted);
-    }
 };
 
 namespace {
@@ -381,42 +361,9 @@ namespace {
 int32_t clear(b2s_adsb *p) {
     B2S_TRY(b2s_memset(p->ctx, p->st.get(), 0, sizeof(State)));
     p->det_bound = p->pk_bound = p->det_rd = p->pk_rd = 0;
-    p->counts_pending = false;
+    p->counts.pending = false;
     p->par = 0;
     p->done = false;
-    return B2S_OK;
-}
-
-// copy up to cap entries [rd, count) to `host` (keeping those `keep` accepts), and empty the list once all are out
-template <typename T, typename H, class K>
-int32_t drain(b2s_adsb *p, Buf<T> &list, unsigned long long State::*count, size_t &rd, size_t &bound,
-              H *host, size_t cap, size_t *n, K keep) {
-    b2s_ctx *ctx = p->ctx;
-    DeviceGuard g(ctx->device);
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    unsigned long long cnt = 0;
-    unsigned long long *d_cnt = &(p->st.get()->*count);
-    B2S_CUDA(ctx, cudaMemcpy(&cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost));
-    size_t out = 0;
-    std::vector<T> tmp;
-    while (out < cap && rd < cnt) {
-        const size_t k = std::min<size_t>(cap - out, cnt - rd);
-        tmp.resize(k);
-        B2S_CUDA(ctx, cudaMemcpy(tmp.data(), list.get() + rd, k * sizeof(T), cudaMemcpyDeviceToHost));
-        for (const T &e : tmp)
-            if (keep(e)) std::memcpy(host + out++, &e, sizeof(T));
-        rd += k;
-    }
-    p->counts_pending = false;                  // the bounds below are exact
-    if (rd == cnt) {
-        const unsigned long long zero = 0;
-        B2S_CUDA(ctx, cudaMemcpy(d_cnt, &zero, sizeof(zero), cudaMemcpyHostToDevice));
-        rd = 0;
-        bound = 0;
-    } else {
-        bound = cnt;
-    }
-    *n = out;
     return B2S_OK;
 }
 
@@ -435,8 +382,7 @@ int32_t b2s_adsb_create(b2s_ctx *ctx, float threshold, int32_t forward_failed_cr
     p->thr = threshold;
     p->forward_failed_crc = forward_failed_crc != 0;
     B2S_TRY(p->st.alloc(ctx, 1, "b2s_adsb_create: state"));
-    B2S_TRY(p->counts.alloc(ctx, 2, "b2s_adsb_create: list counts"));
-    B2S_CUDA(ctx, cudaEventCreateWithFlags(&p->counted, cudaEventDisableTiming));
+    B2S_TRY(p->counts.init(ctx, "b2s_adsb_create: list counts"));
     B2S_TRY(clear(p.get()));
     *out = p.release();
     return B2S_OK;
@@ -472,21 +418,9 @@ int32_t b2s_adsb_exec(b2s_adsb *p, const float *d_samples, size_t n_samples, con
     // the counts behind the last exec tighten the bounds once they have landed; an exec that would have to grow a list
     // waits for them first (growing synchronises anyway), so the capacity follows the true lengths
     const bool tight = p->dets.size() >= p->det_bound + bound_new && p->pks.size() >= p->pk_bound + kPend + bound_new;
-    if (p->counts_pending && !tight) B2S_CUDA(ctx, cudaEventSynchronize(p->counted));
-    if (p->counts_pending) {
-        const cudaError_t q = cudaEventQuery(p->counted);
-        if (q == cudaSuccess) {
-            p->det_bound = (size_t)p->counts.get()[0];
-            p->pk_bound = (size_t)p->counts.get()[1];
-            p->counts_pending = false;
-        } else if (q == cudaErrorNotReady) {
-            cudaGetLastError();                              // not an error: the last exec is still running
-        } else {
-            B2S_CUDA(ctx, q);
-        }
-    }
-    B2S_TRY(grow(ctx, p->dets, p->det_bound + bound_new, p->det_bound, "b2s_adsb_exec: detection list"));
-    B2S_TRY(grow(ctx, p->pks, p->pk_bound + kPend + bound_new, p->pk_bound, "b2s_adsb_exec: packet list"));
+    B2S_TRY(p->counts.refresh(ctx, !tight, {&p->det_bound, &p->pk_bound}));
+    B2S_TRY(list_grow(ctx, p->dets, p->det_bound + bound_new, p->det_bound, "b2s_adsb_exec: detection list"));
+    B2S_TRY(list_grow(ctx, p->pks, p->pk_bound + kPend + bound_new, p->pk_bound, "b2s_adsb_exec: packet list"));
     if (n_tiles) {
         B2S_TRY(p->bits.reserve(ctx, (size_t)n_tiles * 2 * kTW, "b2s_adsb_exec: bitmaps"));
         B2S_TRY(p->tfun.reserve(ctx, (size_t)n_tiles * 32, "b2s_adsb_exec: tile functions"));
@@ -518,9 +452,7 @@ int32_t b2s_adsb_exec(b2s_adsb *p, const float *d_samples, size_t n_samples, con
     demod_kernel<<<(unsigned)ceil_div(warps, 4), 128, 0, s>>>(d_samples, st, p->dets.get(), p->par, p->pks.get());
     B2S_CHECK_LAUNCH(ctx);
     static_assert(offsetof(State, n_pk) == offsetof(State, n_det) + sizeof(unsigned long long), "counts copy");
-    B2S_CUDA(ctx, cudaMemcpyAsync(p->counts.get(), &st->n_det, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, s));
-    B2S_CUDA(ctx, cudaEventRecord(p->counted, s));
-    p->counts_pending = true;
+    B2S_TRY(p->counts.record(ctx, &st->n_det));
     p->det_bound += bound_new;
     p->pk_bound += kPend + bound_new;
     p->par ^= 1;
@@ -533,13 +465,13 @@ int32_t b2s_adsb_exec(b2s_adsb *p, const float *d_samples, size_t n_samples, con
 int32_t b2s_adsb_drain_packets(b2s_adsb *p, b2s_adsb_packet *host, size_t cap, size_t *n) {
     if (!p || !n || (cap && !host)) return b2s_fail(p ? p->ctx : nullptr, B2S_EINVAL, "b2s_adsb_drain_packets: NULL argument");
     const bool all = p->forward_failed_crc;
-    return drain(p, p->pks, &State::n_pk, p->pk_rd, p->pk_bound, host, cap, n,
+    return list_drain(p->ctx, p->pks, &p->st.get()->n_pk, p->counts, p->pk_rd, p->pk_bound, host, cap, n,
                  [all](const Packet &e) { return all || e.crc_passed; });
 }
 
 int32_t b2s_adsb_drain_detections(b2s_adsb *p, b2s_adsb_detection *host, size_t cap, size_t *n) {
     if (!p || !n || (cap && !host)) return b2s_fail(p ? p->ctx : nullptr, B2S_EINVAL, "b2s_adsb_drain_detections: NULL argument");
-    return drain(p, p->dets, &State::n_det, p->det_rd, p->det_bound, host, cap, n,
+    return list_drain(p->ctx, p->dets, &p->st.get()->n_det, p->counts, p->det_rd, p->det_bound, host, cap, n,
                  [](const Det &) { return true; });
 }
 

@@ -6,14 +6,16 @@
 // state in device memory: the FM demodulator's `last` sample
 // (examples/fm-receiver/src/main.rs:99-104) is the previous input item, so item j reads
 // in[j-1] and item 0 reads the carried sample; after the launch the carry is refreshed from
-// in[m-1] on the same stream.
+// in[m-1] on the same stream.  The DC blocker's running average is carry.x, read and written by its kernel.
+#include <cmath>
+
 #include "chunks.cuh"
 
 struct b2s_apply {
     b2s_ctx *ctx = nullptr;
     b2s_op op = B2S_OP_SCALE_F32;
     float param = 1.0f;
-    Buf<float2> d_carry;         // closure state (QUAD_DEMOD*: last sample)
+    Buf<float2> d_carry;         // closure state (QUAD_DEMOD*: last sample; DC_BLOCK_F32: .x = the average)
 };
 
 namespace {
@@ -84,8 +86,63 @@ __global__ void apply_kernel(const void *__restrict__ vin, void *__restrict__ vo
     }
 }
 
+// B2S_OP_DC_BLOCK_F32: s = (1 - alpha) * s + alpha * x; y = x - s (examples/zigbee/src/bin/rx.rs:70-73).  Only the
+// two-operation chain s -> fmul -> fadd is sequential.  One CTA, a three-stage pipeline over chunks of kDcChunk items:
+// in phase k the I/O warps stage chunk k (cp.async) and form alpha * x off the chain, lane 0 of warp 0 runs the chain
+// over chunk k - 1 (overwriting alpha * x with s), and the I/O warps store x - s of chunk k - 2.
+constexpr int kDcChunk = 2048;
+__global__ void __launch_bounds__(kThreads)
+dc_block_kernel(const float *__restrict__ in, float *__restrict__ out, long long m, float alpha, float oma,
+                float2 *__restrict__ carry) {
+    __shared__ float xs[3][kDcChunk];
+    __shared__ float as[3][kDcChunk];
+    const int tid = threadIdx.x;
+    const long long nch = (m + kDcChunk - 1) / kDcChunk;
+    float s = carry->x;
+    for (long long k = 0; k <= nch + 1; k++) {
+        if (tid < 32) {
+            if (tid == 0 && k >= 1 && k <= nch) {
+                float *a = as[(k - 1) % 3];
+                const int cnt = (int)min((long long)kDcChunk, m - (k - 1) * kDcChunk);
+#pragma unroll 8
+                for (int i = 0; i < cnt; i++) {
+                    s = __fadd_rn(__fmul_rn(oma, s), a[i]);
+                    a[i] = s;
+                }
+            }
+        } else {
+            const int t = tid - 32, nt = kThreads - 32;
+            if (k < nch) {                                   // stage chunk k
+                const long long base = k * kDcChunk;
+                const int cnt = (int)min((long long)kDcChunk, m - base);
+                float *x = xs[k % 3], *a = as[k % 3];
+                for (int i = t; i < cnt; i += nt) cp_async::ca4(x + i, in + base + i);
+                cp_async::commit();
+                cp_async::wait<0>();
+                for (int i = t; i < cnt; i += nt) a[i] = __fmul_rn(alpha, x[i]);   // the thread's own copies
+            }
+            if (k >= 2) {                                    // store chunk k - 2
+                const long long base = (k - 2) * kDcChunk;
+                const int cnt = (int)min((long long)kDcChunk, m - base);
+                const float *x = xs[(k - 2) % 3], *a = as[(k - 2) % 3];
+                for (int i = t; i < cnt; i += nt) out[base + i] = __fsub_rn(x[i], a[i]);
+            }
+        }
+        __syncthreads();
+    }
+    if (tid == 0) carry->x = s;
+}
+
 template <int OP>
 int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
+    if constexpr (OP == B2S_OP_DC_BLOCK_F32) {
+        b2s_ctx *ctx = a->ctx;
+        const float oma = 1.0f - a->param;                   // `1.0 - alpha` in f32
+        dc_block_kernel<<<1, kThreads, 0, ctx->stream>>>((const float *)in, (float *)out, (long long)n, a->param, oma,
+                                                          a->d_carry.get());
+        B2S_CHECK_LAUNCH(ctx);
+        return B2S_OK;
+    }
     b2s_ctx *ctx = a->ctx;
     apply_kernel<OP><<<grid_for(ctx, n, 16), kThreads, 0, ctx->stream>>>(in, out, (long long)n, a->param,
                                                                          a->d_carry.get());
@@ -105,7 +162,9 @@ extern "C" {
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out) {
     if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: NULL argument");
     *out = nullptr;
-    if ((int)op < 0 || (int)op > (int)B2S_OP_LOG10_F32) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
+    if ((int)op < 0 || (int)op > (int)B2S_OP_DC_BLOCK_F32) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
+    if (op == B2S_OP_DC_BLOCK_F32 && !std::isfinite(param))
+        return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: DC blocker alpha %g (a finite value)", (double)param);
     DeviceGuard g(ctx->device);
     PlanPtr<b2s_apply> a(new b2s_apply());
     a->ctx = ctx; a->op = op; a->param = param;
@@ -134,6 +193,12 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
     if (!d_in || !d_out) return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: NULL buffer");
     // the demodulators read in[j-1] while a neighbour thread writes out[j-1]: the slices must not overlap
     // (the element-wise ops may run in place)
+    if (a->op == B2S_OP_DC_BLOCK_F32) {
+        if (!word_aligned(d_in) || !word_aligned(d_out))
+            return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: a slice is not 4-byte aligned");
+        if (overlap(d_in, m * sizeof(float), d_out, m * sizeof(float)))
+            return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the DC blocker cannot run in place (input and output overlap)");
+    }
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {
         if (overlap(d_in, m * sizeof(float2), d_out, m * (a->op == B2S_OP_QUAD_DEMOD ? sizeof(float) : sizeof(float2))))
             return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the quadrature demodulator cannot run in place (input and output overlap)");
@@ -150,6 +215,7 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
         case B2S_OP_EXP_F32: rc = launch<B2S_OP_EXP_F32>(a, d_in, d_out, m); break;
         case B2S_OP_MAG_C32: rc = launch<B2S_OP_MAG_C32>(a, d_in, d_out, m); break;
         case B2S_OP_LOG10_F32: rc = launch<B2S_OP_LOG10_F32>(a, d_in, d_out, m); break;
+        case B2S_OP_DC_BLOCK_F32: rc = launch<B2S_OP_DC_BLOCK_F32>(a, d_in, d_out, m); break;
     }
     if (rc != B2S_OK) return rc;
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {

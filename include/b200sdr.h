@@ -205,7 +205,11 @@ typedef enum {
     B2S_OP_QUAD_DEMOD_C32 = 4, /* c32 -> c32 {re: phase, im: 0}: demod packed for PfbArbResampler (SURVEY §7) */
     B2S_OP_EXP_F32       = 5, /* f32 -> f32: exp(x)            (examples/vulkan/src/main.rs:17-29)            */
     B2S_OP_MAG_C32       = 6, /* c32 -> f32: sqrt(re^2 + im^2)                                               */
-    B2S_OP_LOG10_F32     = 7  /* f32 -> f32: param * log10(x)   (spectrum dB stage)                           */
+    B2S_OP_LOG10_F32     = 7, /* f32 -> f32: param * log10(x)   (spectrum dB stage)                           */
+    B2S_OP_DC_BLOCK_F32  = 8  /* f32 -> f32: s = (1 - param) * s + param * x; y = x - s, stateful, s starts at 0
+                               * (the one-pole DC blocker of examples/zigbee/src/bin/rx.rs:66-74 and
+                               * examples/keyfob/src/main.rs:62-68).  param must be finite (B2S_EINVAL otherwise).
+                               * A sequential recurrence: bit-exact under any slicing, one CTA per call. */
 } b2s_op;
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out);
 void    b2s_apply_destroy(b2s_apply *a);
@@ -498,6 +502,45 @@ int32_t b2s_adsb_exec(b2s_adsb *p, const float *d_samples, size_t n_samples, con
                       const float *d_corr, size_t n_corr, int32_t finished, size_t *consumed, int32_t *done);
 int32_t b2s_adsb_drain_packets(b2s_adsb *p, b2s_adsb_packet *host, size_t cap, size_t *n);
 int32_t b2s_adsb_drain_detections(b2s_adsb *p, b2s_adsb_detection *host, size_t cap, size_t *n);
+
+/* ---- Mueller & Muller clock recovery (≙ examples/zigbee/src/clock_recovery_mm.rs:28-97), f32 -> f32, bit for bit.
+ *   create: omega, gain_omega, mu, gain_mu and omega_relative_limit must be finite, omega * omega_relative_limit must
+ *           be >= 0 (f32::clamp panics otherwise) and look_ahead = ceil(omega + omega * omega_relative_limit + gain_mu)
+ *           (f32, saturating cast) must be >= 1 (the loop reads i[ii + 1]); B2S_EINVAL otherwise.
+ *   exec:   the reference's loop over one slice: while ii + look_ahead < n_in and oo < n_out_cap, one output per step.
+ *           Consumption depends on the data, so the call SYNCHRONISES once to return *consumed (ii) and *produced (oo).
+ *           A NaN latches mu: from then on nothing is consumed and every call fills its output.  A step that would
+ *           move ii past n_in (|input| far above the loop's design range, or +inf) is B2S_ESTATE: *consumed /
+ *           *produced and the block's state are those before that step.  Slices: 4-byte aligned, disjoint.
+ *   reset:  back to the parameters given to create. */
+typedef struct b2s_mmclock b2s_mmclock;
+int32_t b2s_mmclock_create(b2s_ctx *ctx, float omega, float gain_omega, float mu, float gain_mu,
+                           float omega_relative_limit, b2s_mmclock **out);
+void    b2s_mmclock_destroy(b2s_mmclock *p);
+int32_t b2s_mmclock_reset(b2s_mmclock *p);
+size_t  b2s_mmclock_look_ahead(const b2s_mmclock *p);
+int32_t b2s_mmclock_exec(b2s_mmclock *p, const float *d_in, size_t n_in, float *d_out, size_t n_out_cap,
+                         size_t *consumed, size_t *produced);
+
+/* ---- the ZigBee (IEEE 802.15.4 O-QPSK) chip decoder (≙ examples/zigbee/src/decoder.rs:78-183) with the Mac's FCS
+ * check (mac.rs:62-85), one f32 stream input, frames out as a list.  Chip = v > 0; a 32-chip shift register matched
+ * against the 16 chip sequences with mask 0x7FFFFFFE and Hamming distance < threshold.
+ *   exec:   consumes the whole slice (4-byte aligned); stream-ordered, no synchronisation except when the exec's worst
+ *           case (one frame per 192 chips) does not fit the list's capacity, which doubles it (see ADS-B above).
+ *   drain:  synchronises, copies up to cap frames in stream order to `host` (*n of them) and removes them.
+ *   reset:  back to the stream's start (Search, empty shift register), list emptied. */
+typedef struct {
+    uint64_t index;       /* stream index of the chip that completed the frame */
+    uint32_t len;         /* bytes posted, FCS included (1..127) */
+    int32_t  crc_ok;      /* Mac::calc_crc(bytes) == 0 && len > 2 */
+    uint8_t  bytes[128];  /* bytes[0..len) */
+} b2s_zigbee_frame;
+typedef struct b2s_zigbee b2s_zigbee;
+int32_t b2s_zigbee_create(b2s_ctx *ctx, uint32_t threshold, b2s_zigbee **out);
+void    b2s_zigbee_destroy(b2s_zigbee *p);
+int32_t b2s_zigbee_reset(b2s_zigbee *p);
+int32_t b2s_zigbee_exec(b2s_zigbee *p, const float *d_in, size_t n_in, size_t *consumed);
+int32_t b2s_zigbee_drain_frames(b2s_zigbee *p, b2s_zigbee_frame *host, size_t cap, size_t *n);
 
 /* ---- tap design, host side, f64 then cast (≙ futuredsp::firdes::kaiser, firdes/basic.rs:310-459)
  * Return the tap count; write taps only if cap is large enough (call with taps=NULL to size). */

@@ -734,6 +734,75 @@ private:
     const Instance &inst_; Handle<b2s_adsb, b2s_adsb_destroy> h_;
 };
 
+// ≙ the ZigBee receiver's ClockRecoveryMm (examples/zigbee/src/clock_recovery_mm.rs:28-97), f32 -> f32 (b2s_mmclock_*).
+// exec() synchronises once (consumption depends on the data); a step that would move past the slice (B2S_ESTATE)
+// throws Error, with the block left before that step.  work() finishes once the input is finished and what is left of
+// it is within the look-ahead, or the call consumed nothing while it produced (a latched mu).  The reference finishes as
+// soon as its input is finished; here a finished input can still hold items, and those are processed first.
+class ClockRecoveryMm {
+public:
+    ClockRecoveryMm(const Instance &inst, float omega, float gain_omega, float mu, float gain_mu,
+                    float omega_relative_limit)
+        : input(inst), output(inst), inst_(inst) {
+        check(b2s_mmclock_create(inst.get(), omega, gain_omega, mu, gain_mu, omega_relative_limit, out_ptr(h_)),
+              inst.get());
+    }
+    void reset() { check(b2s_mmclock_reset(h_.get()), inst_.get()); }
+    size_t look_ahead() const { return b2s_mmclock_look_ahead(h_.get()); }
+    // one call of the reference's loop over device slices: (consumed, produced)
+    std::pair<size_t, size_t> exec(const float *in, size_t n_in, float *out, size_t n_out_cap) {
+        size_t c = 0, p = 0;
+        check(b2s_mmclock_exec(h_.get(), in, n_in, out, n_out_cap, &c, &p), inst_.get());
+        return {c, p};
+    }
+    void work(WorkIo &io) {
+        const size_t n = input.len();
+        auto [c, p] = exec(input.slice(), n, output.slice(), output.capacity());
+        input.consume(c);
+        output.produce(p);
+        if (input.finished() && (n - c <= look_ahead() || (c == 0 && p > 0))) io.finished = true;
+    }
+    Reader<float> input;
+    Writer<float> output;
+private:
+    const Instance &inst_; Handle<b2s_mmclock, b2s_mmclock_destroy> h_;
+};
+
+// ≙ the ZigBee receiver's Decoder (examples/zigbee/src/decoder.rs:78-183) with Mac::check_crc (mac.rs:62-85)
+// (b2s_zigbee_*).  One f32 stream input, no stream output; the frames the reference posts are drained from the block.
+// Every exec consumes its whole slice and never synchronises; work() finishes when the input is finished (:174-176).
+class ZigbeeDecoder {
+public:
+    ZigbeeDecoder(const Instance &inst, uint32_t threshold = 6) : input(inst), inst_(inst) {
+        check(b2s_zigbee_create(inst.get(), threshold, out_ptr(h_)), inst.get());
+    }
+    void reset() { check(b2s_zigbee_reset(h_.get()), inst_.get()); }
+    size_t exec(const float *in, size_t n_in) {
+        size_t c = 0;
+        check(b2s_zigbee_exec(h_.get(), in, n_in, &c), inst_.get());
+        return c;
+    }
+    void work(WorkIo &io) {
+        input.consume(exec(input.slice(), input.len()));
+        if (input.finished()) io.finished = true;
+    }
+    // every frame since the last drain, in stream order (synchronises)
+    std::vector<b2s_zigbee_frame> drain_frames() {
+        std::vector<b2s_zigbee_frame> out;
+        for (;;) {
+            const size_t k = out.size();
+            out.resize(k + 1024);
+            size_t n = 0;
+            check(b2s_zigbee_drain_frames(h_.get(), out.data() + k, 1024, &n), inst_.get());
+            out.resize(k + n);
+            if (n < 1024) return out;
+        }
+    }
+    Reader<float> input;
+private:
+    const Instance &inst_; Handle<b2s_zigbee, b2s_zigbee_destroy> h_;
+};
+
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
 template <typename T, int32_t Deinterleave> class FanOut {
     static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");

@@ -45,7 +45,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 def want(section):
     """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
-    scale)."""
+    zigbee, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -346,6 +346,110 @@ def adsb_section(quick):
                               "driven by edges.Flowgraph from Python"}), flush=True)
 
 
+def zigbee_section(quick):
+    """The ZigBee receive chain (csrc/apply.cu DcBlockF32, csrc/zigbee.cu ClockRecoveryMm and ZigbeeDecoder) at 64 Mi
+    items per exec in Msamples/s, each serial kernel also as SM cycles per step at the card's maximum SM clock; the
+    front end (rx.rs:66-92) end to end through edges.Flowgraph; and the C oracle of each stage on one CPU thread."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import zigbee_oracle as zo
+    from futuresdr_b200 import zigbee
+    from futuresdr_b200.edges import Flowgraph, VectorSource
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    gpu = q[torch.cuda.current_device()] if q else "unknown"
+    print(json.dumps({"kernel": "zigbee_device", "gpu": gpu}), flush=True)
+    try:
+        mhz = float(gpu.split(",")[2].split()[0])
+    except Exception:
+        mhz = float("nan")
+    n = (16 if quick else 64) << 20
+    rng = np.random.default_rng(0)
+    ph = torch.from_numpy((np.sin(np.arange(n) * 0.7) * 1.2 + 0.3 * rng.standard_normal(n)).astype(np.float32)).cuda()
+    out = torch.empty(n, device="cuda")
+
+    def line(name, items, sec, steps=None):
+        d = {"kernel": f"zigbee_{name}", "items": items, "ms": round(sec * 1e3, 3),
+             "Msamples_s": round(items / sec / 1e6, 2)}
+        if steps is not None:
+            d["steps"] = steps
+            d["cycles_per_step_at_max_sm_clock"] = round(sec * mhz * 1e6 / steps, 2)
+        print(json.dumps(d), flush=True)
+
+    dc = B.Apply(B.ApplyOp.DcBlockF32, zigbee.DC_ALPHA)
+    line("dc_block", n, timeit(lambda: dc.apply(ph, out), iters=3, warm=1), n)
+    mm = B.ClockRecoveryMm(zigbee.MM_OMEGA, zigbee.MM_GAIN_OMEGA, zigbee.MM_MU, zigbee.MM_GAIN_MU,
+                           zigbee.MM_OMEGA_RELATIVE_LIMIT)
+    mm.exec(ph[:1 << 20], out)
+    best, produced, clocks = None, 0, []
+    import threading
+    stop = threading.Event()
+
+    def sample():                                                # the SM clock while the one-CTA kernel runs
+        while not stop.wait(0.25):
+            r = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=clocks.sm",
+                                "--format=csv,noheader,nounits"], capture_output=True, text=True).stdout.strip()
+            if r.isdigit():
+                clocks.append(int(r))
+    th = threading.Thread(target=sample)
+    th.start()
+    for _ in range(3):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        c, produced = mm.exec(ph, out)                           # synchronises
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    stop.set()
+    th.join()
+    line("clock_recovery_mm", n, best, produced)
+    if clocks:
+        med = float(np.median(clocks))
+        print(json.dumps({"kernel": "zigbee_clock_recovery_mm_sm_clock", "samples": len(clocks), "median_mhz": med,
+                          "min_mhz": min(clocks), "max_mhz": max(clocks),
+                          "cycles_per_step_at_median_clock": round(best * med * 1e6 / produced, 2)}), flush=True)
+    dec = B.ZigbeeDecoder(zigbee.DECODER_THRESHOLD)
+    noise = torch.randn(n, device="cuda")
+    pre = zo.chips_of(bytes(4))[:256]
+    dense = torch.from_numpy(np.where(np.resize(pre, n) > 0, 1.0, -1.0).astype(np.float32)).cuda()
+    for name, x in (("decoder_noise", noise), ("decoder_all_preamble", dense)):
+        def run():
+            dec.reset()
+            dec.exec(x)
+        line(name, n, timeit(run, iters=5, warm=1))
+    del noise, dense, ph, out
+    torch.cuda.empty_cache()
+    ns = (4 if quick else 16) << 20
+    x = (np.random.default_rng(1).standard_normal(2 * ns).astype(np.float32).view(np.complex64))
+    best = None
+    for _ in range(3):
+        fg = Flowgraph()
+        src = VectorSource(x)
+        fg.add(src)
+        zigbee.front_end(fg, src)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "zigbee_rx_front_end_graph", "items": ns, "s": round(best, 4),
+                      "Msamples_s_end_to_end": round(ns / best / 1e6, 2),
+                      "note": "whole graph, end to end: VectorSource H2D + QuadDemod + DcBlockF32 + ClockRecoveryMm + "
+                              "ZigbeeDecoder, driven by edges.Flowgraph from Python"}), flush=True)
+    m = 4 << 20
+    xs = (np.sin(np.arange(m) * 0.7) * 1.2 + 0.3 * rng.standard_normal(m)).astype(np.float32)
+    t0 = time.perf_counter()
+    zo.DcBlock(zigbee.DC_ALPHA).work(xs)
+    t1 = time.perf_counter()
+    zo.Mm(zigbee.MM_OMEGA, zigbee.MM_GAIN_OMEGA, zigbee.MM_MU, zigbee.MM_GAIN_MU,
+          zigbee.MM_OMEGA_RELATIVE_LIMIT).work(xs, m)
+    t2 = time.perf_counter()
+    zo.Decoder(zigbee.DECODER_THRESHOLD).work(rng.standard_normal(m).astype(np.float32))
+    t3 = time.perf_counter()
+    for name, sec in (("dc_block", t1 - t0), ("clock_recovery_mm", t2 - t1), ("decoder_noise", t3 - t2)):
+        print(json.dumps({"kernel": f"zigbee_oracle_cpu_1thread_{name}", "items": m, "ms": round(sec * 1e3, 2),
+                          "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -533,6 +637,8 @@ def main():
         boxavg_section(quick)
     if want("adsb"):
         adsb_section(quick)
+    if want("zigbee"):
+        zigbee_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
