@@ -634,8 +634,10 @@ class SpectrumPipe(Block, Handle):
     fft_shift, None)`` -> ``Apply(|x|^2)`` -> ``MovingAvg<n>::new(decay_factor, history_size)`` of
     examples/spectrum/src/bin/cpu.rs:21-28, optionally followed by ``log10_scale * log10(.)`` (what the
     reference's CubeCL kernel fuses, perf/burn/src/bin/fft-cubecl-kernel.rs:115-146).  Complex<f32> in, f32 out;
-    only 8 B/sample in and ``n`` floats per ``history_size`` frames out touch HBM.  Values agree with the three
-    separate blocks to rounding (blocked-scan evaluation of the average), counts are MovingAvg's."""
+    only 8 B/sample in and ``n`` floats per ``history_size`` frames out touch HBM.  Counts are MovingAvg's.  Values
+    are the three separate blocks' to rounding: the average is a blocked scan, so every emitted value of every bin is
+    within 2*B + 4*u*V of the float64 recurrence V on the same |X|^2, B being the rounding-error bound of the
+    sequential f32 recurrence (tests/test_gpu_spectrum_bins.py)."""
     _destroy = lib.b2s_spectrum_destroy
     in_dtype = np.complex64
     out_dtype = np.float32

@@ -16,8 +16,11 @@
 //   3. spectrum_fixup  : emitted[o] += a^k * carry_g  (k = frames of group g up to and including the emitting one),
 //      then the optional k*log10.
 // In real arithmetic this IS the reference's recurrence; in f32 the rounding order of the carried-in term differs,
-// so parity with the oracle is a tolerance (1e-5 of the largest average, tests/test_gpu_spectrum.py), not bit
-// equality -- the unfused bit-exact blocks (fft.cu, apply.cu, mavg.cu) remain.  Why not one exact pass: a bin's chain
+// so parity with the oracle is a bound per emitted value of every bin, not bit equality: within 2 B + 4 u V of the
+// float64 recurrence V, B the rounding-error bound of the sequential f32 recurrence (tests/test_gpu_spectrum_bins.py)
+// -- the unfused bit-exact blocks (fft.cu, apply.cu, mavg.cu) remain.  The weights a^k, a^C, the scan's states and
+// the fix-up's product are float64: a^k leaves f32's normal range long before a^k * carry does (k > 38 at decay 0.9,
+// k > 149 at decay 0.5), and an f32 weight would lose the carried-in term there.  Why not one exact pass: a bin's chain
 // is 2 dependent f32 operations per frame (~8 cycles), i.e. at most ~240 M frames/s per bin however many SMs there
 // are.
 #include <cmath>
@@ -34,7 +37,7 @@ struct b2s_spectrum {
     Buf<float2> d_tw;
     Buf<float> d_avg;              // [n] running average, OUTPUT (post-shift) bin order
     Buf<float> d_final;            // [groups][n] local final states / carries (grown on demand)
-    Buf<float> d_pow;              // a^k, k = 0..cap
+    Buf<double> d_pow;             // a^k, k = 0..cap (float64: see the top of the file)
     size_t i = 0;                  // frames since the last emission (moving_avg.rs: self.i)
     int resident = 0;              // CTAs per SM of the kernel instantiation (occupancy query, first exec)
 };
@@ -121,58 +124,59 @@ __global__ void __launch_bounds__(kSpThreads, (LOG2N <= 12 ? 3 : 1)) spectrum_ke
 // per warp and took 224 us.  Carries and fix-up are separate again, each fully parallel.)
 constexpr int kScanSegs = 32;
 __global__ void __launch_bounds__(32 * kScanSegs)
-spectrum_scan(float *fin, float *avg, int n, int groups, float A, float A_last) {
-    __shared__ float sL[kScanSegs][33], sM[kScanSegs][33], sX[kScanSegs][33];
+spectrum_scan(float *fin, float *avg, int n, int groups, double A, double A_last) {
+    __shared__ double sL[kScanSegs][33], sM[kScanSegs][33], sX[kScanSegs][33];
     const int lane = threadIdx.x & 31, seg = threadIdx.x >> 5;
     const int bin = blockIdx.x * 32 + lane;
     const bool live = bin < n;
     const int per = (groups + kScanSegs - 1) / kScanSegs;
     const int g0 = min(seg * per, groups), g1 = min(g0 + per, groups);
-    float L = 0.0f, M = 1.0f;
+    double L = 0.0, M = 1.0;
     if (live) {
 #pragma unroll 4
         for (int g = g0; g < g1; g++) {
-            const float Ag = (g == groups - 1) ? A_last : A;
-            L = fmaf(Ag, L, fin[(size_t)g * n + bin]);
+            const double Ag = (g == groups - 1) ? A_last : A;
+            L = fma(Ag, L, (double)fin[(size_t)g * n + bin]);
             M *= Ag;
         }
     }
     sL[seg][lane] = L; sM[seg][lane] = M;
     __syncthreads();
     if (seg == 0) {
-        float x = live ? avg[bin] : 0.0f;
+        double x = live ? avg[bin] : 0.0;
         for (int sgm = 0; sgm < kScanSegs; sgm++) {
             sX[sgm][lane] = x;
-            x = fmaf(sM[sgm][lane], x, sL[sgm][lane]);
+            x = fma(sM[sgm][lane], x, sL[sgm][lane]);
         }
-        if (live) avg[bin] = x;                              // state after the call
+        if (live) avg[bin] = (float)x;                       // state after the call
     }
     __syncthreads();
     if (!live) return;
-    float x = sX[seg][lane];
+    double x = sX[seg][lane];
 #pragma unroll 4
     for (int g = g0; g < g1; g++) {
-        const float Ag = (g == groups - 1) ? A_last : A;
+        const double Ag = (g == groups - 1) ? A_last : A;
         const float f = fin[(size_t)g * n + bin];
-        fin[(size_t)g * n + bin] = x;                        // carry INTO group g
-        x = fmaf(Ag, x, f);
+        fin[(size_t)g * n + bin] = (float)x;                 // carry INTO group g
+        x = fma(Ag, x, (double)f);
     }
 }
 
 // emitted[row] += a^k * carry_g  (k = frames of group g up to and including the emitting one), then the optional
 // k*log10.  One row (or a 1024-bin slice of it) per CTA: the group / power look-up is per CTA, accesses are float4.
 __global__ void __launch_bounds__(256)
-spectrum_fixup(float *out, const float *__restrict__ carry, const float *__restrict__ apow, int n, long long C,
+spectrum_fixup(float *out, const float *__restrict__ carry, const double *__restrict__ apow, int n, long long C,
                int history, int i0, float log10_k) {
     const long long row = blockIdx.x;
     const long long f = (row + 1) * history - i0 - 1;          // frame (within the call) that emitted this row
     const long long g = f / C;
-    const float w = apow[(int)(f - g * C) + 1];
+    const double w = apow[(int)(f - g * C) + 1];
     const int b = (blockIdx.y * 256 + threadIdx.x) * 4;
     if (b >= n) return;
     float4 v = *reinterpret_cast<float4 *>(out + row * n + b);
     const float4 c = *reinterpret_cast<const float4 *>(carry + (size_t)g * n + b);
-    v.x = fmaf(w, c.x, v.x); v.y = fmaf(w, c.y, v.y); v.z = fmaf(w, c.z, v.z); v.w = fmaf(w, c.w, v.w);
+    v.x = (float)fma(w, (double)c.x, (double)v.x); v.y = (float)fma(w, (double)c.y, (double)v.y);
+    v.z = (float)fma(w, (double)c.z, (double)v.z); v.w = (float)fma(w, (double)c.w, (double)v.w);
     if (log10_k != 0.0f) { v.x = log10_k * log10f(v.x); v.y = log10_k * log10f(v.y); v.z = log10_k * log10f(v.z); v.w = log10_k * log10f(v.w); }
     *reinterpret_cast<float4 *>(out + row * n + b) = v;
 }
@@ -266,10 +270,10 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     if (p->d_pow.size() < C + 1) {
         const size_t want = (C + 1) * 2;
         B2S_TRY(p->d_pow.reserve(ctx, want, "spectrum powers"));
-        std::vector<float> pw(want);
+        std::vector<double> pw(want);
         const double a = (double)(1.0f - p->decay);
-        for (size_t k = 0; k < want; k++) pw[k] = (float)std::pow(a, (double)k);
-        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_pow.get(), pw.data(), want * sizeof(float), cudaMemcpyHostToDevice, st));
+        for (size_t k = 0; k < want; k++) pw[k] = std::pow(a, (double)k);
+        B2S_CUDA(ctx, cudaMemcpyAsync(p->d_pow.get(), pw.data(), want * sizeof(double), cudaMemcpyHostToDevice, st));
         B2S_CUDA(ctx, cudaStreamSynchronize(st));            // pw is a stack-owned vector
     }
     SpArgs a;
@@ -281,7 +285,7 @@ int32_t b2s_spectrum_exec(b2s_spectrum *p, const void *d_in, size_t n_in, void *
     const double ad = (double)(1.0f - p->decay);
     const size_t c_last = frames - (groups - 1) * C;
     spectrum_scan<<<(unsigned)ceil_div(N, (size_t)32), 32 * kScanSegs, 0, st>>>(
-        p->d_final.get(), p->d_avg.get(), (int)N, (int)groups, (float)std::pow(ad, (double)C), (float)std::pow(ad, (double)c_last));
+        p->d_final.get(), p->d_avg.get(), (int)N, (int)groups, std::pow(ad, (double)C), std::pow(ad, (double)c_last));
     B2S_CHECK_LAUNCH(ctx);
     if (rows) {
         dim3 grid((unsigned)rows, (unsigned)ceil_div(N, (size_t)1024));
