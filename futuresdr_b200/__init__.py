@@ -3,10 +3,10 @@ FFT / Apply / PfbArbResampler hot path, and the stream plumbing of branching flo
 
 Python host layer above the C ABI (include/b200sdr.h).  Class and method names mirror the
 reference's Rust API for this path (futuredsp::{FirFilter, DecimatingFirFilter,
-PolyphaseResamplingFir}, futuredsp::{firdes::hilbert, windows::hamming}, futuresdr::blocks::{Fir,
+PolyphaseResamplingFir}, futuredsp::{firdes::{hilbert, lowpass}, windows::hamming}, futuresdr::blocks::{Fir,
 FirBuilder, Fft, Apply, PfbArbResampler, SignalSource, SignalSourceBuilder, FixedPointPhase, Head,
 Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver}, the WLAN / M17 receivers' MovingAverage, the ZigBee
-receiver's ClockRecoveryMm and Decoder,
+receiver's ClockRecoveryMm and Decoder, the keyfob receiver's Decoder,
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -22,7 +22,7 @@ from .filters import (  # noqa: F401
 from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
     Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator, MovingAverage,
-    AdsbDemod, ClockRecoveryMm, ZigbeeDecoder,
+    AdsbDemod, ClockRecoveryMm, ZigbeeDecoder, KeyfobDecoder, KEYFOB_CODE,
 )
-from . import adsb, firdes, windows, zigbee  # noqa: F401
+from . import adsb, firdes, keyfob, windows, zigbee  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

@@ -18,7 +18,8 @@ INSUFFICIENT_INPUT, INSUFFICIENT_OUTPUT, BOTH_SUFFICIENT = 0, 1, 2
 F32_F32, C32_F32, C32_C32, F64_F64 = 0, 1, 2, 3
 ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
- OP_MAG_C32, OP_LOG10_F32, OP_DC_BLOCK_F32) = range(9)
+ OP_MAG_C32, OP_LOG10_F32, OP_DC_BLOCK_F32, OP_SLICE_F32_U8) = range(10)
+KEYFOB_NONE, KEYFOB_CLOSE, KEYFOB_OPEN, KEYFOB_TRUNK = 0, 1, 2, 3
 WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
 (COMBINE_ADD_F32, COMBINE_SUB_F32, COMBINE_MUL_F32, COMBINE_CONJ_MUL_C32, COMBINE_MAG_DIV_C32_F32, COMBINE_TO_C32,
  COMBINE_TO_C32_NEG_Q) = range(7)
@@ -163,6 +164,12 @@ SIGNATURES = {
     "b2s_zigbee_drain_frames": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_window_hamming": (_sz, [_sz, _i32, C.POINTER(C.c_double), _sz]),
     "b2s_firdes_hilbert": (_sz, [C.POINTER(C.c_double), _sz, _f32p, _sz]),
+    "b2s_keyfob_create": (_i32, [_vp, _vpp]),
+    "b2s_keyfob_destroy": (None, [_vp]),
+    "b2s_keyfob_reset": (_i32, [_vp]),
+    "b2s_keyfob_exec": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_keyfob_drain_codes": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_firdes_lowpass": (_sz, [C.c_double, C.POINTER(C.c_double), _sz, _f32p, _sz]),
 }
 
 

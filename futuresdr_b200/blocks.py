@@ -17,6 +17,8 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``ClockRecoveryMm``           examples/zigbee/src/clock_recovery_mm.rs:28-97
   * ``ZigbeeDecoder``             examples/zigbee/src/decoder.rs:78-183 with Mac::check_crc (mac.rs:62-85); helpers in
                                   futuresdr_b200.zigbee
+  * ``KeyfobDecoder``             examples/keyfob/src/decoder.rs:64-127 with print (:36-52); helpers in
+                                  futuresdr_b200.keyfob
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
 
@@ -49,8 +51,8 @@ class WorkIo:
 
 
 def _tdtype(np_dtype):
-    return {np.dtype(np.complex64): torch.complex64, np.dtype(np.float64): torch.float64}.get(np.dtype(np_dtype),
-                                                                                             torch.float32)
+    return {np.dtype(np.complex64): torch.complex64, np.dtype(np.float64): torch.float64,
+            np.dtype(np.uint8): torch.uint8}.get(np.dtype(np_dtype), torch.float32)
 
 
 def _ctx_device(ctx) -> torch.device:
@@ -427,6 +429,7 @@ class ApplyOp(enum.IntEnum):
     MagC32 = _lib.OP_MAG_C32
     Log10F32 = _lib.OP_LOG10_F32
     DcBlockF32 = _lib.OP_DC_BLOCK_F32      # param = alpha: s = (1 - alpha) * s + alpha * x; y = x - s
+    SliceF32U8 = _lib.OP_SLICE_F32_U8      # f32 -> u8: x > 0 ? 1 : 0 (the keyfob receiver's slicer)
 
 
 _APPLY_TYPES = {
@@ -434,7 +437,7 @@ _APPLY_TYPES = {
     ApplyOp.QuadDemod: (np.complex64, np.float32), ApplyOp.NormSqr: (np.complex64, np.float32),
     ApplyOp.QuadDemodC32: (np.complex64, np.complex64), ApplyOp.ExpF32: (np.float32, np.float32),
     ApplyOp.MagC32: (np.complex64, np.float32), ApplyOp.Log10F32: (np.float32, np.float32),
-    ApplyOp.DcBlockF32: (np.float32, np.float32),
+    ApplyOp.DcBlockF32: (np.float32, np.float32), ApplyOp.SliceF32U8: (np.float32, np.uint8),
 }
 
 
@@ -1098,6 +1101,56 @@ class ZigbeeDecoder(Block, Handle):
         i = self.input.slice()
         self.input.consume(self.exec(i))
         if self.input.finished():                                               # decoder.rs:174-176
+            io.finished = True
+
+
+KEYFOB_CODE = np.dtype([("index", np.uint64), ("n_bits", np.uint32), ("label", np.int32), ("bits", np.uint8, 32)],
+                       align=True)                                                           # b2s_keyfob_code
+
+
+class KeyfobDecoder(Block, Handle):
+    """examples/keyfob/src/decoder.rs:64-127 with print (:36-52) as a device block: one u8 stream input, no stream
+    output.  The strings the reference logs come out of ``codes()``, a cumulative numpy structured array (KEYFOB_CODE:
+    the stream position of the flushing edge, the length after the prefix strip, the label of the last 8 bits, the
+    first 256 bits MSB first); reading it synchronises.  Every exec consumes its whole slice and never synchronises."""
+    _destroy = lib.b2s_keyfob_destroy
+    in_dtype = np.uint8
+    out_dtype = None
+
+    def __init__(self, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self._h = C.c_void_p()
+        check(lib.b2s_keyfob_create(self.ctx.handle, C.byref(self._h)), self.ctx.handle)
+        self.input = Reader(self.in_dtype, _ctx_device(self.ctx))
+        self._cd = []
+
+    def exec(self, i: torch.Tensor) -> int:
+        c = C.c_size_t(0)
+        check(lib.b2s_keyfob_exec(self._h, _ptr(i), i.numel(), C.byref(c)), self.ctx.handle)
+        return c.value
+
+    def reset(self):
+        check(lib.b2s_keyfob_reset(self._h), self.ctx.handle)
+        self._cd = []
+
+    def codes(self) -> np.ndarray:
+        """Every code so far (KEYFOB_CODE records, in stream order)."""
+        while True:
+            buf = np.zeros(1 << 12, KEYFOB_CODE)
+            n = C.c_size_t(0)
+            check(lib.b2s_keyfob_drain_codes(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
+                  self.ctx.handle)
+            self._cd.append(buf[:n.value])
+            if n.value < buf.size:
+                break
+        out = np.concatenate(self._cd)
+        self._cd = [out]
+        return out
+
+    def work(self, io: WorkIo):
+        i = self.input.slice()
+        self.input.consume(self.exec(i))
+        if self.input.finished():                                               # decoder.rs:120-122
             io.finished = True
 
 

@@ -6,7 +6,8 @@
 // state in device memory: the FM demodulator's `last` sample
 // (examples/fm-receiver/src/main.rs:99-104) is the previous input item, so item j reads
 // in[j-1] and item 0 reads the carried sample; after the launch the carry is refreshed from
-// in[m-1] on the same stream.  The DC blocker's running average is carry.x, read and written by its kernel.
+// in[m-1] on the same stream.  The DC blocker's running average is carry.x, read and written by its kernel.  The
+// keyfob slicer is the one op with a u8 output.
 #include <cmath>
 
 #include "chunks.cuh"
@@ -133,8 +134,36 @@ dc_block_kernel(const float *__restrict__ in, float *__restrict__ out, long long
     if (tid == 0) carry->x = s;
 }
 
+// B2S_OP_SLICE_F32_U8: x > 0 ? 1 : 0 (examples/keyfob/src/main.rs:73-75).  The chunk split of chunks.cuh with the head
+// aligning the OUTPUT to 4 bytes: a chunk's 4 outputs are one 32-bit store, and its 4 inputs one float4 when the input
+// (4-byte aligned) is then at 16 bytes, word loads otherwise.
+__device__ __forceinline__ unsigned char slice_one(float x) { return x > 0.0f ? 1 : 0; }   // NaN -> 0
+__global__ void __launch_bounds__(kThreads)
+slice_kernel(const float *__restrict__ in, unsigned char *__restrict__ out, unsigned long long m, unsigned head,
+             bool wide) {
+    chunk_loop(m, head,
+               [&](unsigned long long v) {
+                   float r[4];
+                   ld_chunk<1>(in + head + 4 * v, wide, r);
+                   const unsigned w = (unsigned)slice_one(r[0]) | (unsigned)slice_one(r[1]) << 8 |
+                                      (unsigned)slice_one(r[2]) << 16 | (unsigned)slice_one(r[3]) << 24;
+                   reinterpret_cast<unsigned *>(out + head)[v] = w;
+               },
+               [&](unsigned long long i) { out[i] = slice_one(__ldg(in + i)); });
+}
+
 template <int OP>
 int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
+    if constexpr (OP == B2S_OP_SLICE_F32_U8) {
+        b2s_ctx *ctx = a->ctx;
+        const unsigned head = (unsigned)std::min<size_t>(n, (4 - ((uintptr_t)out & 3)) & 3);
+        const float *fin = (const float *)in;
+        const bool wide = (((uintptr_t)(fin + head)) & 15) == 0;
+        slice_kernel<<<grid_for(ctx, std::max<size_t>((n - head) / 4, 1), 16), kThreads, 0, ctx->stream>>>(
+            fin, (unsigned char *)out, n, head, wide);
+        B2S_CHECK_LAUNCH(ctx);
+        return B2S_OK;
+    }
     if constexpr (OP == B2S_OP_DC_BLOCK_F32) {
         b2s_ctx *ctx = a->ctx;
         const float oma = 1.0f - a->param;                   // `1.0 - alpha` in f32
@@ -162,7 +191,7 @@ extern "C" {
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out) {
     if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: NULL argument");
     *out = nullptr;
-    if ((int)op < 0 || (int)op > (int)B2S_OP_DC_BLOCK_F32) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
+    if ((int)op < 0 || (int)op > (int)B2S_OP_SLICE_F32_U8) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
     if (op == B2S_OP_DC_BLOCK_F32 && !std::isfinite(param))
         return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: DC blocker alpha %g (a finite value)", (double)param);
     DeviceGuard g(ctx->device);
@@ -199,6 +228,11 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
         if (overlap(d_in, m * sizeof(float), d_out, m * sizeof(float)))
             return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the DC blocker cannot run in place (input and output overlap)");
     }
+    if (a->op == B2S_OP_SLICE_F32_U8) {
+        if (!word_aligned(d_in)) return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the slicer's input is not 4-byte aligned");
+        if (overlap(d_in, m * sizeof(float), d_out, m))
+            return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the slicer cannot run in place (input and output overlap)");
+    }
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {
         if (overlap(d_in, m * sizeof(float2), d_out, m * (a->op == B2S_OP_QUAD_DEMOD ? sizeof(float) : sizeof(float2))))
             return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the quadrature demodulator cannot run in place (input and output overlap)");
@@ -216,6 +250,7 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
         case B2S_OP_MAG_C32: rc = launch<B2S_OP_MAG_C32>(a, d_in, d_out, m); break;
         case B2S_OP_LOG10_F32: rc = launch<B2S_OP_LOG10_F32>(a, d_in, d_out, m); break;
         case B2S_OP_DC_BLOCK_F32: rc = launch<B2S_OP_DC_BLOCK_F32>(a, d_in, d_out, m); break;
+        case B2S_OP_SLICE_F32_U8: rc = launch<B2S_OP_SLICE_F32_U8>(a, d_in, d_out, m); break;
     }
     if (rc != B2S_OK) return rc;
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {

@@ -135,4 +135,13 @@ size_t b2s_firdes_hilbert(const double *window, size_t len, float *taps, size_t 
     return len;
 }
 
+// firdes::lowpass (basic.rs:25-42): window[n] * sinc term, omega_c / pi at x == 0, then cast to f32
+size_t b2s_firdes_lowpass(double cutoff, const double *window, size_t len, float *taps, size_t cap) {
+    if (len == 0 || !(std::fabs(cutoff) < 0.5)) return 0;
+    if (!window || !taps || cap < len) return len;
+    const auto h = windowed_sinc(cutoff, std::vector<double>(window, window + len));
+    for (size_t i = 0; i < len; i++) taps[i] = (float)h[i];
+    return len;
+}
+
 }  // extern "C"

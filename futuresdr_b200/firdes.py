@@ -1,4 +1,5 @@
-"""Tap design (host, f64): futuredsp::firdes::kaiser and firdes::hilbert (crates/futuredsp/src/firdes/basic.rs)."""
+"""Tap design (host, f64): futuredsp::firdes::kaiser, firdes::lowpass and firdes::hilbert
+(crates/futuredsp/src/firdes/basic.rs)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -39,4 +40,16 @@ def hilbert(window) -> np.ndarray:
     t = np.zeros(w.size, np.float32)
     lib.b2s_firdes_hilbert(w.ctypes.data_as(C.POINTER(C.c_double)), w.size, t.ctypes.data_as(C.POINTER(C.c_float)),
                            w.size)
+    return t
+
+
+def lowpass(cutoff: float, window) -> np.ndarray:
+    """firdes::lowpass::<f32> (basic.rs:25-42): the windowed sinc with cutoff in cycles per sample, one tap per window
+    entry."""
+    w = np.ascontiguousarray(window, dtype=np.float64)
+    assert abs(cutoff) < 0.5, "cutoff must be in ]-1/2, 1/2["                 # basic.rs:26
+    t = np.zeros(w.size, np.float32)
+    if w.size:
+        lib.b2s_firdes_lowpass(float(cutoff), w.ctypes.data_as(C.POINTER(C.c_double)), w.size,
+                               t.ctypes.data_as(C.POINTER(C.c_float)), w.size)
     return t

@@ -206,10 +206,13 @@ typedef enum {
     B2S_OP_EXP_F32       = 5, /* f32 -> f32: exp(x)            (examples/vulkan/src/main.rs:17-29)            */
     B2S_OP_MAG_C32       = 6, /* c32 -> f32: sqrt(re^2 + im^2)                                               */
     B2S_OP_LOG10_F32     = 7, /* f32 -> f32: param * log10(x)   (spectrum dB stage)                           */
-    B2S_OP_DC_BLOCK_F32  = 8  /* f32 -> f32: s = (1 - param) * s + param * x; y = x - s, stateful, s starts at 0
+    B2S_OP_DC_BLOCK_F32  = 8, /* f32 -> f32: s = (1 - param) * s + param * x; y = x - s, stateful, s starts at 0
                                * (the one-pole DC blocker of examples/zigbee/src/bin/rx.rs:66-74 and
                                * examples/keyfob/src/main.rs:62-68).  param must be finite (B2S_EINVAL otherwise).
                                * A sequential recurrence: bit-exact under any slicing, one CTA per call. */
+    B2S_OP_SLICE_F32_U8  = 9  /* f32 -> u8: x > 0 ? 1 : 0 (NaN and +-0 give 0), the keyfob receiver's slicer
+                               * (examples/keyfob/src/main.rs:73-75).  The input slice must be 4-byte aligned, the
+                               * output may start at any byte; the slices must not overlap (B2S_EINVAL otherwise). */
 } b2s_op;
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out);
 void    b2s_apply_destroy(b2s_apply *a);
@@ -542,6 +545,33 @@ int32_t b2s_zigbee_reset(b2s_zigbee *p);
 int32_t b2s_zigbee_exec(b2s_zigbee *p, const float *d_in, size_t n_in, size_t *consumed);
 int32_t b2s_zigbee_drain_frames(b2s_zigbee *p, b2s_zigbee_frame *host, size_t cap, size_t *n);
 
+/* ---- the keyfob receiver's Decoder (≙ examples/keyfob/src/decoder.rs:64-127 with print, :36-52), one u8 stream
+ * input, key codes out as a list.  An edge is a 1 while Down or a 0 while Up (other values are ignored); diff = its
+ * position minus the last edge's.  diff in 63..=83 sets `output`, or, if it was set, clears it and appends a bit;
+ * 131..=161 clears it and appends a bit (a rising edge appends 0, a falling edge 1); any other diff flushes the string
+ * through print: a string holding 10101111 is reported from its first occurrence on.  A string still pending when the
+ * input ends is never reported, as in the reference.
+ *   exec:   consumes the whole slice (any alignment); stream-ordered, no synchronisation except when the exec's worst
+ *           case (one code per 8 * 63 items, plus 2) does not fit the list's capacity, which doubles it.
+ *   drain:  synchronises, copies up to cap codes in stream order to `host` (*n of them) and removes them.
+ *   reset:  back to the stream's start (Down(0), output false, empty string), list emptied. */
+#define B2S_KEYFOB_NONE  0
+#define B2S_KEYFOB_CLOSE 1   /* the string ends in 11010101 */
+#define B2S_KEYFOB_OPEN  2   /* 11100011 */
+#define B2S_KEYFOB_TRUNK 3   /* 10111001 */
+typedef struct {
+    uint64_t index;       /* stream position of the flushing edge */
+    uint32_t n_bits;      /* length after the prefix strip (>= 8; saturates at 2^32 - 1) */
+    int32_t  label;       /* B2S_KEYFOB_*, from the string's true last 8 bits even when n_bits > 256 */
+    uint8_t  bits[32];    /* the first min(n_bits, 256) bits, MSB first; the rest 0 */
+} b2s_keyfob_code;
+typedef struct b2s_keyfob b2s_keyfob;
+int32_t b2s_keyfob_create(b2s_ctx *ctx, b2s_keyfob **out);
+void    b2s_keyfob_destroy(b2s_keyfob *p);
+int32_t b2s_keyfob_reset(b2s_keyfob *p);
+int32_t b2s_keyfob_exec(b2s_keyfob *p, const uint8_t *d_in, size_t n_in, size_t *consumed);
+int32_t b2s_keyfob_drain_codes(b2s_keyfob *p, b2s_keyfob_code *host, size_t cap, size_t *n);
+
 /* ---- tap design, host side, f64 then cast (≙ futuredsp::firdes::kaiser, firdes/basic.rs:310-459)
  * Return the tap count; write taps only if cap is large enough (call with taps=NULL to size). */
 size_t b2s_firdes_kaiser_lowpass(double cutoff, double transition_bw, double max_ripple,
@@ -554,6 +584,9 @@ size_t b2s_window_hamming(size_t len, int32_t periodic, double *out, size_t cap)
 /* ≙ futuredsp::firdes::hilbert (firdes/basic.rs:202-222): taps of the window's length, f64 then cast to f32.
  * The reference asserts an odd length: an even (or zero) length returns 0 taps. */
 size_t b2s_firdes_hilbert(const double *window, size_t len, float *taps, size_t cap);
+/* ≙ futuredsp::firdes::lowpass (firdes/basic.rs:25-42): the windowed sinc, one tap per window entry, f64 then cast to
+ * f32.  The reference asserts |cutoff| < 1/2: a cutoff outside that (or NaN), or len == 0, returns 0 taps. */
+size_t b2s_firdes_lowpass(double cutoff, const double *window, size_t len, float *taps, size_t cap);
 
 #ifdef __cplusplus
 }

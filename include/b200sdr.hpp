@@ -7,7 +7,7 @@
 //   futuresdr::blocks::{Fir, FirBuilder, Iir, IirBuilder, Fft, Apply, PfbArbResampler, SignalSource,
 //                       SignalSourceBuilder, FixedPointPhase, Head, Combine, Split, Delay,
 //                       StreamDuplicator, StreamDeinterleaver}                          (src/blocks/*.rs)
-//   futuredsp::{firdes::hilbert, windows::hamming}
+//   futuredsp::{firdes::{hilbert, lowpass}, windows::hamming}
 //   futuresdr::runtime::{WorkIo, mocker::Mocker}                        (work_io.rs, mocker.rs)
 //
 // The reference is Rust; no Rust toolchain exists in this image, so this header is the
@@ -430,7 +430,7 @@ private:
     const Instance &inst_; size_t len_; Handle<b2s_fft, b2s_fft_destroy> plan_;
 };
 
-// ≙ blocks::Apply (src/blocks/apply.rs:100-131) for the device op catalogue
+// ≙ blocks::Apply (src/blocks/apply.rs:100-131) for the device op catalogue; B2S_OP_SLICE_F32_U8 is Apply<float, uint8_t>
 template <typename A, typename B> class Apply {
 public:
     Apply(const Instance &inst, b2s_op op, float param = 1.0f) : input(inst), output(inst), inst_(inst) {
@@ -803,6 +803,41 @@ private:
     const Instance &inst_; Handle<b2s_zigbee, b2s_zigbee_destroy> h_;
 };
 
+// ≙ the keyfob receiver's Decoder (examples/keyfob/src/decoder.rs:64-127 with print, :36-52) (b2s_keyfob_*).  One u8
+// stream input, no stream output; the strings the reference logs are drained from the block as codes.  Every exec
+// consumes its whole slice and never synchronises; work() finishes when the input is finished (:120-122).
+class KeyfobDecoder {
+public:
+    explicit KeyfobDecoder(const Instance &inst) : input(inst), inst_(inst) {
+        check(b2s_keyfob_create(inst.get(), out_ptr(h_)), inst.get());
+    }
+    void reset() { check(b2s_keyfob_reset(h_.get()), inst_.get()); }
+    size_t exec(const uint8_t *in, size_t n_in) {
+        size_t c = 0;
+        check(b2s_keyfob_exec(h_.get(), in, n_in, &c), inst_.get());
+        return c;
+    }
+    void work(WorkIo &io) {
+        input.consume(exec(input.slice(), input.len()));
+        if (input.finished()) io.finished = true;
+    }
+    // every code since the last drain, in stream order (synchronises)
+    std::vector<b2s_keyfob_code> drain_codes() {
+        std::vector<b2s_keyfob_code> out;
+        for (;;) {
+            const size_t k = out.size();
+            out.resize(k + 1024);
+            size_t n = 0;
+            check(b2s_keyfob_drain_codes(h_.get(), out.data() + k, 1024, &n), inst_.get());
+            out.resize(k + n);
+            if (n < 1024) return out;
+        }
+    }
+    Reader<uint8_t> input;
+private:
+    const Instance &inst_; Handle<b2s_keyfob, b2s_keyfob_destroy> h_;
+};
+
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
 template <typename T, int32_t Deinterleave> class FanOut {
     static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");
@@ -837,7 +872,7 @@ template <typename T> using StreamDuplicator = FanOut<T, 0>;
 // ≙ blocks::StreamDeinterleaver<T> (stream_deinterleaver.rs:25-98): output[k][j] = input[j N + k], whole groups only
 template <typename T> using StreamDeinterleaver = FanOut<T, 1>;
 
-// ---- firdes::hilbert (firdes/basic.rs:202-222) and windows::hamming (windows.rs:109-120) ---------------------------
+// ---- firdes::hilbert (firdes/basic.rs:202-222), firdes::lowpass (:25-42) and windows::hamming (windows.rs:109-120) ---------------------------
 namespace windows {
 inline std::vector<double> hamming(size_t len, bool periodic) {
     std::vector<double> w(len);
@@ -850,6 +885,12 @@ inline std::vector<float> hilbert(const std::vector<double> &window) {
     if (window.size() % 2 == 0) throw Error(B2S_EINVAL, "firdes::hilbert: Must be an odd number");   // basic.rs:204
     std::vector<float> t(window.size());
     b2s_firdes_hilbert(window.data(), window.size(), t.data(), t.size());
+    return t;
+}
+inline std::vector<float> lowpass(double cutoff, const std::vector<double> &window) {
+    if (!(std::abs(cutoff) < 0.5)) throw Error(B2S_EINVAL, "firdes::lowpass: cutoff must be in ]-1/2, 1/2[");   // :26
+    std::vector<float> t(window.size());
+    if (!window.empty()) b2s_firdes_lowpass(cutoff, window.data(), window.size(), t.data(), t.size());
     return t;
 }
 }  // namespace firdes

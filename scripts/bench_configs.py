@@ -45,7 +45,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 def want(section):
     """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
-    zigbee, scale)."""
+    zigbee, keyfob, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -450,6 +450,80 @@ def zigbee_section(quick):
                           "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
 
 
+def keyfob_section(quick):
+    """The keyfob receive chain (csrc/apply.cu SliceF32U8, csrc/keyfob.cu KeyfobDecoder) at 64 Mi items per exec: the
+    slicer as a fraction of 3.35 TB/s at 5 B per item, the decoder on all zeros, on the slicer output of noise and on
+    the densest valid-pulse stream as items/s and as a fraction of 3.35 TB/s at 1 B per item; the front end
+    (main.rs:39-79) end to end through edges.Flowgraph; and the C oracle on one CPU thread."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import keyfob_oracle as ko
+    from futuresdr_b200 import keyfob
+    from futuresdr_b200.edges import Flowgraph, VectorSource
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    gpu = q[torch.cuda.current_device()] if q else "unknown"
+    print(json.dumps({"kernel": "keyfob_device", "gpu": gpu}), flush=True)
+    n = (16 if quick else 64) << 20
+    peak = 3.35e12
+
+    def line(name, items, sec, bytes_per_item):
+        print(json.dumps({"kernel": f"keyfob_{name}", "items": items, "ms": round(sec * 1e3, 3),
+                          "Gitems_s": round(items / sec / 1e9, 2),
+                          "frac_of_3p35_TBs": round(items * bytes_per_item / sec / peak, 3)}), flush=True)
+
+    x = torch.randn(n, device="cuda")
+    u = torch.empty(n, dtype=torch.uint8, device="cuda")
+    sl = B.Apply(B.ApplyOp.SliceF32U8)
+    line("slicer", n, timeit(lambda: sl.apply(x, u), iters=10, warm=2), 5)
+    lp = torch.from_numpy(np.convolve(np.random.default_rng(2).standard_normal(n + 127).astype(np.float32),
+                                      keyfob.lowpass_taps(), "valid").astype(np.float32)).cuda()
+    noise = torch.empty(n, dtype=torch.uint8, device="cuda")
+    sl.apply(lp, noise)
+    del x, lp
+    zeros = torch.zeros(n, dtype=torch.uint8, device="cuda")
+    dense = torch.from_numpy(np.resize(np.repeat(np.array([0, 1], np.uint8), 63), n)).cuda()
+    dec = B.KeyfobDecoder()
+    for name, s in (("decoder_zeros", zeros), ("decoder_noise_slicer", noise), ("decoder_dense_63", dense)):
+        def run():
+            dec.reset()
+            dec.exec(s)
+        line(name, n, timeit(run, iters=10, warm=2), 1)
+    del zeros, noise, dense, u
+    torch.cuda.empty_cache()
+    ns = (4 if quick else 16) << 20
+    xc = (np.random.default_rng(1).standard_normal(2 * ns).astype(np.float32).view(np.complex64))
+    best = None
+    for _ in range(3):
+        fg = Flowgraph()
+        src = VectorSource(xc)
+        fg.add(src)
+        keyfob.front_end(fg, src)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "keyfob_rx_front_end_graph", "items": ns, "s": round(best, 4),
+                      "Msamples_s_end_to_end": round(ns / best / 1e6, 2),
+                      "note": "whole graph at 4 Msps in: VectorSource H2D + resampler 1/16 + NormSqr + DcBlockF32 + "
+                              "128-tap FIR + SliceF32U8 + KeyfobDecoder, driven by edges.Flowgraph from Python"}),
+          flush=True)
+    m = 16 << 20
+    xs = np.random.default_rng(3).standard_normal(m).astype(np.float32)
+    ys = np.convolve(xs, keyfob.lowpass_taps(), "same").astype(np.float32)
+    t0 = time.perf_counter()
+    bits = ko.slice_u8(ys)
+    t1 = time.perf_counter()
+    ko.Decoder().work(bits)
+    t2 = time.perf_counter()
+    ko.Decoder().work(np.resize(np.repeat(np.array([0, 1], np.uint8), 63), m))
+    t3 = time.perf_counter()
+    for name, sec in (("slicer", t1 - t0), ("decoder_noise_slicer", t2 - t1), ("decoder_dense_63", t3 - t2)):
+        print(json.dumps({"kernel": f"keyfob_oracle_cpu_1thread_{name}", "items": m, "ms": round(sec * 1e3, 2),
+                          "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -639,6 +713,8 @@ def main():
         adsb_section(quick)
     if want("zigbee"):
         zigbee_section(quick)
+    if want("keyfob"):
+        keyfob_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
