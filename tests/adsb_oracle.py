@@ -1,47 +1,33 @@
 """CPU oracle of the ADS-B receiver's PreambleDetector -> Demodulator -> Decoder::check_crc (TEST INFRASTRUCTURE ONLY).
 
-ctypes front-end to ``tests/adsb_oracle.c`` (one reference call at a time, compiled with the system gcc into a
-temporary directory on first use).  ``replay`` drives the three blocks over any sequence of detector calls, and
-``np_detect`` / ``np_demod_bits`` are an independent numpy float32 transcription for cross-checking the C file.
+ctypes front-end to ``tests/adsb_oracle.c`` (one reference call at a time, compiled by ``native.load_oracle`` on
+first use).  ``replay`` drives the three blocks over any sequence of detector calls, and ``np_detect`` /
+``np_demod_bits`` are an independent numpy float32 transcription for cross-checking the C file.
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "adsb_oracle.c")
+from native import load_oracle
+
 _f32p = C.POINTER(C.c_float)
 _u64p = C.POINTER(C.c_uint64)
 _u8p = C.POINTER(C.c_uint8)
-_lib = None
 PACKET_SAMPLES = 480
 PREAMBLE_SAMPLES = 32
 
+SIGNATURES = {
+    "orc_adsb_detect": (C.c_size_t, [C.c_float, _f32p, C.c_size_t, _f32p, C.c_size_t, _f32p, C.c_size_t, C.c_size_t,
+                                     _u64p, _f32p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "orc_adsb_demod_bits": (None, [_f32p, C.c_size_t, _u8p]),
+    "orc_adsb_check_crc": (C.c_int, [_u8p, C.c_size_t]),
+}
+
 
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="adsb_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libadsb_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so], check=True)
-        L = C.CDLL(so)
-        L.orc_adsb_detect.restype = C.c_size_t
-        L.orc_adsb_detect.argtypes = [C.c_float, _f32p, C.c_size_t, _f32p, C.c_size_t, _f32p, C.c_size_t, C.c_size_t,
-                                      _u64p, _f32p, C.c_size_t, C.POINTER(C.c_size_t)]
-        L.orc_adsb_demod_bits.restype = None
-        L.orc_adsb_demod_bits.argtypes = [_f32p, C.c_size_t, _u8p]
-        L.orc_adsb_check_crc.restype = C.c_int
-        L.orc_adsb_check_crc.argtypes = [_u8p, C.c_size_t]
-        _lib = L
-    return _lib
+    return load_oracle("adsb_oracle", SIGNATURES)
 
 
 def _f(a):

@@ -1,8 +1,8 @@
 """CPU oracle of the WLAN and M17 receivers' MovingAverage (TEST INFRASTRUCTURE ONLY).
 
 ctypes front-end to ``tests/boxavg_oracle.c``, the C restatement of one work() call of
-examples/wlan/src/moving_average.rs:67-107 and examples/m17/src/moving_average.rs:41-81.  The library is compiled with
-the system gcc into a temporary directory on first use, so the repository tree may be read-only.
+examples/wlan/src/moving_average.rs:67-107 and examples/m17/src/moving_average.rs:41-81, compiled by
+``native.load_oracle`` on first use.
 
 ``BoxAvgRef.work`` is one reference call; ``BoxAvgRef.run`` emulates what one device exec covers: the calls the
 reference makes back to back on what is left of the slices, until a call makes no progress or ``max_calls`` calls have
@@ -10,41 +10,28 @@ run.  ``np_work`` is an independent numpy float32 transcription of one call, for
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 from dataclasses import dataclass
 
 import numpy as np
 
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "boxavg_oracle.c")
+from native import load_oracle
+
 _f32p = C.POINTER(C.c_float)
 _szp = C.POINTER(C.c_size_t)
 _ip = C.POINTER(C.c_int)
-_lib = None
 MAX_ITER = 4000
+
+SIGNATURES = {
+    "orc_boxavg_work_f32": (C.c_int, [C.c_size_t, C.c_int, C.c_float, _szp, _f32p, C.c_size_t, C.c_int, _f32p,
+                                      C.c_size_t, _szp, _szp, _ip, _ip]),
+    "orc_boxavg_work_c32": (C.c_int, [C.c_size_t, _szp, _f32p, C.c_size_t, C.c_int, _f32p, C.c_size_t, _szp, _szp,
+                                      _ip, _ip]),
+}
 
 
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="boxavg_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libboxavg_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so], check=True)
-        L = C.CDLL(so)
-        L.orc_boxavg_work_f32.restype = C.c_int
-        L.orc_boxavg_work_f32.argtypes = [C.c_size_t, C.c_int, C.c_float, _szp, _f32p, C.c_size_t, C.c_int, _f32p,
-                                          C.c_size_t, _szp, _szp, _ip, _ip]
-        L.orc_boxavg_work_c32.restype = C.c_int
-        L.orc_boxavg_work_c32.argtypes = [C.c_size_t, _szp, _f32p, C.c_size_t, C.c_int, _f32p, C.c_size_t, _szp,
-                                          _szp, _ip, _ip]
-        _lib = L
-    return _lib
+    return load_oracle("boxavg_oracle", SIGNATURES)
 
 
 @dataclass

@@ -1,20 +1,16 @@
 // test_adsb_host.cpp -- the ADS-B detector / demodulator / CRC block through the C++ host layer (include/b200sdr.hpp)
 // on a GPU: a public DF17 frame laid out as ideal PPM decodes to its bytes, a one-bit error is dropped or forwarded as
 // forward_failed_crc says, the repeated-index rule of the detector, ragged execs agree with one exec, and the
-// refusals.  Built by __graft_entry__.build(); run by tests/test_gpu_adsb_cpp_host.py (needs an H100).
+// refusals.  Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <limits>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 static const uint8_t kFrame[14] = {0x8D, 0x48, 0x40, 0xD6, 0x20, 0x2C, 0xC3, 0x71, 0xC3, 0x2C, 0xE0, 0x57, 0x60, 0x98};
 
@@ -121,7 +117,5 @@ int main() {
     }
     inst.sync();
     CHECK(b2s_ctx_bytes_held(inst.get()) == held);
-    if (failures) { std::printf("%d checks failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

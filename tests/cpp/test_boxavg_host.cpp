@@ -1,19 +1,15 @@
 // test_boxavg_host.cpp -- the WLAN / M17 MovingAverage through the C++ host layer (include/b200sdr.hpp) on a GPU: the
 // reference's own Mocker known answers (examples/wlan/src/moving_average.rs:117-153), the call loop, a Complex32 case,
 // the M17 divisor and the refusals.
-// Built by __graft_entry__.build(); run by tests/test_gpu_boxavg_cpp_host.py (needs an H100).
+// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 template <typename Block> static WorkIo mocker_run(Block &b) {                     // Mocker::run: again while call_again
     WorkIo io;
@@ -97,7 +93,5 @@ int main() {
     }
     inst.sync();
     CHECK(b2s_ctx_bytes_held(inst.get()) == held);
-    if (failures) { std::printf("%d checks failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

@@ -6,13 +6,9 @@
 #include <random>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 using CS = ComputationStatus;
 static bool eq(const FilterResult &r, size_t c, size_t p, CS s) {
@@ -241,6 +237,5 @@ int main() {
         // |X|^2 = N^2 at the tone; avg after 6 frames with decay 0.5 = N^2 * (1 - 0.5^6)
         if (v.size() == 2 * N) CHECK(std::fabs(v[N + peak] - (float)(N * N) * (1.0f - 0.015625f)) <= 1e-3f * N * N);
     }
-    std::printf(failures ? "C++ host layer: %d FAILURES\n" : "C++ host layer: all checks passed\n", failures);
-    return failures ? 1 : 0;
+    return report();
 }

@@ -1,17 +1,13 @@
 // test_iir_host.cpp -- the reference's IirFilter tests (crates/futuredsp/src/iir.rs:23-31, :186-236) replayed through
 // the C++ host layer (include/b200sdr.hpp) on a GPU, under every algorithm that admits the filter.
-// Built by __graft_entry__.build(); run by tests/test_gpu_iir_cpp_host.py (needs an H100).
+// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cstdio>
 #include <optional>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 // the Feeder of iir.rs:186-203: append one sample, filter into a one-item slice, drain what was consumed
 struct Feeder {
@@ -85,7 +81,5 @@ int main() {
         CHECK(y.size() == 4 && y[0] == 15.0f && y[1] == 17.5f && y[2] == 18.75f && y[3] == 19.375f);
     }
     inst.sync();
-    if (failures) { std::printf("%d check(s) failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

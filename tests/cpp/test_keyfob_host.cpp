@@ -1,7 +1,7 @@
 // test_keyfob_host.cpp -- the keyfob slicer and Decoder through the C++ host layer (include/b200sdr.hpp) on a GPU: the
 // slicer's outputs, a level stream carrying "0110" + 10101111 + 11010101 decodes to one Close code at the flushing
 // edge, ragged execs agree with one exec, reset starts over, firdes::lowpass gives the keyfob's 128 taps, and the
-// refusals.  Built by __graft_entry__.build(); run by tests/test_gpu_keyfob_cpp_host.py (needs an H100).
+// refusals.  Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -9,13 +9,9 @@
 #include <string>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 // a bit b is appended by the edge ending a period at level b: a long period from level b, a short one first otherwise
 static std::vector<uint8_t> levels(const std::string &bits, size_t lead) {
@@ -83,7 +79,5 @@ int main() {
     }
     inst.sync();
     CHECK(b2s_ctx_bytes_held(inst.get()) == held);
-    if (failures) { std::printf("%d checks failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

@@ -1,18 +1,14 @@
 // test_sigsrc_host.cpp -- SignalSourceBuilder, SignalSource and Head (src/blocks/signal_source/mod.rs, head.rs) through
 // the C++ host layer (include/b200sdr.hpp) on a GPU.  The expected samples come from the host-side FixedPointPhase
 // (b2s_fxpt_phase_new / b2s_fxpt_sin_cos): phase k = phase0 + k inc (wrapping), sample = f(phase) * amplitude.
-// Built by __graft_entry__.build(); run by tests/test_gpu_sigsrc_cpp_host.py (needs an H100).
+// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cstdio>
 #include <cstring>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 static bool same_bits(const void *a, const void *b, size_t bytes) { return std::memcmp(a, b, bytes) == 0; }
 
@@ -88,7 +84,5 @@ int main() {
         CHECK(refused);
     }
     inst.sync();
-    if (failures) { std::printf("%d check(s) failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

@@ -1,19 +1,15 @@
 // test_stream_host.cpp -- Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver, firdes::hilbert and
 // windows::hamming through the C++ host layer (include/b200sdr.hpp) on a GPU, with the reference's own known answers
 // (tests/combine.rs, tests/split.rs, firdes/basic.rs:229-247) and small restated cases.
-// Built by __graft_entry__.build(); run by tests/test_gpu_stream_cpp_host.py (needs an H100).
+// Built by __graft_entry__.build(); run by tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 template <typename Block> static WorkIo run(Block &b) {
     WorkIo io;
@@ -121,7 +117,5 @@ int main() {
     }
     inst.sync();
     CHECK(b2s_ctx_bytes_held(inst.get()) == held);
-    if (failures) { std::printf("%d check(s) failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

@@ -2,20 +2,16 @@
 // GPU: with omega 1, mu 0 and no gains the clock recovery passes its input through; an out-of-slice step throws
 // B2S_ESTATE; a Mac-framed frame laid out as chips decodes to its bytes with a passing FCS, a flipped payload bit fails
 // it, ragged execs agree with one exec, reset starts over, and the refusals.  Built by __graft_entry__.build(); run by
-// tests/test_gpu_zigbee_cpp_host.py (needs an H100).
+// tests/test_gpu_cpp_host.py (needs an H100).
 #include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <limits>
 
 #include "b200sdr.hpp"
+#include "check.hpp"
 
 using namespace b2s;
-static int failures = 0;
-#define CHECK(cond)                                                                 \
-    do {                                                                            \
-        if (!(cond)) { std::printf("FAIL %s:%d  %s\n", __FILE__, __LINE__, #cond); failures++; } \
-    } while (0)
 
 static const uint32_t kChips[16] = {1618456172u, 1309113062u, 1826650030u, 1724778362u, 778887287u,  2061946375u,
                                     2007919840u, 125494990u,  529027475u,  838370585u,  320833617u,  422705285u,
@@ -123,7 +119,5 @@ int main() {
     }
     inst.sync();
     CHECK(b2s_ctx_bytes_held(inst.get()) == held);
-    if (failures) { std::printf("%d checks failed\n", failures); return 1; }
-    std::printf("all checks passed\n");
-    return 0;
+    return report();
 }

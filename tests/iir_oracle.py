@@ -1,44 +1,35 @@
 """CPU oracle of futuredsp::IirFilter (TEST INFRASTRUCTURE ONLY).
 
-ctypes front-end to ``tests/iir_oracle.c``, the C restatement of crates/futuredsp/src/iir.rs:78-178.  The library is
-compiled with the system gcc into a temporary directory on first use, so the repository tree may be read-only.
+ctypes front-end to ``tests/iir_oracle.c``, the C restatement of crates/futuredsp/src/iir.rs:78-178, compiled by
+``native.load_oracle`` on first use.
 Status codes follow ``futuredsp::ComputationStatus``: 0 InsufficientInput, 1 InsufficientOutput, 2 BothSufficient.
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "iir_oracle.c")
+from native import load_oracle
+
 _f32p = C.POINTER(C.c_float)
 _f64p = C.POINTER(C.c_double)
 _szp = C.POINTER(C.c_size_t)
-_lib = None
+
+
+def _work(p):
+    return C.c_int, [p, C.c_size_t, p, C.c_size_t, p, _szp, p, C.c_size_t, p, C.c_size_t, _szp, _szp]
+
+
+SIGNATURES = {
+    "orc_iir_work_f32": _work(_f32p),
+    "orc_iir_work_f64": _work(_f64p),
+    "orc_iir_exact_f32": (None, [_f32p, C.c_size_t, _f32p, C.c_size_t, _f32p, C.c_size_t, _f64p]),
+}
 
 
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="iir_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libiir_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so], check=True)
-        L = C.CDLL(so)
-        for name, p in (("orc_iir_work_f32", _f32p), ("orc_iir_work_f64", _f64p)):
-            fn = getattr(L, name)
-            fn.restype = C.c_int
-            fn.argtypes = [p, C.c_size_t, p, C.c_size_t, p, _szp, p, C.c_size_t, p, C.c_size_t, _szp, _szp]
-        L.orc_iir_exact_f32.restype = None
-        L.orc_iir_exact_f32.argtypes = [_f32p, C.c_size_t, _f32p, C.c_size_t, _f32p, C.c_size_t, _f64p]
-        _lib = L
-    return _lib
+    return load_oracle("iir_oracle", SIGNATURES)
 
 
 def _as(a, dt):

@@ -1,25 +1,20 @@
 """CPU oracle of the keyfob receiver's running average, slicer and Decoder (TEST INFRASTRUCTURE ONLY).
 
-ctypes front-end to ``tests/keyfob_oracle.c`` (one reference call at a time, compiled with the system gcc into a
-temporary directory on first use).  ``Avg`` and ``Decoder`` carry a block's state across calls; ``py_decode`` is an
-independent pure-Python transcription of decoder.rs for cross-checking the C file; ``code_tuple`` turns a device
-KEYFOB_CODE record into the oracle's tuple form.
+ctypes front-end to ``tests/keyfob_oracle.c`` (one reference call at a time, compiled by ``native.load_oracle`` on
+first use).  ``Avg`` and ``Decoder`` carry a block's state across calls; ``py_decode`` is an independent pure-Python
+transcription of decoder.rs for cross-checking the C file; ``code_tuple`` turns a device KEYFOB_CODE record into the
+oracle's tuple form.
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "keyfob_oracle.c")
+from native import load_oracle
+
 _f32p = C.POINTER(C.c_float)
 _u8p = C.POINTER(C.c_uint8)
-_lib = None
 
 LABELS = {"11010101": 1, "11100011": 2, "10111001": 3}          # Close, Open, Trunk
 
@@ -33,27 +28,17 @@ class Code(C.Structure):
     _fields_ = [("index", C.c_uint64), ("n_bits", C.c_uint32), ("label", C.c_int32), ("bits", C.c_uint8 * 32)]
 
 
+SIGNATURES = {
+    "orc_kf_avg": (None, [C.c_float, _f32p, _f32p, C.c_size_t, _f32p]),
+    "orc_kf_slice": (None, [_f32p, C.c_size_t, _u8p]),
+    "orc_kf_dec_new": (None, [C.POINTER(DecState)]),
+    "orc_kf_dec_free": (None, [C.POINTER(DecState)]),
+    "orc_kf_dec_work": (C.c_size_t, [C.POINTER(DecState), _u8p, C.c_size_t, C.POINTER(Code), C.c_size_t]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="keyfob_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libkeyfob_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so], check=True)
-        L = C.CDLL(so)
-        L.orc_kf_avg.restype = None
-        L.orc_kf_avg.argtypes = [C.c_float, _f32p, _f32p, C.c_size_t, _f32p]
-        L.orc_kf_slice.restype = None
-        L.orc_kf_slice.argtypes = [_f32p, C.c_size_t, _u8p]
-        L.orc_kf_dec_new.restype = None
-        L.orc_kf_dec_new.argtypes = [C.POINTER(DecState)]
-        L.orc_kf_dec_free.restype = None
-        L.orc_kf_dec_free.argtypes = [C.POINTER(DecState)]
-        L.orc_kf_dec_work.restype = C.c_size_t
-        L.orc_kf_dec_work.argtypes = [C.POINTER(DecState), _u8p, C.c_size_t, C.POINTER(Code), C.c_size_t]
-        _lib = L
-    return _lib
+    return load_oracle("keyfob_oracle", SIGNATURES)
 
 
 class Avg:

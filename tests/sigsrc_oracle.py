@@ -1,28 +1,23 @@
 """CPU oracle of blocks::SignalSource and FixedPointPhase (TEST INFRASTRUCTURE ONLY).
 
 ctypes front-end to ``tests/sigsrc_oracle.c``, the C restatement of src/blocks/signal_source/{mod,fxpt_nco,
-fxpt_phase}.rs, fed with the reference's sine table from ``tests/golden/reference_fxpt_sine_table.json``.  The library
-is compiled with the system gcc into a temporary directory on first use, so the repository tree may be read-only.
+fxpt_phase}.rs, fed with the reference's sine table from ``tests/golden/reference_fxpt_sine_table.json`` and compiled
+by ``native.load_oracle`` on first use.
 ``np_*`` is a second, independent transcription in numpy float32 that the CPU tests hold the C oracle to.
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
 import json
 import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "sigsrc_oracle.c")
-FIXTURE = os.path.join(_HERE, "golden", "reference_fxpt_sine_table.json")
+from native import load_oracle
+
+FIXTURE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_fxpt_sine_table.json")
 COS, SIN, SQUARE = 0, 1, 2
 _f32p = C.POINTER(C.c_float)
-_lib = None
 
 
 def table() -> np.ndarray:
@@ -34,27 +29,18 @@ def table() -> np.ndarray:
 TABLE = table()
 
 
+SIGNATURES = {
+    "orc_fxpt_phase_new": (C.c_int32, [C.c_float]),
+    "orc_sigsrc_inc": (C.c_int32, [C.c_float, C.c_float]),
+    "orc_fxpt_sin": (C.c_float, [_f32p, C.c_int32]),
+    "orc_fxpt_cos": (C.c_float, [_f32p, C.c_int32]),
+    "orc_sigsrc_work": (None, [_f32p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_int32, C.c_float, _f32p,
+                               C.c_size_t]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="sigsrc_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libsigsrc_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so, "-lm"], check=True)
-        L = C.CDLL(so)
-        L.orc_fxpt_phase_new.restype = C.c_int32
-        L.orc_fxpt_phase_new.argtypes = [C.c_float]
-        L.orc_sigsrc_inc.restype = C.c_int32
-        L.orc_sigsrc_inc.argtypes = [C.c_float, C.c_float]
-        for name in ("orc_fxpt_sin", "orc_fxpt_cos"):
-            getattr(L, name).restype = C.c_float
-            getattr(L, name).argtypes = [_f32p, C.c_int32]
-        L.orc_sigsrc_work.restype = None
-        L.orc_sigsrc_work.argtypes = [_f32p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.c_int32, C.c_float, _f32p,
-                                      C.c_size_t]
-        _lib = L
-    return _lib
+    return load_oracle("sigsrc_oracle", SIGNATURES)
 
 
 def _tp():

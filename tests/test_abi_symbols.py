@@ -66,39 +66,6 @@ def test_product_firdes_matches_oracle():
         assert a.size == b.size and np.array_equal(a, b)
 
 
-def test_struct_layouts_and_constants_match_the_header(tmp_path):
-    """The ctypes mirror of the ABI's one by-value struct (b2s_handshake) and of its constants must agree with what a C
-    compiler makes of include/b200sdr.h -- a Rust bindgen / cgo binding sees exactly these numbers."""
-    from futuresdr_b200 import _lib
-    probe = tmp_path / "probe.c"
-    probe.write_text('''#include <stdio.h>
-#include <stddef.h>
-#include "b200sdr.h"
-int main(void) {
-    printf("%zu %zu %zu %zu %zu %zu %zu\\n", sizeof(b2s_handshake), offsetof(b2s_handshake, publish_flag),
-           offsetof(b2s_handshake, publish_value), offsetof(b2s_handshake, wait_flag), offsetof(b2s_handshake, wait_value),
-           offsetof(b2s_handshake, done_flag), offsetof(b2s_handshake, done_value));
-    printf("%d %d %d %d %d %d %d %d\\n", B2S_OK, B2S_EINVAL, B2S_ECUDA, B2S_ENOMEM, B2S_EAGAIN, B2S_EUNSUPPORTED, B2S_ESTATE, B2S_ETIMEOUT);
-    printf("%d %d %d %d %d\\n", (int)B2S_F32_F32, (int)B2S_C32_F32, (int)B2S_C32_C32, (int)B2S_F64_F64, B2S_IPC_HANDLE_BYTES);
-    printf("%d %d %d %d\\n", (int)B2S_ALGO_AUTO, (int)B2S_ALGO_DIRECT, (int)B2S_ALGO_TENSOR, (int)B2S_ALGO_FFT);
-    return 0;
-}
-''')
-    exe = tmp_path / "probe"
-    r = subprocess.run(["/usr/bin/gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(probe), "-o", str(exe)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    lines = subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split("\n")
-    hs = _lib.Handshake
-    assert [int(v) for v in lines[0].split()] == [C.sizeof(hs), hs.publish_flag.offset, hs.publish_value.offset,
-                                                  hs.wait_flag.offset, hs.wait_value.offset, hs.done_flag.offset,
-                                                  hs.done_value.offset]
-    assert [int(v) for v in lines[1].split()] == [_lib.OK, _lib.EINVAL, _lib.ECUDA, _lib.ENOMEM, _lib.EAGAIN,
-                                                  _lib.EUNSUPPORTED, _lib.ESTATE, _lib.ETIMEOUT]
-    assert [int(v) for v in lines[2].split()] == [_lib.F32_F32, _lib.C32_F32, _lib.C32_C32, _lib.F64_F64, 64]
-    assert [int(v) for v in lines[3].split()] == [_lib.ALGO_AUTO, _lib.ALGO_DIRECT, _lib.ALGO_TENSOR, _lib.ALGO_FFT]
-
-
 def test_numa_helpers_without_a_gpu():
     """futuresdr_b200.numa: cpulist parsing, and binding degrades gracefully (no NVML here) and restores the CPU set."""
     from futuresdr_b200 import numa

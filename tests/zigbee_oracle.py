@@ -1,28 +1,23 @@
 """CPU oracle of the ZigBee receiver's DC blocker, ClockRecoveryMm, Decoder and Mac::calc_crc (TEST INFRASTRUCTURE ONLY).
 
-ctypes front-end to ``tests/zigbee_oracle.c`` (one reference call at a time, compiled with the system gcc into a
-temporary directory on first use).  ``DcBlock``, ``Mm`` and ``Decoder`` carry a block's state across calls;
-``np_*`` are an independent numpy float32 transcription for cross-checking the C file, and ``crc16_table`` a
-table-driven CRC for cross-checking ``calc_crc``.
+ctypes front-end to ``tests/zigbee_oracle.c`` (one reference call at a time, compiled by ``native.load_oracle`` on
+first use).  ``DcBlock``, ``Mm`` and ``Decoder`` carry a block's state across calls; ``np_*`` are an independent
+numpy float32 transcription for cross-checking the C file, and ``crc16_table`` a table-driven CRC for cross-checking
+``calc_crc``.
 """
 from __future__ import annotations
 
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
-_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "zigbee_oracle.c")
+from native import load_oracle
+
 _f32p = C.POINTER(C.c_float)
 _u64p = C.POINTER(C.c_uint64)
 _u32p = C.POINTER(C.c_uint32)
 _u8p = C.POINTER(C.c_uint8)
 _szp = C.POINTER(C.c_size_t)
-_lib = None
 
 CHIP_MAPPING = np.array([1618456172, 1309113062, 1826650030, 1724778362, 778887287, 2061946375, 2007919840,
                          125494990, 529027475, 838370585, 320833617, 422705285, 1368596360, 85537272, 139563807,
@@ -42,30 +37,19 @@ class DecState(C.Structure):
                 ("data", C.c_uint8 * 128)]
 
 
+SIGNATURES = {
+    "orc_zb_dc_block": (None, [C.c_float, _f32p, _f32p, C.c_size_t, _f32p]),
+    "orc_zb_mm_new": (None, [C.POINTER(MmState)] + [C.c_float] * 5),
+    "orc_zb_mm_work": (C.c_int, [C.POINTER(MmState), _f32p, C.c_size_t, _f32p, C.c_size_t, _szp, _szp]),
+    "orc_zb_decoder_new": (None, [C.POINTER(DecState), C.c_uint32]),
+    "orc_zb_decoder_work": (C.c_size_t, [C.POINTER(DecState), _f32p, C.c_size_t, C.c_uint64, _u64p, _u32p, _u8p,
+                                         C.c_size_t]),
+    "orc_zb_calc_crc": (C.c_uint32, [_u8p, C.c_size_t]),
+}
+
+
 def lib() -> C.CDLL:
-    global _lib
-    if _lib is None:
-        tmp = tempfile.mkdtemp(prefix="zigbee_oracle_")
-        atexit.register(shutil.rmtree, tmp, True)
-        so = os.path.join(tmp, "libzigbee_oracle.so")
-        subprocess.run(["/usr/bin/gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", _SRC,
-                        "-o", so], check=True)
-        L = C.CDLL(so)
-        L.orc_zb_dc_block.restype = None
-        L.orc_zb_dc_block.argtypes = [C.c_float, _f32p, _f32p, C.c_size_t, _f32p]
-        L.orc_zb_mm_new.restype = None
-        L.orc_zb_mm_new.argtypes = [C.POINTER(MmState)] + [C.c_float] * 5
-        L.orc_zb_mm_work.restype = C.c_int
-        L.orc_zb_mm_work.argtypes = [C.POINTER(MmState), _f32p, C.c_size_t, _f32p, C.c_size_t, _szp, _szp]
-        L.orc_zb_decoder_new.restype = None
-        L.orc_zb_decoder_new.argtypes = [C.POINTER(DecState), C.c_uint32]
-        L.orc_zb_decoder_work.restype = C.c_size_t
-        L.orc_zb_decoder_work.argtypes = [C.POINTER(DecState), _f32p, C.c_size_t, C.c_uint64, _u64p, _u32p, _u8p,
-                                          C.c_size_t]
-        L.orc_zb_calc_crc.restype = C.c_uint32
-        L.orc_zb_calc_crc.argtypes = [_u8p, C.c_size_t]
-        _lib = L
-    return _lib
+    return load_oracle("zigbee_oracle", SIGNATURES)
 
 
 def _f(a):
