@@ -6,7 +6,7 @@ reference's Rust API for this path (futuredsp::{FirFilter, DecimatingFirFilter,
 PolyphaseResamplingFir}, futuredsp::{firdes::{hilbert, lowpass}, windows::hamming}, futuresdr::blocks::{Fir,
 FirBuilder, Fft, Apply, PfbArbResampler, SignalSource, SignalSourceBuilder, FixedPointPhase, Head,
 Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver}, the WLAN / M17 receivers' MovingAverage, the ZigBee
-receiver's ClockRecoveryMm and Decoder, the keyfob receiver's Decoder,
+receiver's ClockRecoveryMm and Decoder, the keyfob receiver's Decoder, ApplyNM and the SSB example's oscillator mixers,
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -22,7 +22,7 @@ from .filters import (  # noqa: F401
 from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
     Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator, MovingAverage,
-    AdsbDemod, ClockRecoveryMm, ZigbeeDecoder, KeyfobDecoder, KEYFOB_CODE,
+    AdsbDemod, ClockRecoveryMm, ZigbeeDecoder, KeyfobDecoder, KEYFOB_CODE, ApplyNM, ApplyNMOp, Mixer, MixOp,
 )
-from . import adsb, firdes, keyfob, windows, zigbee  # noqa: F401
+from . import adsb, firdes, keyfob, ssb, windows, zigbee  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

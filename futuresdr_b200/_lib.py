@@ -18,7 +18,8 @@ INSUFFICIENT_INPUT, INSUFFICIENT_OUTPUT, BOTH_SUFFICIENT = 0, 1, 2
 F32_F32, C32_F32, C32_C32, F64_F64 = 0, 1, 2, 3
 ALGO_AUTO, ALGO_DIRECT, ALGO_TENSOR, ALGO_FFT, ALGO_SCAN = 0, 1, 2, 3, 4
 (OP_SCALE_F32, OP_SCALE_C32, OP_QUAD_DEMOD, OP_NORM_SQR, OP_QUAD_DEMOD_C32, OP_EXP_F32,
- OP_MAG_C32, OP_LOG10_F32, OP_DC_BLOCK_F32, OP_SLICE_F32_U8) = range(10)
+ OP_MAG_C32, OP_LOG10_F32, OP_DC_BLOCK_F32, OP_SLICE_F32_U8, OP_DIV_C32, OP_C32_TO_I16_IQ) = range(12)
+MIX_ROTATE_C32, MIX_ROTATE_SCALE_C32, MIX_WEAVER_F32 = 0, 1, 2
 KEYFOB_NONE, KEYFOB_CLOSE, KEYFOB_OPEN, KEYFOB_TRUNK = 0, 1, 2, 3
 WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
 (COMBINE_ADD_F32, COMBINE_SUB_F32, COMBINE_MUL_F32, COMBINE_CONJ_MUL_C32, COMBINE_MAG_DIV_C32_F32, COMBINE_TO_C32,
@@ -81,6 +82,10 @@ SIGNATURES = {
     "b2s_rotator_reset": (_i32, [_vp]),
     "b2s_rotator_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _i32p]),
     "b2s_xlating_taps": (_i32, [_f32p, _sz, _f32, _f32, _sz, _f32p, _f32p]),
+    "b2s_mixer_create": (_i32, [_vp, C.c_int, _f32, _f32, _vpp]),
+    "b2s_mixer_destroy": (None, [_vp]),
+    "b2s_mixer_reset": (_i32, [_vp]),
+    "b2s_mixer_exec": (_i32, [_vp, _vp, _sz, _vp, _sz, _szp, _szp]),
     "b2s_chan_plan_c32": (_i32, [_vp, _sz, _f32p, _sz, _f32, _vpp]),
     "b2s_chan_destroy": (None, [_vp]),
     "b2s_chan_decimation": (_sz, [_vp]),

@@ -7,6 +7,9 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
   * ``Head``                      src/blocks/head.rs:22-84
   * ``Fft`` / ``FftDirection``    src/blocks/fft.rs:30-221
   * ``Apply``                     src/blocks/apply.rs:100-131 (closed catalogue of closures)
+  * ``ApplyNM``                   src/blocks/applynm.rs:92-121 (closed catalogue of closures)
+  * ``Mixer``                     Apply over the SSB example's oscillator closures (examples/ssb); helpers in
+                                  futuresdr_b200.ssb
   * ``PfbArbResampler``           src/blocks/pfb/arb_resampler.rs:72-231
   * ``Combine`` / ``Split``       src/blocks/combine.rs:31-137, split.rs:31-127 (closed catalogues of closures)
   * ``Delay``                     src/blocks/delay.rs:31-169
@@ -52,7 +55,7 @@ class WorkIo:
 
 def _tdtype(np_dtype):
     return {np.dtype(np.complex64): torch.complex64, np.dtype(np.float64): torch.float64,
-            np.dtype(np.uint8): torch.uint8}.get(np.dtype(np_dtype), torch.float32)
+            np.dtype(np.uint8): torch.uint8, np.dtype(np.int16): torch.int16}.get(np.dtype(np_dtype), torch.float32)
 
 
 def _ctx_device(ctx) -> torch.device:
@@ -430,6 +433,7 @@ class ApplyOp(enum.IntEnum):
     Log10F32 = _lib.OP_LOG10_F32
     DcBlockF32 = _lib.OP_DC_BLOCK_F32      # param = alpha: s = (1 - alpha) * s + alpha * x; y = x - s
     SliceF32U8 = _lib.OP_SLICE_F32_U8      # f32 -> u8: x > 0 ? 1 : 0 (the keyfob receiver's slicer)
+    DivC32 = _lib.OP_DIV_C32               # c32 -> c32: x / param per part (the SSB transmitter's file level)
 
 
 _APPLY_TYPES = {
@@ -438,6 +442,7 @@ _APPLY_TYPES = {
     ApplyOp.QuadDemodC32: (np.complex64, np.complex64), ApplyOp.ExpF32: (np.float32, np.float32),
     ApplyOp.MagC32: (np.complex64, np.float32), ApplyOp.Log10F32: (np.float32, np.float32),
     ApplyOp.DcBlockF32: (np.float32, np.float32), ApplyOp.SliceF32U8: (np.float32, np.uint8),
+    ApplyOp.DivC32: (np.complex64, np.complex64),
 }
 
 
@@ -472,6 +477,46 @@ class Apply(Block, Handle):
             self.input.consume(m)
             self.output.produce(m)
         if self.input.finished() and m == i_len:                                 # apply.rs:126-128
+            io.finished = True
+
+
+class ApplyNMOp(enum.IntEnum):
+    """The ApplyNM closures that exist as device ops (b2s_op)."""
+    C32ToI16Iq = _lib.OP_C32_TO_I16_IQ     # c32 -> 2 x i16: (re * param * 32767.0) as i16, then im (ssb transmit)
+
+
+_APPLYNM_TYPES = {ApplyNMOp.C32ToI16Iq: (np.complex64, np.int16, 1, 2)}     # (in, out, N, M)
+
+
+class ApplyNM(Block, Handle):
+    """blocks::ApplyNM<_, A, B, N, M> (src/blocks/applynm.rs:92-121) for the closures of ApplyNMOp: N input items become
+    M output items.  Rust's ``as i16`` truncates toward zero, saturates and maps NaN to 0, and so does the device."""
+    _destroy = lib.b2s_apply_destroy
+
+    def __init__(self, op: ApplyNMOp, param: float = 1.0, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.op = ApplyNMOp(op)
+        self.in_dtype, self.out_dtype, self.n, self.m = _APPLYNM_TYPES[self.op]
+        self._h = C.c_void_p()
+        check(lib.b2s_apply_create(self.ctx.handle, int(self.op), float(param), C.byref(self._h)), self.ctx.handle)
+        self._ports()
+
+    def apply(self, i: torch.Tensor, o: torch.Tensor) -> tuple[int, int]:
+        """The closure over device slices (asynchronous) -> (consumed, produced)."""
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_apply_exec(self._h, _ptr(i), i.numel(), _ptr(o), o.numel(), C.byref(c), C.byref(p)),
+              self.ctx.handle)
+        return c.value, p.value
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()
+        i_len = i.numel()
+        m = min(i_len // self.n, o.numel() // self.m)                           # applynm.rs:109
+        if m > 0:
+            self.apply(i[:self.n * m], o[:self.m * m])
+            self.input.consume(self.n * m)
+            self.output.produce(self.m * m)
+        if self.input.finished() and i_len - self.n * m < self.n:               # applynm.rs:118-120
             io.finished = True
 
 
@@ -533,6 +578,52 @@ class Rotator(Handle):
 
     def reset(self):
         check(lib.b2s_rotator_reset(self._h), self.ctx.handle)
+
+
+class MixOp(enum.IntEnum):
+    """The SSB example's oscillator closures, ``osc *= shift; f(v, osc)`` (b2s_mix_op)."""
+    RotateC32 = _lib.MIX_ROTATE_C32             # v * osc                                  (transmit.rs:102-107)
+    RotateScaleC32 = _lib.MIX_ROTATE_SCALE_C32  # v * osc * param                          (receive.rs:58-66)
+    WeaverF32 = _lib.MIX_WEAVER_F32             # param * (v.re*osc.re + v.im*osc.im), f32 (receive.rs:73-83)
+
+
+class Mixer(Block, Handle):
+    """blocks::Apply over one oscillator closure of MixOp, with shift = Complex32::from_polar(1.0, phase_incr): the
+    Rotator's recurrence replayed bit for bit (csrc/rotator.cu), so the output is the reference closure's under any
+    slicing.  Work and finish rules are Apply's (apply.rs:100-131)."""
+    _destroy = lib.b2s_mixer_destroy
+    in_dtype = np.complex64
+
+    def __init__(self, op: MixOp, phase_incr: float, param: float = 1.0, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.op = MixOp(op)
+        self.out_dtype = np.float32 if self.op == MixOp.WeaverF32 else np.complex64
+        self._h = C.c_void_p()
+        check(lib.b2s_mixer_create(self.ctx.handle, int(self.op), float(np.float32(phase_incr)), float(np.float32(param)),
+                                   C.byref(self._h)), self.ctx.handle)
+        self._ports()
+
+    def mix(self, i: torch.Tensor, o: torch.Tensor) -> int:
+        """The closure over min(len) items of device slices (asynchronous); returns that count."""
+        c, p = C.c_size_t(0), C.c_size_t(0)
+        check(lib.b2s_mixer_exec(self._h, _ptr(i), i.numel(), _ptr(o), o.numel(), C.byref(c), C.byref(p)),
+              self.ctx.handle)
+        return c.value
+
+    def reset(self):
+        """osc back to 1 + 0i."""
+        check(lib.b2s_mixer_reset(self._h), self.ctx.handle)
+
+    def work(self, io: WorkIo):
+        i, o = self.input.slice(), self.output.slice()
+        i_len = i.numel()
+        m = min(i_len, o.numel())                                               # apply.rs:109
+        if m > 0:
+            self.mix(i, o)
+            self.input.consume(m)
+            self.output.produce(m)
+        if self.input.finished() and m == i_len:                                 # apply.rs:126-128
+            io.finished = True
 
 
 class XlatingFir(Block):

@@ -7,7 +7,8 @@
 // (examples/fm-receiver/src/main.rs:99-104) is the previous input item, so item j reads
 // in[j-1] and item 0 reads the carried sample; after the launch the carry is refreshed from
 // in[m-1] on the same stream.  The DC blocker's running average is carry.x, read and written by its kernel.  The
-// keyfob slicer is the one op with a u8 output.
+// keyfob slicer is the one op with a u8 output, and the SSB transmitter's i16 converter the one that writes two output
+// items per input item (ApplyNM<1, 2>, src/blocks/applynm.rs:100-121).
 #include <cmath>
 
 #include "chunks.cuh"
@@ -83,6 +84,9 @@ __global__ void apply_kernel(const void *__restrict__ vin, void *__restrict__ vo
             ((float *)vout)[j] = hypotf(v.x, v.y);                                         // Complex::norm
         } else if constexpr (OP == B2S_OP_LOG10_F32) {
             ((float *)vout)[j] = param * log10f(((const float *)vin)[j]);
+        } else if constexpr (OP == B2S_OP_DIV_C32) {
+            const float2 v = ((const float2 *)vin)[j];
+            ((float2 *)vout)[j] = make_float2(__fdiv_rn(v.x, param), __fdiv_rn(v.y, param));   // Complex / f32
         }
     }
 }
@@ -152,8 +156,35 @@ slice_kernel(const float *__restrict__ in, unsigned char *__restrict__ out, unsi
                [&](unsigned long long i) { out[i] = slice_one(__ldg(in + i)); });
 }
 
+// B2S_OP_C32_TO_I16_IQ: (x * param * 32767.0) as i16 per part (examples/ssb/transmit.rs:109-112).  cvt.rzi.s16.f32
+// is Rust's `as i16`: it truncates toward zero, clamps to the i16 range and turns NaN into 0.  The pair is one 32-bit
+// store when the output is 4-byte aligned, two 16-bit stores otherwise.
+__device__ __forceinline__ short to_i16(float x, float param) {
+    const float y = __fmul_rn(__fmul_rn(x, param), 32767.0f);
+    short r;
+    asm("cvt.rzi.s16.f32 %0, %1;" : "=h"(r) : "f"(y));
+    return r;
+}
+__global__ void __launch_bounds__(kThreads)
+to_i16_iq_kernel(const float2 *__restrict__ in, short *__restrict__ out, long long n, float param, bool pair32) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
+        const float2 v = in[j];
+        const short re = to_i16(v.x, param), im = to_i16(v.y, param);
+        if (pair32) reinterpret_cast<unsigned *>(out)[j] = (unsigned)(unsigned short)re | (unsigned)(unsigned short)im << 16;
+        else { out[2 * j] = re; out[2 * j + 1] = im; }
+    }
+}
+
 template <int OP>
 int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
+    if constexpr (OP == B2S_OP_C32_TO_I16_IQ) {
+        b2s_ctx *ctx = a->ctx;
+        to_i16_iq_kernel<<<grid_for(ctx, n, 16), kThreads, 0, ctx->stream>>>(
+            (const float2 *)in, (short *)out, (long long)n, a->param, ((uintptr_t)out & 3) == 0);
+        B2S_CHECK_LAUNCH(ctx);
+        return B2S_OK;
+    }
     if constexpr (OP == B2S_OP_SLICE_F32_U8) {
         b2s_ctx *ctx = a->ctx;
         const unsigned head = (unsigned)std::min<size_t>(n, (4 - ((uintptr_t)out & 3)) & 3);
@@ -181,7 +212,7 @@ int32_t launch(b2s_apply *a, const void *in, void *out, size_t n) {
 
 bool in_is_complex(b2s_op op) {
     return op == B2S_OP_SCALE_C32 || op == B2S_OP_QUAD_DEMOD || op == B2S_OP_NORM_SQR ||
-           op == B2S_OP_QUAD_DEMOD_C32 || op == B2S_OP_MAG_C32;
+           op == B2S_OP_QUAD_DEMOD_C32 || op == B2S_OP_MAG_C32 || op == B2S_OP_DIV_C32 || op == B2S_OP_C32_TO_I16_IQ;
 }
 
 }  // namespace
@@ -191,7 +222,7 @@ extern "C" {
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out) {
     if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: NULL argument");
     *out = nullptr;
-    if ((int)op < 0 || (int)op > (int)B2S_OP_SLICE_F32_U8) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
+    if ((int)op < 0 || (int)op > (int)B2S_OP_C32_TO_I16_IQ) return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: bad op %d", (int)op);
     if (op == B2S_OP_DC_BLOCK_F32 && !std::isfinite(param))
         return b2s_fail(ctx, B2S_EINVAL, "b2s_apply_create: DC blocker alpha %g (a finite value)", (double)param);
     DeviceGuard g(ctx->device);
@@ -216,8 +247,10 @@ int32_t b2s_apply_reset(b2s_apply *a) {
 int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
                        size_t *consumed, size_t *produced) {
     if (!a || !consumed || !produced) return b2s_fail(a ? a->ctx : nullptr, B2S_EINVAL, "b2s_apply_exec: NULL argument");
-    const size_t m = n_in < n_out_cap ? n_in : n_out_cap;        // apply.rs:109
-    *consumed = m; *produced = m;
+    const bool iq = a->op == B2S_OP_C32_TO_I16_IQ;                // two i16 items out per c32 item in
+    const size_t out_items = iq ? n_out_cap / 2 : n_out_cap;
+    const size_t m = n_in < out_items ? n_in : out_items;         // apply.rs:109, applynm.rs:109
+    *consumed = m; *produced = iq ? 2 * m : m;
     if (m == 0) return B2S_OK;
     if (!d_in || !d_out) return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: NULL buffer");
     // the demodulators read in[j-1] while a neighbour thread writes out[j-1]: the slices must not overlap
@@ -232,6 +265,13 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
         if (!word_aligned(d_in)) return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the slicer's input is not 4-byte aligned");
         if (overlap(d_in, m * sizeof(float), d_out, m))
             return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the slicer cannot run in place (input and output overlap)");
+    }
+    if (iq) {
+        if (((uintptr_t)d_in & 7) || ((uintptr_t)d_out & 1))
+            return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the i16 converter needs an 8-byte aligned input and a "
+                                                "2-byte aligned output");
+        if (overlap(d_in, m * sizeof(float2), d_out, m * 2 * sizeof(short)))
+            return b2s_fail(a->ctx, B2S_EINVAL, "b2s_apply_exec: the i16 converter cannot run in place (input and output overlap)");
     }
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {
         if (overlap(d_in, m * sizeof(float2), d_out, m * (a->op == B2S_OP_QUAD_DEMOD ? sizeof(float) : sizeof(float2))))
@@ -251,6 +291,8 @@ int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out,
         case B2S_OP_LOG10_F32: rc = launch<B2S_OP_LOG10_F32>(a, d_in, d_out, m); break;
         case B2S_OP_DC_BLOCK_F32: rc = launch<B2S_OP_DC_BLOCK_F32>(a, d_in, d_out, m); break;
         case B2S_OP_SLICE_F32_U8: rc = launch<B2S_OP_SLICE_F32_U8>(a, d_in, d_out, m); break;
+        case B2S_OP_DIV_C32: rc = launch<B2S_OP_DIV_C32>(a, d_in, d_out, m); break;
+        case B2S_OP_C32_TO_I16_IQ: rc = launch<B2S_OP_C32_TO_I16_IQ>(a, d_in, d_out, m); break;
     }
     if (rc != B2S_OK) return rc;
     if (a->op == B2S_OP_QUAD_DEMOD || a->op == B2S_OP_QUAD_DEMOD_C32) {

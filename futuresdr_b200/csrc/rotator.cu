@@ -1,5 +1,6 @@
-// rotator.cu -- futuredsp::Rotator (crates/futuredsp/src/rotator.rs:13-48) and the band-pass tap
-// construction of XlatingFir (src/blocks/xlating_fir.rs:72-103) -- SURVEY.md §8f row 1.
+// rotator.cu -- futuredsp::Rotator (crates/futuredsp/src/rotator.rs:13-48), the band-pass tap
+// construction of XlatingFir (src/blocks/xlating_fir.rs:72-103) -- SURVEY.md §8f row 1 -- and the SSB example's
+// oscillator closures (examples/ssb/{transmit,receive}.rs), which run the same recurrence (b2s_mixer, DESIGN §4.18).
 //
 // The reference rotator is an f32 product recurrence with NO renormalisation:
 //     phase *= phase_incr;  out = in * phase          (per sample, num_complex Mul)
@@ -56,6 +57,14 @@ struct b2s_rotator {
     }
 };
 
+// The SSB example's oscillator closures (b2s_mix_op): the same replay, a different epilogue per sample.
+struct b2s_mixer {
+    b2s_ctx *ctx = nullptr;
+    b2s_mix_op op = B2S_MIX_ROTATE_C32;
+    float param = 1.f;
+    b2s_rotator rot;
+};
+
 namespace {
 
 void rotator_worker(b2s_rotator *r) {
@@ -93,9 +102,31 @@ __device__ __forceinline__ float2 cmul_rn(float2 a, float2 b) {       // num_com
                        __fadd_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)));
 }
 
+// What a sample becomes once its phase is known: the closures `osc *= shift; f(v, osc)` differ only in f.
+struct EpiRotate {                                                     // v * osc (rotator.rs:45, transmit.rs:104-107)
+    using Out = float2;
+    __device__ __forceinline__ float2 operator()(float2 v, float2 p) const { return cmul_rn(v, p); }
+};
+struct EpiRotateScale {                                                // v * osc * s, Complex * f32 per part (receive.rs:63-66)
+    using Out = float2;
+    float s;
+    __device__ __forceinline__ float2 operator()(float2 v, float2 p) const {
+        const float2 t = cmul_rn(v, p);
+        return make_float2(__fmul_rn(t.x, s), __fmul_rn(t.y, s));
+    }
+};
+struct EpiWeaver {                                                     // s * (v.re*osc.re + v.im*osc.im) (receive.rs:78-83)
+    using Out = float;
+    float s;
+    __device__ __forceinline__ float operator()(float2 v, float2 p) const {
+        return __fmul_rn(s, __fadd_rn(__fmul_rn(v.x, p.x), __fmul_rn(v.y, p.y)));
+    }
+};
+
 // sample s of the call is sample (off + s) of the record span: record (off + s) / 8, then (off + s) % 8 + 1 steps
-__global__ void rotator_kernel(const float2 *__restrict__ in, float2 *__restrict__ out,
-                               const float2 *__restrict__ recs, float2 incr, long long n, int off) {
+template <class Epi>
+__global__ void rotator_kernel(const float2 *__restrict__ in, typename Epi::Out *__restrict__ out,
+                               const float2 *__restrict__ recs, float2 incr, long long n, int off, Epi epi) {
     const long long stride = (long long)gridDim.x * blockDim.x;
     for (long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x; s < n; s += stride) {
         const long long a = s + off;
@@ -104,37 +135,22 @@ __global__ void rotator_kernel(const float2 *__restrict__ in, float2 *__restrict
 #pragma unroll
         for (int i = 0; i < kRotSub; i++)
             if (i <= j) p = cmul_rn(p, incr);                          // phase *= phase_incr, (j+1) times
-        out[s] = cmul_rn(in[s], p);                                    // *v *= phase
+        out[s] = epi(in[s], p);
     }
 }
 
-}  // namespace
-
-extern "C" {
-
-int32_t b2s_rotator_create(b2s_ctx *ctx, float phase_incr, b2s_rotator **out) {
-    if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_rotator_create: NULL argument");
-    *out = nullptr;
-    DeviceGuard g(ctx->device);
-    PlanPtr<b2s_rotator> r(new b2s_rotator());
+int32_t replay_init(b2s_rotator *r, b2s_ctx *ctx, float phase_incr) {
     r->ctx = ctx;
     // Complex32::from_polar(1.0, phase_incr) = (1.0 * cos, 1.0 * sin) in f32 (rotator.rs:17)
     r->incr[0] = 1.0f * std::cos(phase_incr);
     r->incr[1] = 1.0f * std::sin(phase_incr);
     B2S_TRY(r->h_ring.alloc(ctx, kRingRecs, "rotator: pinned record ring"));
     for (int i = 0; i < 2; i++) B2S_CUDA(ctx, cudaEventCreateWithFlags(&r->ev[i], cudaEventDisableTiming));
-    r->worker = std::thread(rotator_worker, r.get());
-    *out = r.release();
+    r->worker = std::thread(rotator_worker, r);
     return B2S_OK;
 }
 
-void b2s_rotator_destroy(b2s_rotator *r) {
-    if (r) r->stop_worker();
-    PlanDeleter<b2s_rotator>()(r);
-}
-
-int32_t b2s_rotator_reset(b2s_rotator *r) {
-    if (!r) return b2s_fail(nullptr, B2S_EINVAL, "rotator is NULL");
+int32_t replay_reset(b2s_rotator *r) {
     DeviceGuard g(r->ctx->device);
     // copies of the old sequence may still be reading the ring
     B2S_CUDA(r->ctx, cudaStreamSynchronize(r->ctx->stream));
@@ -144,20 +160,11 @@ int32_t b2s_rotator_reset(b2s_rotator *r) {
     return B2S_OK;
 }
 
-// ≙ Rotator::rotate (rotator.rs:32-47); d_in == d_out is rotate_inplace (:24-29)
-int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
-                         size_t *processed, int32_t *status) {
-    if (!r || !processed || !status) return b2s_fail(r ? r->ctx : nullptr, B2S_EINVAL, "b2s_rotator_exec: NULL argument");
+// n > 0 samples of the stream through `epi`, each with the phase the recurrence gives it
+template <class Epi>
+int32_t replay_exec(b2s_rotator *r, const float2 *in, typename Epi::Out *out, size_t n, Epi epi) {
     b2s_ctx *ctx = r->ctx;
-    size_t n;
-    if (n_in > n_out_cap) { n = n_out_cap; *status = B2S_INSUFFICIENT_OUTPUT; }
-    else if (n_in == n_out_cap) { n = n_out_cap; *status = B2S_BOTH_SUFFICIENT; }
-    else { n = n_in; *status = B2S_INSUFFICIENT_INPUT; }
-    *processed = n;
-    if (n == 0) return B2S_OK;
-    if (!d_in || !d_out) return b2s_fail(ctx, B2S_EINVAL, "b2s_rotator_exec: NULL buffer");
     DeviceGuard g(ctx->device);
-    NvtxRange nvtx("b2s_rotator_exec");
     // pieces of at most a quarter of the ring, so that the worker can keep running ahead while a piece is in flight
     const size_t piece_max = (kRingRecs / 4) * kRotSub;
     const size_t d_need = std::min(n, piece_max) / kRotSub + 2;
@@ -200,13 +207,101 @@ int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_
             B2S_CUDA(ctx, cudaMemcpyAsync(drec + first, r->h_ring.get(), (cnt - first) * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
         B2S_CUDA(ctx, cudaEventRecord(r->ev[h], ctx->stream));
         r->span_end[h] = rec0;                                      // records below rec0 are never needed again
-        rotator_kernel<<<grid_for(ctx, m, 16), kThreads, 0, ctx->stream>>>(
-            (const float2 *)d_in + done, (float2 *)d_out + done, drec, make_float2(r->incr[0], r->incr[1]), (long long)m,
-            (int)(a0 % kRotSub));
+        rotator_kernel<Epi><<<grid_for(ctx, m, 16), kThreads, 0, ctx->stream>>>(
+            in + done, out + done, drec, make_float2(r->incr[0], r->incr[1]), (long long)m, (int)(a0 % kRotSub), epi);
         B2S_CHECK_LAUNCH(ctx);
         r->pos = a1; r->half ^= 1; done += m;
     }
     return B2S_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int32_t b2s_rotator_create(b2s_ctx *ctx, float phase_incr, b2s_rotator **out) {
+    if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_rotator_create: NULL argument");
+    *out = nullptr;
+    DeviceGuard g(ctx->device);
+    PlanPtr<b2s_rotator> r(new b2s_rotator());
+    B2S_TRY(replay_init(r.get(), ctx, phase_incr));
+    *out = r.release();
+    return B2S_OK;
+}
+
+void b2s_rotator_destroy(b2s_rotator *r) {
+    if (r) r->stop_worker();
+    PlanDeleter<b2s_rotator>()(r);
+}
+
+int32_t b2s_rotator_reset(b2s_rotator *r) {
+    if (!r) return b2s_fail(nullptr, B2S_EINVAL, "rotator is NULL");
+    return replay_reset(r);
+}
+
+// ≙ Rotator::rotate (rotator.rs:32-47); d_in == d_out is rotate_inplace (:24-29)
+int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
+                         size_t *processed, int32_t *status) {
+    if (!r || !processed || !status) return b2s_fail(r ? r->ctx : nullptr, B2S_EINVAL, "b2s_rotator_exec: NULL argument");
+    size_t n;
+    if (n_in > n_out_cap) { n = n_out_cap; *status = B2S_INSUFFICIENT_OUTPUT; }
+    else if (n_in == n_out_cap) { n = n_out_cap; *status = B2S_BOTH_SUFFICIENT; }
+    else { n = n_in; *status = B2S_INSUFFICIENT_INPUT; }
+    *processed = n;
+    if (n == 0) return B2S_OK;
+    if (!d_in || !d_out) return b2s_fail(r->ctx, B2S_EINVAL, "b2s_rotator_exec: NULL buffer");
+    NvtxRange nvtx("b2s_rotator_exec");
+    return replay_exec(r, (const float2 *)d_in, (float2 *)d_out, n, EpiRotate{});
+}
+
+int32_t b2s_mixer_create(b2s_ctx *ctx, b2s_mix_op op, float phase_incr, float param, b2s_mixer **out) {
+    if (!ctx || !out) return b2s_fail(ctx, B2S_EINVAL, "b2s_mixer_create: NULL argument");
+    *out = nullptr;
+    if ((int)op < 0 || (int)op > (int)B2S_MIX_WEAVER_F32) return b2s_fail(ctx, B2S_EINVAL, "b2s_mixer_create: bad op %d", (int)op);
+    DeviceGuard g(ctx->device);
+    PlanPtr<b2s_mixer> m(new b2s_mixer());
+    m->ctx = ctx; m->op = op; m->param = param;
+    B2S_TRY(replay_init(&m->rot, ctx, phase_incr));
+    *out = m.release();
+    return B2S_OK;
+}
+
+void b2s_mixer_destroy(b2s_mixer *m) {
+    if (m) m->rot.stop_worker();
+    PlanDeleter<b2s_mixer>()(m);
+}
+
+// `let mut osc = Complex32::new(1.0, 0.0)` (receive.rs:58, :73; transmit.rs:101)
+int32_t b2s_mixer_reset(b2s_mixer *m) {
+    if (!m) return b2s_fail(nullptr, B2S_EINVAL, "mixer is NULL");
+    return replay_reset(&m->rot);
+}
+
+// ≙ Apply::work (apply.rs:100-131) over one of the closures: m = min(n_in, n_out_cap) samples (:109)
+int32_t b2s_mixer_exec(b2s_mixer *m, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
+                       size_t *consumed, size_t *produced) {
+    if (!m || !consumed || !produced) return b2s_fail(m ? m->ctx : nullptr, B2S_EINVAL, "b2s_mixer_exec: NULL argument");
+    const size_t n = std::min(n_in, n_out_cap);
+    *consumed = n; *produced = n;
+    if (n == 0) return B2S_OK;
+    if (!d_in || !d_out) return b2s_fail(m->ctx, B2S_EINVAL, "b2s_mixer_exec: NULL buffer");
+    const bool weaver = m->op == B2S_MIX_WEAVER_F32;
+    const size_t ob = weaver ? sizeof(float) : sizeof(float2);
+    if (((uintptr_t)d_in & 7) || ((uintptr_t)d_out & (ob - 1)))
+        return b2s_fail(m->ctx, B2S_EINVAL, "b2s_mixer_exec: a slice is not aligned to its item");
+    // a thread reads in[s] and writes out[s]: the ROTATE ops may run exactly in place; the Weaver's f32 out[s] lies on
+    // in[s / 2], which another thread reads, so it needs disjoint slices
+    if (weaver ? overlap(d_in, n * sizeof(float2), d_out, n * ob)
+               : bad_alias(d_out, n * ob, ob, d_in, n * sizeof(float2), sizeof(float2)))
+        return b2s_fail(m->ctx, B2S_EINVAL, "b2s_mixer_exec: input and output overlap");
+    NvtxRange nvtx("b2s_mixer_exec");
+    const float2 *in = (const float2 *)d_in;
+    switch (m->op) {
+        case B2S_MIX_ROTATE_C32: return replay_exec(&m->rot, in, (float2 *)d_out, n, EpiRotate{});
+        case B2S_MIX_ROTATE_SCALE_C32: return replay_exec(&m->rot, in, (float2 *)d_out, n, EpiRotateScale{m->param});
+        case B2S_MIX_WEAVER_F32: return replay_exec(&m->rot, in, (float *)d_out, n, EpiWeaver{m->param});
+    }
+    return b2s_fail(m->ctx, B2S_EINVAL, "b2s_mixer_exec: bad op");
 }
 
 // bpf[i] = Complex32::from_polar(1.0, i as f32 * TAU * offset / sample_rate) * tap[i]   (xlating_fir.rs:80-86)

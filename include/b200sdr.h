@@ -210,14 +210,25 @@ typedef enum {
                                * (the one-pole DC blocker of examples/zigbee/src/bin/rx.rs:66-74 and
                                * examples/keyfob/src/main.rs:62-68).  param must be finite (B2S_EINVAL otherwise).
                                * A sequential recurrence: bit-exact under any slicing, one CTA per call. */
-    B2S_OP_SLICE_F32_U8  = 9  /* f32 -> u8: x > 0 ? 1 : 0 (NaN and +-0 give 0), the keyfob receiver's slicer
+    B2S_OP_SLICE_F32_U8  = 9, /* f32 -> u8: x > 0 ? 1 : 0 (NaN and +-0 give 0), the keyfob receiver's slicer
                                * (examples/keyfob/src/main.rs:73-75).  The input slice must be 4-byte aligned, the
                                * output may start at any byte; the slices must not overlap (B2S_EINVAL otherwise). */
+    B2S_OP_DIV_C32       = 10, /* c32 -> c32: x / param, each part divided (num_complex Complex / f32).  With
+                               * B2S_OP_SCALE_C32 by 2 in front it is the SSB transmitter's file level
+                               * `v * 2.0 / 0.0001` (examples/ssb/transmit.rs:125) bit for bit. */
+    B2S_OP_C32_TO_I16_IQ = 11  /* c32 -> i16 pairs: out[2j] = (re * param * 32767.0) as i16, out[2j+1] the same of im
+                               * (examples/ssb/transmit.rs:109-112, param 0.9): products rounded in that order, then
+                               * Rust's `as i16` -- truncation toward zero, saturation to [-32768, 32767], NaN -> 0.
+                               * TWO output items per input item: consumed = min(n_in, n_out_cap / 2) and
+                               * produced = 2 * consumed (ApplyNM<1, 2>, src/blocks/applynm.rs:109-117).  The input
+                               * must be 8-byte aligned and the output 2-byte aligned (any i16 item start); the
+                               * slices must not overlap (B2S_EINVAL otherwise). */
 } b2s_op;
 int32_t b2s_apply_create(b2s_ctx *ctx, b2s_op op, float param, b2s_apply **out);
 void    b2s_apply_destroy(b2s_apply *a);
 int32_t b2s_apply_reset(b2s_apply *a); /* closure state back to its initial value */
-/* m = min(n_in, n_out_cap) items are processed (apply.rs:109).  Element-wise ops may run in place (d_in == d_out);
+/* m = min(n_in, n_out_cap) items are processed (apply.rs:109), except by B2S_OP_C32_TO_I16_IQ (above).
+ * Element-wise ops may run in place (d_in == d_out);
  * the stateful demodulators (B2S_OP_QUAD_DEMOD*) need disjoint slices (B2S_EINVAL otherwise) and FINITE input
  * (their atan2 is a finite-input polynomial: inf/inf gives NaN where libm gives +-pi/4, +-3pi/4). */
 int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
@@ -237,6 +248,26 @@ int32_t b2s_rotator_exec(b2s_rotator *r, const void *d_in, size_t n_in, void *d_
 /* xlating_fir.rs:80-86 and :97-99: band-pass taps (2*ntaps floats) and the rotator's phase increment */
 int32_t b2s_xlating_taps(const float *taps, size_t ntaps, float offset, float sample_rate, size_t decimation,
                          float *bpf_interleaved, float *rotator_phase_incr);
+
+/* ---- Oscillator mixers: the Apply closures of the SSB example that carry an oscillator,
+ *      `let mut osc = Complex32::new(1.0, 0.0); ... osc *= shift; f(v, osc)` with
+ *      shift = Complex32::from_polar(1.0, phase_incr) -- the Rotator's recurrence, replayed by the same code, so every
+ *      op is bit-identical to the reference closure under any slicing of the stream (DESIGN §4.18). */
+typedef enum {
+    B2S_MIX_ROTATE_C32       = 0, /* c32 -> c32: v * osc (examples/ssb/transmit.rs:102-107); == b2s_rotator_exec     */
+    B2S_MIX_ROTATE_SCALE_C32 = 1, /* c32 -> c32: v * osc * param, each part scaled (receive.rs:58-66, param 0.0001)   */
+    B2S_MIX_WEAVER_F32       = 2  /* c32 -> f32: param * (v.re * osc.re + v.im * osc.im) (receive.rs:73-83, param 0.5) */
+} b2s_mix_op;
+typedef struct b2s_mixer b2s_mixer;
+int32_t b2s_mixer_create(b2s_ctx *ctx, b2s_mix_op op, float phase_incr, float param, b2s_mixer **out);
+void    b2s_mixer_destroy(b2s_mixer *m);
+int32_t b2s_mixer_reset(b2s_mixer *m); /* osc back to 1 + 0i (the closure's initial state) */
+/* m = min(n_in, n_out_cap) samples (apply.rs:109); consumed = produced = m.  The input must be 8-byte aligned and the
+ * output aligned to its item.  The ROTATE ops may run in place (d_in == d_out, no other overlap); the Weaver needs
+ * disjoint slices (B2S_EINVAL otherwise).  Like b2s_rotator_exec, a call only waits when the stream has outrun the
+ * host replay of the recurrence. */
+int32_t b2s_mixer_exec(b2s_mixer *m, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
+                       size_t *consumed, size_t *produced);
 
 /* ---- PfbChannelizer (≙ src/blocks/pfb/channelizer.rs:88-223; SURVEY §8f-2): polyphase FIR bank +
  * N-point inverse FFT per output vector.  Stateful like the block: one exec == one Kernel::work

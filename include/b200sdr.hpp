@@ -485,6 +485,34 @@ private:
     const Instance &inst_; Handle<b2s_rotator, b2s_rotator_destroy> h_;
 };
 
+// ≙ Apply over one of the SSB example's oscillator closures (b2s_mix_op): `osc *= shift; f(v, osc)`, bit for bit.
+// Mixer<float> is the Weaver demodulator (c32 -> f32), Mixer<Complex32> the two ROTATE ops.
+template <typename Out> class Mixer {
+public:
+    Mixer(const Instance &inst, b2s_mix_op op, float phase_incr, float param = 1.0f) : input(inst), output(inst), inst_(inst) {
+        if ((op == B2S_MIX_WEAVER_F32) != std::is_same<Out, float>::value)
+            throw Error(B2S_EINVAL, "Mixer: the Weaver op writes float, the ROTATE ops Complex32");
+        check(b2s_mixer_create(inst.get(), op, phase_incr, param, out_ptr(h_)), inst.get());
+    }
+    // one exec on device slices -> (consumed, produced); d_in == d_out runs a ROTATE op in place
+    std::pair<size_t, size_t> mix_device(const Complex32 *d_in, size_t n_in, Out *d_out, size_t n_out) {
+        size_t c = 0, p = 0;
+        check(b2s_mixer_exec(h_.get(), d_in, n_in, d_out, n_out, &c, &p), inst_.get());
+        return {c, p};
+    }
+    void reset() { check(b2s_mixer_reset(h_.get()), inst_.get()); }
+    void work(WorkIo &io) {                                                        // apply.rs:100-131
+        const size_t i_len = input.len();
+        auto [c, p] = mix_device(input.slice(), i_len, output.slice(), output.capacity());
+        input.consume(c); output.produce(p);
+        if (input.finished() && c == i_len) io.finished = true;
+    }
+    Reader<Complex32> input;
+    Writer<Out> output;
+private:
+    const Instance &inst_; Handle<b2s_mixer, b2s_mixer_destroy> h_;
+};
+
 // ≙ blocks::XlatingFir (src/blocks/xlating_fir.rs:22-126): band-pass complex taps (:80-86), decimating FIR,
 // Rotator at the output rate (:97-99, :118)
 class XlatingFir {

@@ -45,7 +45,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 def want(section):
     """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
-    zigbee, keyfob, scale)."""
+    zigbee, keyfob, ssb, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -524,6 +524,112 @@ def keyfob_section(quick):
                           "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
 
 
+def ssb_section(quick):
+    """The SSB transceiver's device closures at 64 Mi items per exec: each oscillator mixer (csrc/rotator.cu) as kernel
+    time (torch.profiler, the record ring filled before the exec) and as sustained exec time (host clock over back-to-
+    back execs, paced by the host replay of the recurrence), the record H2D copies, Apply(DivC32) and
+    ApplyNM(C32ToI16Iq) (csrc/apply.cu); fractions of 3.35 TB/s from algorithmic bytes (a mixer: 8 B in, 8 or 4 B out
+    and 1 B of records per sample).  Then the receive graph (receive.rs:54-87) end to end from a FileSource, and the C
+    oracle on one CPU thread."""
+    import subprocess
+    import tempfile
+    from torch.profiler import ProfilerActivity, profile
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import ssb_oracle as so
+    from futuresdr_b200 import ssb
+    from futuresdr_b200.edges import FileSource, Flowgraph, VectorSink
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    gpu = q[torch.cuda.current_device()] if q else "unknown"
+    print(json.dumps({"kernel": "ssb_device", "gpu": gpu}), flush=True)
+    n = (16 if quick else 64) << 20
+    peak = 3.35e12
+
+    def line(name, items, sec, bytes_per_item, **extra):
+        print(json.dumps({"kernel": f"ssb_{name}", "items": items, "ms": round(sec * 1e3, 3),
+                          "Gitems_s": round(items / sec / 1e9, 3),
+                          "frac_of_3p35_TBs": round(items * bytes_per_item / sec / peak, 3), **extra}), flush=True)
+
+    def device_us(prof, needle):
+        tot, cnt = 0.0, 0
+        for e in prof.key_averages():
+            if needle in e.key:
+                tot += getattr(e, "device_time_total", 0.0) or getattr(e, "cuda_time_total", 0.0)
+                cnt += e.count
+        return tot, cnt
+
+    x = torch.view_as_complex(torch.randn(n, 2, device="cuda"))
+    for op, out_b in ((B.MixOp.RotateC32, 8), (B.MixOp.RotateScaleC32, 8), (B.MixOp.WeaverF32, 4)):
+        o = torch.empty(n, dtype=torch.float32 if op == B.MixOp.WeaverF32 else torch.complex64, device="cuda")
+        m = B.Mixer(op, float(ssb.xlating_phase()), 0.5)
+        m.mix(x[:1 << 20], o[:1 << 20])                          # warm-up (module load, record buffers)
+        torch.cuda.synchronize()
+        m.reset()
+        time.sleep(0.5)                                          # the worker fills its 32 Mi-sample ring meanwhile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            m.mix(x, o)
+            torch.cuda.synchronize()
+        k_us, k_n = device_us(prof, "rotator_kernel")
+        c_us, c_n = device_us(prof, "Memcpy HtoD")
+        line(f"mixer_{op.name}_kernel", n, k_us * 1e-6, 8 + out_b + 1, launches=k_n,
+             records_h2d_ms=round(c_us * 1e-3, 3), h2d_copies=c_n)
+        execs = 2 if quick else 4
+        m.mix(x, o)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for _ in range(execs):
+            m.mix(x, o)
+        torch.cuda.synchronize()
+        line(f"mixer_{op.name}_sustained", n, (time.perf_counter() - t0) / execs, 8 + out_b + 1,
+             note="exec rate with the replay worker running: paced by the host recurrence, not by the GPU")
+        m.close()
+        del o
+    y = torch.empty_like(x)
+    div = B.Apply(B.ApplyOp.DivC32, 0.0001)
+    line("apply_DivC32", n, timeit(lambda: div.apply(x, y), iters=10, warm=2), 16)
+    del y
+    q16 = torch.empty(2 * n, dtype=torch.int16, device="cuda")
+    conv = B.ApplyNM(B.ApplyNMOp.C32ToI16Iq, 0.9)
+    line("applynm_C32ToI16Iq", n, timeit(lambda: conv.apply(x, q16), iters=10, warm=2), 12)
+    q16u = q16[1:]                                               # output 2-byte but not 4-byte aligned
+    line("applynm_C32ToI16Iq_out_unaligned", n - 1, timeit(lambda: conv.apply(x[:n - 1], q16u), iters=10, warm=2), 12)
+    del x, q16, q16u
+    torch.cuda.empty_cache()
+    ns = (4 if quick else 16) << 20
+    xc = (np.random.default_rng(1).standard_normal(2 * ns).astype(np.float32) * 5000).view(np.complex64)
+    with tempfile.TemporaryDirectory() as tmp:
+        path = os.path.join(tmp, "ssb_lsb_256k.dat")
+        xc.tofile(path)
+        for rate in (48_000, 8_000):
+            best = None
+            for _ in range(2):
+                fg = Flowgraph()
+                src = FileSource(path, np.complex64, repeat=False, chunk_items=1 << 20)
+                fg.add(src)
+                b = ssb.receiver(fg, src, rate)
+                fg.connect(b["weaver"], VectorSink(np.float32))
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                fg.run(buffer_items=4 << 20)
+                sec = time.perf_counter() - t0
+                best = sec if best is None else min(best, sec)
+            print(json.dumps({"kernel": f"ssb_rx_graph_{rate // 1000}k", "items": ns, "s": round(best, 4),
+                              "Msamples_s_end_to_end": round(ns / best / 1e6, 2),
+                              "note": "FileSource (256 kHz c32 file) + xlating mixer + resampler + Weaver mixer + "
+                                      "VectorSink, driven by edges.Flowgraph from Python"}), flush=True)
+    m = 16 << 20
+    xs = xc[:m]
+    for name, fn in (("mixer_RotateC32", lambda: so.Mixer(so.ROTATE, 0.1).work(xs)),
+                     ("mixer_RotateScaleC32", lambda: so.Mixer(so.ROTATE_SCALE, 0.1, 1e-4).work(xs)),
+                     ("mixer_WeaverF32", lambda: so.Mixer(so.WEAVER, 0.1, 0.5).work(xs)),
+                     ("file_level", lambda: so.file_level(xs)), ("to_i16_iq", lambda: so.to_i16_iq(xs))):
+        t0 = time.perf_counter()
+        fn()
+        sec = time.perf_counter() - t0
+        print(json.dumps({"kernel": f"ssb_oracle_cpu_1thread_{name}", "items": m, "ms": round(sec * 1e3, 2),
+                          "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -715,6 +821,8 @@ def main():
         zigbee_section(quick)
     if want("keyfob"):
         keyfob_section(quick)
+    if want("ssb"):
+        ssb_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
