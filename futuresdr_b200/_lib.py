@@ -26,6 +26,7 @@ WAVE_COS, WAVE_SIN, WAVE_SQUARE = 0, 1, 2
  COMBINE_TO_C32_NEG_Q) = range(7)
 SPLIT_RE_IM, SPLIT_DUP_F32 = 0, 1
 FANOUT_MAX_OUTPUTS = 256
+LORA_MAX_PAYLOAD = 255
 
 _vp, _sz, _i32, _f32 = C.c_void_p, C.c_size_t, C.c_int32, C.c_float
 _szp, _i32p, _vpp, _f32p = C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_float)
@@ -175,6 +176,17 @@ SIGNATURES = {
     "b2s_keyfob_exec": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_keyfob_drain_codes": (_i32, [_vp, _vp, _sz, _szp]),
     "b2s_firdes_lowpass": (_sz, [C.c_double, C.POINTER(C.c_double), _sz, _f32p, _sz]),
+    "b2s_lora_symbol_count": (_i32, [_i32, _i32, _i32, _i32, _i32, _sz, _szp]),
+    "b2s_lora_encode": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _szp, _sz, _vp, _sz, _szp]),
+    "b2s_lora_tx_create": (_i32, [_vp, _i32, _i32, _i32, _i32, _i32, _sz, C.POINTER(C.c_uint32), _sz, _sz, _vpp]),
+    "b2s_lora_tx_destroy": (None, [_vp]),
+    "b2s_lora_tx_reset": (_i32, [_vp]),
+    "b2s_lora_tx_push": (_i32, [_vp, _vp, _szp, _sz]),
+    "b2s_lora_tx_set_sync_word": (_i32, [_vp, C.c_uint32, C.c_uint32]),
+    "b2s_lora_tx_finish": (_i32, [_vp]),
+    "b2s_lora_tx_pending": (_i32, [_vp, C.POINTER(C.c_uint64)]),
+    "b2s_lora_tx_exec": (_i32, [_vp, _vp, _sz, _szp, _i32p]),
+    "b2s_lora_tx_drain_bursts": (_i32, [_vp, _vp, _sz, _szp]),
 }
 
 

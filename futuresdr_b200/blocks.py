@@ -22,6 +22,8 @@ Reference interfaces mirrored (names, argument meaning and finish rules):
                                   futuresdr_b200.zigbee
   * ``KeyfobDecoder``             examples/keyfob/src/decoder.rs:64-127 with print (:36-52); helpers in
                                   futuresdr_b200.keyfob
+  * ``LoraTransmitter``           examples/lora/src/transmitter.rs:12-168 (Encoder + Modulator); helpers in
+                                  futuresdr_b200.lora
   * ``WorkIo``                    src/runtime/work_io.rs:11-34
   * ``Mocker``                    src/runtime/mocker.rs:33-190 (single-block harness)
 
@@ -1242,6 +1244,90 @@ class KeyfobDecoder(Block, Handle):
         i = self.input.slice()
         self.input.consume(self.exec(i))
         if self.input.finished():                                               # decoder.rs:120-122
+            io.finished = True
+
+
+LORA_BURST = np.dtype([("index", np.uint64), ("len", np.uint64)], align=True)                   # b2s_lora_burst
+
+
+class LoraTransmitter(Block, Handle):
+    """examples/lora/src/transmitter.rs:12-168 (Encoder + Modulator) as a device source: no input port, one Complex32
+    output.  ``push`` is the ``msg`` handler (bytes or str payloads, encoded on the device at once), ``set_sync_word``
+    the ``synch_word`` handler and ``finish`` its Pmt::Finished.  ``work`` fills the output slice with the next samples
+    of the concatenated frames, across frame boundaries; the stream is bit-identical for every slicing.  ``bursts()``
+    returns the burst_start tags (stream index, length) of the frames started so far, a cumulative LORA_BURST array.
+    Finish rule: finished once ``finish`` has been called and every queued sample has been produced."""
+    _destroy = lib.b2s_lora_tx_destroy
+    in_dtype = None
+    out_dtype = np.complex64
+
+    def __init__(self, sf: int, code_rate: int, has_crc: bool, ldro_enabled: bool, implicit_header: bool,
+                 oversampling: int, sync_symbols, preamble_len: int, pad: int, ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.sf, self.code_rate, self.has_crc = int(sf), int(code_rate), bool(has_crc)
+        self.ldro_enabled, self.implicit_header = bool(ldro_enabled), bool(implicit_header)
+        self.oversampling, self.preamble_len, self.pad = int(oversampling), int(preamble_len), int(pad)
+        sw = (C.c_uint32 * 2)(*[int(v) for v in sync_symbols])
+        self._h = C.c_void_p()
+        check(lib.b2s_lora_tx_create(self.ctx.handle, self.sf, self.code_rate, int(self.has_crc),
+                                     int(self.ldro_enabled), int(self.implicit_header), self.oversampling, sw,
+                                     self.preamble_len, self.pad, C.byref(self._h)), self.ctx.handle)
+        self.input = None
+        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
+        self._bu = []
+
+    def push(self, *payloads):
+        """Queue frames (transmitter.rs:77-78: Pmt::Blob or Pmt::String); all or nothing."""
+        data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+        lens = (C.c_size_t * max(len(data), 1))(*[len(d) for d in data])
+        buf = b"".join(data)
+        check(lib.b2s_lora_tx_push(self._h, C.c_char_p(buf) if buf else None, lens, len(data)), self.ctx.handle)
+
+    def set_sync_word(self, word):
+        """transmitter.rs:88-110: a compact u8 (int, or one byte) expands as SynchWord::from(u8); two bytes are the
+        expanded symbols.  A word that does not fit the spreading factor raises and leaves the old one."""
+        from .lora import SynchWord
+        s0, s1 = SynchWord.from_pmt(word).expand()
+        check(lib.b2s_lora_tx_set_sync_word(self._h, s0, s1), self.ctx.handle)
+
+    def finish(self):
+        check(lib.b2s_lora_tx_finish(self._h), self.ctx.handle)
+
+    def pending(self) -> int:
+        """Queued samples not yet produced."""
+        v = C.c_uint64(0)
+        check(lib.b2s_lora_tx_pending(self._h, C.byref(v)), self.ctx.handle)
+        return v.value
+
+    def exec(self, o: torch.Tensor) -> tuple[int, bool]:
+        """Write the next samples into the device slice ``o`` (asynchronous) -> (produced, finished)."""
+        p, f = C.c_size_t(0), C.c_int32(0)
+        check(lib.b2s_lora_tx_exec(self._h, _ptr(o), o.numel(), C.byref(p), C.byref(f)), self.ctx.handle)
+        return p.value, bool(f.value)
+
+    def reset(self):
+        check(lib.b2s_lora_tx_reset(self._h), self.ctx.handle)
+        self._bu = []
+
+    def bursts(self) -> np.ndarray:
+        """Every burst_start tag so far (LORA_BURST records, in stream order)."""
+        while True:
+            buf = np.zeros(1 << 12, LORA_BURST)
+            n = C.c_size_t(0)
+            check(lib.b2s_lora_tx_drain_bursts(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
+                  self.ctx.handle)
+            self._bu.append(buf[:n.value])
+            if n.value < buf.size:
+                break
+        out = np.concatenate(self._bu)
+        self._bu = [out]
+        return out
+
+    def work(self, io: WorkIo):
+        o = self.output.slice()
+        p, finished = self.exec(o)
+        self.output.produce(p)
+        if finished:
             io.finished = True
 
 

@@ -619,6 +619,54 @@ size_t b2s_firdes_hilbert(const double *window, size_t len, float *taps, size_t 
  * f32.  The reference asserts |cutoff| < 1/2: a cutoff outside that (or NaN), or len == 0, returns 0 taps. */
 size_t b2s_firdes_lowpass(double cutoff, const double *window, size_t len, float *taps, size_t cap);
 
+/* ---- the LoRa transmitter (≙ examples/lora/src/encoder.rs:33-284, modulator.rs:46-152, transmitter.rs:34-168 with
+ * build_upchirp_phase_coherent and samples_from_phase_diff, utils.rs:917-963).  Configuration as Encoder::new: sf 5..12,
+ * code_rate 1..4 (CR 4/5 .. 4/8), has_crc, ldro_enabled, implicit_header (B2S_EINVAL otherwise).  A payload of more than
+ * B2S_LORA_MAX_PAYLOAD bytes, or of fewer than 2 bytes with has_crc, is B2S_EINVAL (the reference panics on both) and
+ * then nothing of the call is encoded or queued.  An empty payload without CRC is a frame of one interleaver block.
+ *   symbol_count: the u16 symbols Encoder::encode makes of a payload of payload_len bytes (host only).
+ *   encode:       a batch on the device: frame i is lengths[i] (HOST array) bytes of d_payloads, back to back, and its
+ *                 symbols follow those of frame i - 1 in d_symbols; *n_symbols is their total.  symbols_cap below
+ *                 the total is B2S_EINVAL.  Asynchronous on the context's stream. */
+#define B2S_LORA_MAX_PAYLOAD 255
+int32_t b2s_lora_symbol_count(int32_t sf, int32_t code_rate, int32_t has_crc, int32_t ldro_enabled,
+                              int32_t implicit_header, size_t payload_len, size_t *n_symbols);
+int32_t b2s_lora_encode(b2s_ctx *ctx, int32_t sf, int32_t code_rate, int32_t has_crc, int32_t ldro_enabled,
+                        int32_t implicit_header, const uint8_t *d_payloads, const size_t *lengths, size_t n_frames,
+                        uint16_t *d_symbols, size_t symbols_cap, size_t *n_symbols);
+/* Transmitter: a source of Complex<f32> samples, the concatenation of its frames, bit-identical to the reference under
+ * any slicing of the stream (cos / sin: see DESIGN §4.19).  A frame of n_sym symbols has
+ * 2 pad + (preamble_len + 4 [+ 2 if sf < 7]) N + N/4 - OS + n_sym N samples, N = 2^sf OS.
+ *   create:        sync_symbols is the expanded sync word (SynchWord::verify_and_expand); a symbol >= 2^sf,
+ *                  oversampling == 0, 2^sf oversampling > 2^20, or a frame that could exceed 2^32 - 1 samples is
+ *                  B2S_EINVAL.
+ *   push:          the `msg` handler for n_frames payloads (HOST memory, back to back): queues them in order and
+ *                  encodes them on the device.  May wait for the context's stream when a device buffer grows.
+ *   set_sync_word: the `synch_word` handler; applies to every frame whose first sample has not been produced yet.
+ *                  A refused word (B2S_EINVAL) leaves the old one in place.
+ *   exec:          writes the next min(n_out_cap, pending) samples of the stream to d_out (8-byte aligned); one exec
+ *                  may span several frames.  Stream-ordered, never synchronises.  *finished is set once finish has been
+ *                  called and every queued sample has been produced (Pmt::Finished, transmitter.rs:79, :134-136).
+ *   drain_bursts:  the burst_start tags (transmitter.rs:129-132, :153-159) of the frames whose first sample has been
+ *                  produced, in stream order, up to cap of them (*n); they are removed.
+ *   reset:         drops the queue, the stream position, the bursts and the finish; the sync word returns to create's. */
+typedef struct {
+    uint64_t index;       /* stream index of the frame's first sample */
+    uint64_t len;         /* the frame's samples */
+} b2s_lora_burst;
+typedef struct b2s_lora_tx b2s_lora_tx;
+int32_t b2s_lora_tx_create(b2s_ctx *ctx, int32_t sf, int32_t code_rate, int32_t has_crc, int32_t ldro_enabled,
+                           int32_t implicit_header, size_t oversampling, const uint32_t sync_symbols[2],
+                           size_t preamble_len, size_t pad, b2s_lora_tx **out);
+void    b2s_lora_tx_destroy(b2s_lora_tx *p);
+int32_t b2s_lora_tx_reset(b2s_lora_tx *p);
+int32_t b2s_lora_tx_push(b2s_lora_tx *p, const uint8_t *payloads, const size_t *lengths, size_t n_frames);
+int32_t b2s_lora_tx_set_sync_word(b2s_lora_tx *p, uint32_t sync0, uint32_t sync1);
+int32_t b2s_lora_tx_finish(b2s_lora_tx *p);
+int32_t b2s_lora_tx_pending(const b2s_lora_tx *p, uint64_t *samples);   /* queued samples not yet produced */
+int32_t b2s_lora_tx_exec(b2s_lora_tx *p, void *d_out, size_t n_out_cap, size_t *produced, int32_t *finished);
+int32_t b2s_lora_tx_drain_bursts(b2s_lora_tx *p, b2s_lora_burst *host, size_t cap, size_t *n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -16,6 +16,7 @@
 #pragma once
 
 #include <algorithm>
+#include <array>
 #include <complex>
 #include <cstdint>
 #include <cstring>
@@ -864,6 +865,70 @@ public:
     Reader<uint8_t> input;
 private:
     const Instance &inst_; Handle<b2s_keyfob, b2s_keyfob_destroy> h_;
+};
+
+// ≙ examples/lora/src/encoder.rs:33-284 over a batch: frame i is lengths[i] bytes of d_payloads (device, back to
+// back); its symbols follow frame i - 1's in d_symbols.  Returns the symbol total.
+inline size_t lora_encode(const Instance &inst, int sf, int code_rate, bool has_crc, bool ldro_enabled,
+                          bool implicit_header, const uint8_t *d_payloads, const std::vector<size_t> &lengths,
+                          uint16_t *d_symbols, size_t symbols_cap) {
+    size_t n = 0;
+    check(b2s_lora_encode(inst.get(), sf, code_rate, has_crc, ldro_enabled, implicit_header, d_payloads,
+                          lengths.data(), lengths.size(), d_symbols, symbols_cap, &n), inst.get());
+    return n;
+}
+
+// ≙ examples/lora/src/transmitter.rs:12-168: a source of Complex<f32> (std::complex<float>) samples; push is the msg
+// handler, set_sync_word the synch_word handler (expanded symbols), finish its Pmt::Finished
+class LoraTransmitter {
+public:
+    LoraTransmitter(const Instance &inst, int sf, int code_rate, bool has_crc, bool ldro_enabled, bool implicit_header,
+                    size_t oversampling, std::array<uint32_t, 2> sync_symbols, size_t preamble_len, size_t pad)
+        : output(inst), inst_(inst) {
+        check(b2s_lora_tx_create(inst.get(), sf, code_rate, has_crc, ldro_enabled, implicit_header, oversampling,
+                                 sync_symbols.data(), preamble_len, pad, out_ptr(h_)), inst.get());
+    }
+    void push(const std::vector<std::vector<uint8_t>> &payloads) {
+        std::vector<uint8_t> bytes;
+        std::vector<size_t> lens;
+        for (const auto &p : payloads) { bytes.insert(bytes.end(), p.begin(), p.end()); lens.push_back(p.size()); }
+        check(b2s_lora_tx_push(h_.get(), bytes.data(), lens.data(), lens.size()), inst_.get());
+    }
+    void set_sync_word(uint32_t s0, uint32_t s1) { check(b2s_lora_tx_set_sync_word(h_.get(), s0, s1), inst_.get()); }
+    void finish() { check(b2s_lora_tx_finish(h_.get()), inst_.get()); }
+    void reset() { check(b2s_lora_tx_reset(h_.get()), inst_.get()); }
+    uint64_t pending() const {
+        uint64_t v = 0;
+        check(b2s_lora_tx_pending(h_.get(), &v), inst_.get());
+        return v;
+    }
+    // (produced, finished) of one exec into a device slice
+    std::pair<size_t, bool> exec(std::complex<float> *d_out, size_t cap) {
+        size_t p = 0;
+        int32_t f = 0;
+        check(b2s_lora_tx_exec(h_.get(), d_out, cap, &p, &f), inst_.get());
+        return {p, f != 0};
+    }
+    void work(WorkIo &io) {
+        auto [p, f] = exec(output.slice(), output.capacity());
+        output.produce(p);
+        if (f) io.finished = true;
+    }
+    // the burst_start tags since the last drain, in stream order
+    std::vector<b2s_lora_burst> drain_bursts() {
+        std::vector<b2s_lora_burst> out;
+        for (;;) {
+            const size_t k = out.size();
+            out.resize(k + 1024);
+            size_t n = 0;
+            check(b2s_lora_tx_drain_bursts(h_.get(), out.data() + k, 1024, &n), inst_.get());
+            out.resize(k + n);
+            if (n < 1024) return out;
+        }
+    }
+    Writer<std::complex<float>> output;
+private:
+    const Instance &inst_; Handle<b2s_lora_tx, b2s_lora_tx_destroy> h_;
 };
 
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)

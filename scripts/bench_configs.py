@@ -45,7 +45,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 def want(section):
     """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
-    zigbee, keyfob, ssb, scale)."""
+    zigbee, keyfob, ssb, lora, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -630,6 +630,106 @@ def ssb_section(quick):
                           "Msamples_s": round(m / sec / 1e6, 2)}), flush=True)
 
 
+def lora_section(quick):
+    """The LoRa transmitter (csrc/lora.cu): the modulator over many queued frames as kernel time (CUDA events around one
+    exec that produces every queued sample) in Gsamples/s and as a fraction of 3.35 TB/s at 8 B/sample written; one SF7
+    frame in cycles per sample at the SM clock nvidia-smi reports as the maximum; the device encoder in frames/s; the C
+    oracle (encode + modulate with libm) on one CPU thread; and the transmit graph into a VectorSink end to end."""
+    import subprocess
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import lora_oracle as lo
+    from futuresdr_b200 import lora
+    from futuresdr_b200.edges import Flowgraph, VectorSink
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    gpu = q[torch.cuda.current_device()] if q else "unknown"
+    print(json.dumps({"kernel": "lora_device", "gpu": gpu}), flush=True)
+    try:
+        mhz = float(gpu.split(",")[2].split()[0])
+    except (IndexError, ValueError):
+        mhz = float("nan")
+    rng = np.random.default_rng(7)
+    peak = 3.35e12
+
+    def modulate_rate(name, n_frames, sf, os_, payload_len, reps):
+        tx = B.LoraTransmitter(sf, 1, True, sf >= 11, False, os_, (8, 16), 8, 0)
+        pays = [rng.integers(0, 256, payload_len, dtype=np.uint8).tobytes() for _ in range(n_frames)]
+        tx.push(*pays)
+        total = tx.pending()
+        out = torch.empty(total, dtype=torch.complex64, device="cuda")
+        best = None
+        for r in range(reps + 1):
+            if r:
+                tx.push(*pays)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            e0.record()
+            tx.exec(out)
+            e1.record()
+            torch.cuda.synchronize()
+            sec = e0.elapsed_time(e1) * 1e-3
+            if r:                                             # the first exec warms up (module load)
+                best = sec if best is None else min(best, sec)
+        print(json.dumps({"kernel": f"lora_modulate_{name}", "frames": n_frames, "samples": total,
+                          "ms": round(best * 1e3, 3), "Gsamples_s": round(total / best / 1e9, 3),
+                          "frac_of_3p35_TBs": round(total * 8 / best / peak, 3),
+                          "cycles_per_sample_per_chain": round(best * mhz * 1e6 / (total / n_frames), 2)}),
+              flush=True)
+        tx.close()
+        del out
+        torch.cuda.empty_cache()
+
+    modulate_rate("4096x_sf7_os4_16B", 4096, 7, 4, 16, 2 if quick else 5)
+    modulate_rate("1024x_sf7_os4_16B", 1024, 7, 4, 16, 2 if quick else 5)
+    modulate_rate("256x_sf12_os8_255B", 256 if not quick else 32, 12, 8, 255, 1 if quick else 2)
+    modulate_rate("1x_sf7_os4_16B", 1, 7, 4, 16, 5)
+    modulate_rate("1x_sf7_os1_255B", 1, 7, 1, 255, 5)
+    nf = 4096 if quick else 65536
+    pays = [rng.integers(0, 256, 64, dtype=np.uint8).tobytes() for _ in range(nf)]
+    lora.encode(pays[:16], 7, 1, True, False, False)
+    torch.cuda.synchronize()
+    best = None
+    for _ in range(3):
+        t0 = time.perf_counter()
+        lora.encode(pays, 7, 1, True, False, False)
+        torch.cuda.synchronize()
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "lora_encode_64B_sf7_cr1", "frames": nf, "ms": round(best * 1e3, 3),
+                      "frames_s": round(nf / best, 1), "note": "host clock: upload, one launch, synchronise"}),
+          flush=True)
+    t0 = time.perf_counter()
+    for p in pays[:1000]:
+        lo.encode(p, 7, 1, True, False, False)
+    sec = time.perf_counter() - t0
+    print(json.dumps({"kernel": "lora_oracle_cpu_1thread_encode_64B", "frames_s": round(1000 / sec, 1)}), flush=True)
+    sym = lo.encode(pays[0][:16], 7, 1, True, False, False)
+    t0 = time.perf_counter()
+    out, _ = lo.modulate(sym, 7, 4, (8, 16), 8, 0)
+    sec = time.perf_counter() - t0
+    print(json.dumps({"kernel": "lora_oracle_cpu_1thread_modulate_sf7_os4", "samples": out.size,
+                      "Msamples_s": round(out.size / sec / 1e6, 2)}), flush=True)
+    n_graph = 256 if quick else 2048
+    best = None
+    for _ in range(2):
+        fg = Flowgraph()
+        tx = lora.transmitter(fg, sf=lora.SpreadingFactor.SF7, os_factor=4)
+        sink = VectorSink(np.complex64)
+        fg.connect(tx, sink)
+        tx.push(*[rng.integers(0, 256, 16, dtype=np.uint8).tobytes() for _ in range(n_graph)])
+        total = tx.pending()
+        tx.finish()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "lora_tx_graph_sf7_os4_16B", "frames": n_graph, "samples": total,
+                      "s": round(best, 4), "Msamples_s_end_to_end": round(total / best / 1e6, 2),
+                      "note": "LoraTransmitter + VectorSink (D2H to host memory) driven by edges.Flowgraph"}),
+          flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -823,6 +923,8 @@ def main():
         keyfob_section(quick)
     if want("ssb"):
         ssb_section(quick)
+    if want("lora"):
+        lora_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)
