@@ -1331,6 +1331,91 @@ class LoraTransmitter(Block, Handle):
             io.finished = True
 
 
+WLAN_BURST = np.dtype([("index", np.uint64), ("len", np.uint64)], align=True)                   # b2s_wlan_burst
+
+
+class WlanTransmitter(Block, Handle):
+    """The WLAN transmit chain of examples/wlan/src/bin/tx.rs:44-66 (Mac -> Encoder -> Mapper -> Fft(64, Inverse,
+    shift, sqrt(1/52)) -> Prefix) as a device source: no input port, one Complex32 output.  ``push`` is the Mac's
+    ``tx`` handler: payloads (bytes or str) at the default MCS, or per-frame MCS numbers (-1: the default), framed and
+    encoded on the device at once.  ``work`` fills the output slice with the next samples of the concatenated bursts;
+    the stream is the same for every slicing.  ``bursts()`` returns the burst_start tags (stream index, length) of the
+    frames started so far, a cumulative WLAN_BURST array.  Finished once ``finish`` has been called and every queued
+    sample has been produced."""
+    _destroy = lib.b2s_wlan_tx_destroy
+    in_dtype = None
+    out_dtype = np.complex64
+
+    def __init__(self, src_mac, dst_mac, bss_mac, default_mcs: int, pad_front: int, pad_tail: int,
+                 ctx: Optional[Context] = None):
+        self.ctx = ctx or default_context()
+        self.addrs = tuple(bytes(a) for a in (src_mac, dst_mac, bss_mac))
+        if any(len(a) != 6 for a in self.addrs):
+            raise ValueError("WlanTransmitter: MAC addresses are 6 bytes")
+        self.default_mcs, self.pad_front, self.pad_tail = int(default_mcs), int(pad_front), int(pad_tail)
+        self._h = C.c_void_p()
+        check(lib.b2s_wlan_tx_create(self.ctx.handle, *[C.c_char_p(a) for a in self.addrs], self.default_mcs,
+                                     self.pad_front, self.pad_tail, C.byref(self._h)), self.ctx.handle)
+        self.input = None
+        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
+        self._bu = []
+
+    def push(self, *payloads, mcs=None):
+        """Queue frames, all or nothing.  ``mcs``: None (every frame at the default MCS, Pmt::Blob) or one MCS
+        number per payload, -1 meaning the default (the (data, mcs) pair)."""
+        data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+        n = len(data)
+        lens = (C.c_size_t * max(n, 1))(*[len(d) for d in data])
+        m = None
+        if mcs is not None:
+            if len(mcs) != n:
+                raise ValueError(f"WlanTransmitter.push: {len(mcs)} MCS for {n} payloads")
+            m = (C.c_int32 * max(n, 1))(*[int(v) for v in mcs])
+        buf = b"".join(data)
+        check(lib.b2s_wlan_tx_push(self._h, C.c_char_p(buf) if buf else None, lens, m, n), self.ctx.handle)
+
+    def finish(self):
+        check(lib.b2s_wlan_tx_finish(self._h), self.ctx.handle)
+
+    def pending(self) -> int:
+        """Queued samples not yet produced."""
+        v = C.c_uint64(0)
+        check(lib.b2s_wlan_tx_pending(self._h, C.byref(v)), self.ctx.handle)
+        return v.value
+
+    def exec(self, o: torch.Tensor) -> tuple[int, bool]:
+        """Write the next samples into the device slice ``o`` (asynchronous) -> (produced, finished)."""
+        p, f = C.c_size_t(0), C.c_int32(0)
+        check(lib.b2s_wlan_tx_exec(self._h, _ptr(o), o.numel(), C.byref(p), C.byref(f)), self.ctx.handle)
+        return p.value, bool(f.value)
+
+    def reset(self):
+        """Back to the created state: scrambler seed 1, sequence number 0, a zero bit buffer, nothing queued."""
+        check(lib.b2s_wlan_tx_reset(self._h), self.ctx.handle)
+        self._bu = []
+
+    def bursts(self) -> np.ndarray:
+        """Every burst_start tag so far (WLAN_BURST records, in stream order)."""
+        while True:
+            buf = np.zeros(1 << 12, WLAN_BURST)
+            n = C.c_size_t(0)
+            check(lib.b2s_wlan_tx_drain_bursts(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
+                  self.ctx.handle)
+            self._bu.append(buf[:n.value])
+            if n.value < buf.size:
+                break
+        out = np.concatenate(self._bu)
+        self._bu = [out]
+        return out
+
+    def work(self, io: WorkIo):
+        o = self.output.slice()
+        p, finished = self.exec(o)
+        self.output.produce(p)
+        if finished:
+            io.finished = True
+
+
 class _FanOut(Block):
     """One input, ``n`` outputs in the list attribute ``self._list``, moved by one b2s_fanout_exec launch."""
     _list = ""

@@ -19,9 +19,9 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdint>
-#include <deque>
 
 #include "common.cuh"
+#include "tx_common.cuh"
 
 namespace {
 
@@ -327,45 +327,6 @@ __global__ void __launch_bounds__(kModThreads, 2) lora_mod_kernel(ModParams m) {
     if (warp == 0 && (unsigned)lane < nj && s_job[lane].cut) m.frames[s_job[lane].frame & m.frame_mask].S = S;
 }
 
-// ---- device rings of the transmitter ----------------------------------------------------------------------------
-// Items are numbered by absolute counters; item a lives at a & (capacity - 1).  Growing moves the live items
-// [tail, head) to the new capacity under the same numbers, and synchronises.
-template <typename T> struct DevRing {
-    Buf<T> b;
-    unsigned long long mask() const { return b.size() ? b.size() - 1 : 0; }
-    int32_t make_room(b2s_ctx *ctx, unsigned long long tail, unsigned long long head, size_t n, const char *what) {
-        const size_t live = head - tail;
-        if (live + n <= b.size()) return B2S_OK;
-        size_t cap = b.size() ? b.size() : 1024;
-        while (cap < live + n) cap *= 2;
-        Buf<T> nb;
-        B2S_TRY(nb.alloc(ctx, cap, what));
-        for (unsigned long long a = tail; a < head;) {
-            const size_t so = a & mask(), d = a & (cap - 1);
-            const size_t k = std::min<size_t>({head - a, b.size() - so, cap - d});
-            B2S_CUDA(ctx, cudaMemcpyAsync(nb.get() + d, b.get() + so, k * sizeof(T), cudaMemcpyDeviceToDevice,
-                                          ctx->stream));
-            a += k;
-        }
-        B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        b = std::move(nb);
-        return B2S_OK;
-    }
-    // n host items to positions [a, a + n)
-    int32_t put(b2s_ctx *ctx, unsigned long long a, const T *host, size_t n) {
-        for (size_t i = 0; i < n;) {
-            const size_t d = (a + i) & mask(), k = std::min(n - i, b.size() - d);
-            B2S_CUDA(ctx, cudaMemcpyAsync(b.get() + d, host + i, k * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-            i += k;
-        }
-        return B2S_OK;
-    }
-};
-
-struct HostFrame {
-    unsigned long long start, len, sym_abs;
-};
-
 }  // namespace
 
 struct b2s_lora_tx {
@@ -379,12 +340,7 @@ struct b2s_lora_tx {
     DevRing<TxFrame> frames;
     Buf<unsigned char> bytes;          // the payloads of the last push
     Buf<EncFrame> enc;
-    std::deque<HostFrame> queue;       // frames not yet fully produced; the front one is frame f_tail
-    unsigned long long f_tail = 0, f_head = 0, s_tail = 0, s_head = 0;
-    unsigned long long pos = 0, total = 0;   // samples produced, samples queued
-    bool finishing = false;
-    std::vector<b2s_lora_burst> bursts;
-    size_t bursts_rd = 0;
+    TxQueue<b2s_lora_burst> q;
 };
 
 namespace {
@@ -491,13 +447,7 @@ void b2s_lora_tx_destroy(b2s_lora_tx *p) { PlanDeleter<b2s_lora_tx>()(p); }
 
 int32_t b2s_lora_tx_reset(b2s_lora_tx *p) {
     if (!p) return b2s_fail(nullptr, B2S_EINVAL, "lora transmitter is NULL");
-    p->queue.clear();
-    p->f_tail = p->f_head;
-    p->s_tail = p->s_head;
-    p->pos = p->total = 0;
-    p->finishing = false;
-    p->bursts.clear();
-    p->bursts_rd = 0;
+    p->q.reset();
     p->sync[0] = p->sync_create[0];
     p->sync[1] = p->sync_create[1];
     return B2S_OK;
@@ -508,15 +458,15 @@ int32_t b2s_lora_tx_push(b2s_lora_tx *p, const uint8_t *payloads, const size_t *
     b2s_ctx *ctx = p->ctx;
     std::vector<EncFrame> enc(n_frames);
     std::vector<TxFrame> rec(n_frames);
-    std::vector<HostFrame> hf(n_frames);
+    std::vector<TxHostFrame> hf(n_frames);
     size_t nb = 0;
-    unsigned long long ns = 0, start = p->total;
+    unsigned long long ns = 0, start = p->q.total;
     for (size_t i = 0; i < n_frames; ++i) {
         B2S_TRY(check_payload(ctx, p->cfg, lengths[i], "b2s_lora_tx_push"));
         const unsigned n_sym = (unsigned)symbol_count(p->cfg, lengths[i]);
-        enc[i] = EncFrame{nb, p->s_head + ns, (unsigned)lengths[i]};
-        rec[i] = TxFrame{start, p->s_head + ns, n_sym, 0, 0, 0.0f, 0};
-        hf[i] = HostFrame{start, p->base_len + (unsigned long long)n_sym * p->N, p->s_head + ns};
+        enc[i] = EncFrame{nb, p->q.s_head + ns, (unsigned)lengths[i]};
+        rec[i] = TxFrame{start, p->q.s_head + ns, n_sym, 0, 0, 0.0f, 0};
+        hf[i] = TxHostFrame{start, p->base_len + (unsigned long long)n_sym * p->N, p->q.s_head + ns};
         start += hf[i].len;
         nb += lengths[i];
         ns += n_sym;
@@ -525,19 +475,16 @@ int32_t b2s_lora_tx_push(b2s_lora_tx *p, const uint8_t *payloads, const size_t *
     if (!n_frames) return B2S_OK;
     DeviceGuard g(ctx->device);
     NvtxRange nvtx("b2s_lora_tx_push");
-    B2S_TRY(p->frames.make_room(ctx, p->f_tail, p->f_head, n_frames, "b2s_lora_tx_push: frame records"));
-    B2S_TRY(p->sym.make_room(ctx, p->s_tail, p->s_head, ns, "b2s_lora_tx_push: symbols"));
+    B2S_TRY(p->frames.make_room(ctx, p->q.f_tail, p->q.f_head, n_frames, "b2s_lora_tx_push: frame records"));
+    B2S_TRY(p->sym.make_room(ctx, p->q.s_tail, p->q.s_head, ns, "b2s_lora_tx_push: symbols"));
     B2S_TRY(p->bytes.reserve(ctx, std::max<size_t>(nb, 1), "b2s_lora_tx_push: payloads"));
     B2S_TRY(p->enc.reserve(ctx, n_frames, "b2s_lora_tx_push: frame table"));
     if (nb) B2S_CUDA(ctx, cudaMemcpyAsync(p->bytes.get(), payloads, nb, cudaMemcpyHostToDevice, ctx->stream));
     B2S_CUDA(ctx, cudaMemcpyAsync(p->enc.get(), enc.data(), n_frames * sizeof(EncFrame), cudaMemcpyHostToDevice,
                                   ctx->stream));
-    B2S_TRY(p->frames.put(ctx, p->f_head, rec.data(), n_frames));
+    B2S_TRY(p->frames.put(ctx, p->q.f_head, rec.data(), n_frames));
     B2S_TRY(launch_encode(ctx, p->bytes.get(), p->enc.get(), n_frames, p->cfg, p->sym.b.get(), p->sym.mask()));
-    p->queue.insert(p->queue.end(), hf.begin(), hf.end());
-    p->f_head += n_frames;
-    p->s_head += ns;
-    p->total = start;
+    p->q.append(hf, ns);
     return B2S_OK;
 }
 
@@ -551,13 +498,13 @@ int32_t b2s_lora_tx_set_sync_word(b2s_lora_tx *p, uint32_t sync0, uint32_t sync1
 
 int32_t b2s_lora_tx_finish(b2s_lora_tx *p) {
     if (!p) return b2s_fail(nullptr, B2S_EINVAL, "lora transmitter is NULL");
-    p->finishing = true;
+    p->q.finishing = true;
     return B2S_OK;
 }
 
 int32_t b2s_lora_tx_pending(const b2s_lora_tx *p, uint64_t *samples) {
     if (!p || !samples) return b2s_fail(p ? p->ctx : nullptr, B2S_EINVAL, "b2s_lora_tx_pending: NULL argument");
-    *samples = p->total - p->pos;
+    *samples = p->q.total - p->q.pos;
     return B2S_OK;
 }
 
@@ -565,19 +512,14 @@ int32_t b2s_lora_tx_exec(b2s_lora_tx *p, void *d_out, size_t n_out_cap, size_t *
     if (!p || !produced || !finished) return b2s_fail(p ? p->ctx : nullptr, B2S_EINVAL, "b2s_lora_tx_exec: NULL argument");
     b2s_ctx *ctx = p->ctx;
     *produced = 0;
-    const unsigned long long cnt = std::min<unsigned long long>(n_out_cap, p->total - p->pos);
+    const unsigned long long cnt = std::min<unsigned long long>(n_out_cap, p->q.total - p->q.pos);
     if (cnt) {
         if (!d_out || ((uintptr_t)d_out & 7))
             return b2s_fail(ctx, B2S_EINVAL, "b2s_lora_tx_exec: output slice NULL or not 8-byte aligned");
         DeviceGuard g(ctx->device);
         NvtxRange nvtx("b2s_lora_tx_exec");
-        const unsigned long long end = p->pos + cnt;
-        size_t n_jobs = 0;
-        for (const HostFrame &f : p->queue) {
-            if (f.start >= end) break;
-            if (f.start >= p->pos) p->bursts.push_back(b2s_lora_burst{f.start, f.len});   // burst_start tag
-            ++n_jobs;
-        }
+        const unsigned long long end = p->q.pos + cnt;
+        const size_t n_jobs = p->q.open(end);
         const size_t target = 2 * (size_t)std::max(ctx->sm_count, 1);
         const unsigned jpc = (unsigned)std::min<size_t>(kJobs, std::max<size_t>(1, ceil_div(n_jobs, target)));
         ModParams m;
@@ -586,10 +528,10 @@ int32_t b2s_lora_tx_exec(b2s_lora_tx *p, void *d_out, size_t n_out_cap, size_t *
         m.sym_mask = p->sym.mask();
         m.frames = p->frames.b.get();
         m.frame_mask = p->frames.mask();
-        m.f_lo = p->f_tail;
+        m.f_lo = p->q.f_tail;
         m.n_jobs = (unsigned)n_jobs;
         m.jpc = jpc;
-        m.pos = p->pos;
+        m.pos = p->q.pos;
         m.cnt = cnt;
         m.out = static_cast<float2 *>(d_out);
         m.N = p->N; m.Q = p->Q; m.pad = p->pad; m.P = p->P; m.extra = p->extra; m.base_len = p->base_len;
@@ -598,28 +540,16 @@ int32_t b2s_lora_tx_exec(b2s_lora_tx *p, void *d_out, size_t n_out_cap, size_t *
         m.sync0 = p->sync[0]; m.sync1 = p->sync[1];
         lora_mod_kernel<<<(unsigned)ceil_div(n_jobs, jpc), kModThreads, kModSmem, ctx->stream>>>(m);
         B2S_CHECK_LAUNCH(ctx);
-        p->pos = end;
-        while (!p->queue.empty() && p->queue.front().start + p->queue.front().len <= p->pos) {
-            p->queue.pop_front();
-            ++p->f_tail;
-        }
-        p->s_tail = p->queue.empty() ? p->s_head : p->queue.front().sym_abs;
+        p->q.close(end);
         *produced = (size_t)cnt;
     }
-    *finished = p->finishing && p->pos == p->total;
+    *finished = p->q.finished();
     return B2S_OK;
 }
 
 int32_t b2s_lora_tx_drain_bursts(b2s_lora_tx *p, b2s_lora_burst *host, size_t cap, size_t *n) {
     if (!p || !n || (cap && !host)) return b2s_fail(p ? p->ctx : nullptr, B2S_EINVAL, "b2s_lora_tx_drain_bursts: NULL argument");
-    const size_t k = std::min(cap, p->bursts.size() - p->bursts_rd);
-    std::copy(p->bursts.begin() + p->bursts_rd, p->bursts.begin() + p->bursts_rd + k, host);
-    p->bursts_rd += k;
-    if (p->bursts_rd == p->bursts.size()) {
-        p->bursts.clear();
-        p->bursts_rd = 0;
-    }
-    *n = k;
+    *n = p->q.drain(host, cap);
     return B2S_OK;
 }
 

@@ -667,6 +667,67 @@ int32_t b2s_lora_tx_pending(const b2s_lora_tx *p, uint64_t *samples);   /* queue
 int32_t b2s_lora_tx_exec(b2s_lora_tx *p, void *d_out, size_t n_out_cap, size_t *produced, int32_t *finished);
 int32_t b2s_lora_tx_drain_bursts(b2s_lora_tx *p, b2s_lora_burst *host, size_t cap, size_t *n);
 
+/* ---- the WLAN transmitter (≙ examples/wlan/src/mac.rs:16-103, encoder.rs:22-277, mapper.rs:23-132, the
+ * Fft::with_options(64, Inverse, true, sqrt(1/52)) of bin/tx.rs:53-59 and prefix.rs:57-141).  MCS numbers follow the
+ * reference's Mcs enum (B2S_WLAN_*); a payload is the MAC data frame's body, at most B2S_WLAN_MAX_PAYLOAD bytes, and
+ * its PSDU adds the 24-byte header and the 4-byte FCS.  One OFDM symbol is 48 subcarrier bytes (split_symbols: n_bpsc
+ * coded bits each), and a frame is its SIGNAL symbol followed by FrameParam::n_symbols data symbols.
+ *   frame_param: FrameParam::new (lib.rs:323-363) of a PSDU of psdu_len bytes (at most B2S_WLAN_MAX_PSDU).
+ *   encode:      Mac + Encoder + the SIGNAL field over a batch, from a fresh encoder (zero bit buffer) whose scrambler
+ *                seed (1..127) and sequence number (0..4095) are given: frame i is lengths[i] bytes of d_payloads
+ *                (device, back to back) at MCS mcs[i] (HOST arrays).  Each frame writes 48 (1 + n_symbols) bytes to
+ *                d_symbols, frame after frame; *n_symbols is the OFDM symbol total.  symbols_cap below it, or an
+ *                oversized payload, is B2S_EINVAL and nothing is encoded.  Asynchronous on the context's stream.
+ * Pad bits are the reference's: encoder.rs never clears its bit buffer, so the pad bits of a frame are the bits an
+ * earlier, longer frame left there (DESIGN §4.20). */
+#define B2S_WLAN_BPSK_1_2   0
+#define B2S_WLAN_BPSK_3_4   1
+#define B2S_WLAN_QPSK_1_2   2
+#define B2S_WLAN_QPSK_3_4   3
+#define B2S_WLAN_QAM16_1_2  4
+#define B2S_WLAN_QAM16_3_4  5
+#define B2S_WLAN_QAM64_2_3  6
+#define B2S_WLAN_QAM64_3_4  7
+#define B2S_WLAN_MAX_PAYLOAD 1500
+#define B2S_WLAN_MAX_PSDU    1528
+int32_t b2s_wlan_frame_param(int32_t mcs, size_t psdu_len, size_t *n_symbols, size_t *n_data_bits, size_t *n_pad);
+int32_t b2s_wlan_encode(b2s_ctx *ctx, const uint8_t src[6], const uint8_t dst[6], const uint8_t bss[6],
+                        uint32_t sequence_number, uint32_t scrambler_seed, const uint8_t *d_payloads,
+                        const size_t *lengths, const int32_t *mcs, size_t n_frames, uint8_t *d_symbols,
+                        size_t symbols_cap, size_t *n_symbols);
+/* Transmitter: a source of Complex<f32> samples, the concatenation of the Prefix block's bursts.  A frame of n OFDM
+ * symbols (SIGNAL included) has pad_front + 320 + 80 n + max(pad_tail, 1) samples.  The FFT is the library's own
+ * 64-point inverse transform (bit-identical to b2s_fft_* with shift and norm sqrtf(1/52)), so the samples are not the
+ * reference's bits (rustfft's); everything around it is its f32 arithmetic in its order.  The sample after the last
+ * symbol is windowed against 0 (the reference reads a buffer slot it has not written there).
+ *   create:       the Mac's three addresses and the Encoder's default MCS; pads above 2^32 - 1 are B2S_EINVAL.
+ *   push:         the Mac's `tx` handler for n_frames payloads (HOST memory, back to back): mcs NULL, or mcs[i] == -1,
+ *                 is the default MCS (Pmt::Blob), otherwise frame i's (the (data, mcs) pair).  A payload above
+ *                 B2S_WLAN_MAX_PAYLOAD or an MCS outside -1..7 is B2S_EINVAL and nothing is queued.  Frames are never
+ *                 dropped (the reference's encoder queue holds 1000).  Sequence number and scrambler seed advance per
+ *                 frame.  May wait for the context's stream when a device buffer grows.
+ *   exec:         writes the next min(n_out_cap, pending) samples to d_out (8-byte aligned); one exec may span
+ *                 several frames.  Stream-ordered, never synchronises.  *finished is set once finish has been called
+ *                 and every queued sample has been produced.
+ *   drain_bursts: the burst_start tags (prefix.rs:133) of the frames whose first sample has been produced, in stream
+ *                 order, up to cap of them (*n); they are removed.
+ *   reset:        the created state: seed 1, sequence number 0, a zero bit buffer, no queue, position 0, no finish. */
+typedef struct {
+    uint64_t index;       /* stream index of the frame's first sample */
+    uint64_t len;         /* the frame's samples */
+} b2s_wlan_burst;
+typedef struct b2s_wlan_tx b2s_wlan_tx;
+int32_t b2s_wlan_tx_create(b2s_ctx *ctx, const uint8_t src[6], const uint8_t dst[6], const uint8_t bss[6],
+                           int32_t default_mcs, size_t pad_front, size_t pad_tail, b2s_wlan_tx **out);
+void    b2s_wlan_tx_destroy(b2s_wlan_tx *p);
+int32_t b2s_wlan_tx_reset(b2s_wlan_tx *p);
+int32_t b2s_wlan_tx_push(b2s_wlan_tx *p, const uint8_t *payloads, const size_t *lengths, const int32_t *mcs,
+                         size_t n_frames);
+int32_t b2s_wlan_tx_finish(b2s_wlan_tx *p);
+int32_t b2s_wlan_tx_pending(const b2s_wlan_tx *p, uint64_t *samples);   /* queued samples not yet produced */
+int32_t b2s_wlan_tx_exec(b2s_wlan_tx *p, void *d_out, size_t n_out_cap, size_t *produced, int32_t *finished);
+int32_t b2s_wlan_tx_drain_bursts(b2s_wlan_tx *p, b2s_wlan_burst *host, size_t cap, size_t *n);
+
 #ifdef __cplusplus
 }
 #endif

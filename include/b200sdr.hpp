@@ -931,6 +931,75 @@ private:
     const Instance &inst_; Handle<b2s_lora_tx, b2s_lora_tx_destroy> h_;
 };
 
+// ≙ examples/wlan/src/{mac,encoder}.rs + the SIGNAL field over a batch from a fresh encoder: frame i is lengths[i]
+// bytes of d_payloads (device, back to back) at mcs[i]; 48 subcarrier bytes per OFDM symbol, SIGNAL first, frame after
+// frame in d_symbols.  Returns the OFDM symbol total.
+inline size_t wlan_encode(const Instance &inst, const std::array<uint8_t, 6> &src, const std::array<uint8_t, 6> &dst,
+                          const std::array<uint8_t, 6> &bss, uint32_t sequence_number, uint32_t scrambler_seed,
+                          const uint8_t *d_payloads, const std::vector<size_t> &lengths,
+                          const std::vector<int32_t> &mcs, uint8_t *d_symbols, size_t symbols_cap) {
+    if (mcs.size() != lengths.size()) throw Error(B2S_EINVAL, "wlan_encode: one MCS per payload");
+    size_t n = 0;
+    check(b2s_wlan_encode(inst.get(), src.data(), dst.data(), bss.data(), sequence_number, scrambler_seed, d_payloads,
+                          lengths.data(), mcs.data(), lengths.size(), d_symbols, symbols_cap, &n), inst.get());
+    return n;
+}
+
+// ≙ examples/wlan/src/bin/tx.rs:44-66 without the radio sink (Mac -> Encoder -> Mapper -> Fft -> Prefix): a source of
+// Complex<f32> (std::complex<float>) samples; push is the Mac's tx handler, finish its Pmt::Finished
+class WlanTransmitter {
+public:
+    WlanTransmitter(const Instance &inst, const std::array<uint8_t, 6> &src, const std::array<uint8_t, 6> &dst,
+                    const std::array<uint8_t, 6> &bss, int32_t default_mcs, size_t pad_front, size_t pad_tail)
+        : output(inst), inst_(inst) {
+        check(b2s_wlan_tx_create(inst.get(), src.data(), dst.data(), bss.data(), default_mcs, pad_front, pad_tail,
+                                 out_ptr(h_)), inst.get());
+    }
+    // mcs empty: every frame at the default MCS; otherwise one per payload, -1 meaning the default
+    void push(const std::vector<std::vector<uint8_t>> &payloads, const std::vector<int32_t> &mcs = {}) {
+        if (!mcs.empty() && mcs.size() != payloads.size()) throw Error(B2S_EINVAL, "wlan push: one MCS per payload");
+        std::vector<uint8_t> bytes;
+        std::vector<size_t> lens;
+        for (const auto &p : payloads) { bytes.insert(bytes.end(), p.begin(), p.end()); lens.push_back(p.size()); }
+        check(b2s_wlan_tx_push(h_.get(), bytes.data(), lens.data(), mcs.empty() ? nullptr : mcs.data(), lens.size()),
+              inst_.get());
+    }
+    void finish() { check(b2s_wlan_tx_finish(h_.get()), inst_.get()); }
+    void reset() { check(b2s_wlan_tx_reset(h_.get()), inst_.get()); }
+    uint64_t pending() const {
+        uint64_t v = 0;
+        check(b2s_wlan_tx_pending(h_.get(), &v), inst_.get());
+        return v;
+    }
+    // (produced, finished) of one exec into a device slice
+    std::pair<size_t, bool> exec(std::complex<float> *d_out, size_t cap) {
+        size_t p = 0;
+        int32_t f = 0;
+        check(b2s_wlan_tx_exec(h_.get(), d_out, cap, &p, &f), inst_.get());
+        return {p, f != 0};
+    }
+    void work(WorkIo &io) {
+        auto [p, f] = exec(output.slice(), output.capacity());
+        output.produce(p);
+        if (f) io.finished = true;
+    }
+    // the burst_start tags since the last drain, in stream order
+    std::vector<b2s_wlan_burst> drain_bursts() {
+        std::vector<b2s_wlan_burst> out;
+        for (;;) {
+            const size_t k = out.size();
+            out.resize(k + 1024);
+            size_t n = 0;
+            check(b2s_wlan_tx_drain_bursts(h_.get(), out.data() + k, 1024, &n), inst_.get());
+            out.resize(k + n);
+            if (n < 1024) return out;
+        }
+    }
+    Writer<std::complex<float>> output;
+private:
+    const Instance &inst_; Handle<b2s_wlan_tx, b2s_wlan_tx_destroy> h_;
+};
+
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
 template <typename T, int32_t Deinterleave> class FanOut {
     static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");

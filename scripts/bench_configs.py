@@ -45,7 +45,7 @@ def report(name, n_in, bytes_alg, sec, extra=""):
 
 def want(section):
     """--only a,b,c runs just the named sections (fir, f32, chain, fft, resamp, next, iir, sigsrc, stream, boxavg, adsb,
-    zigbee, keyfob, ssb, lora, scale)."""
+    zigbee, keyfob, ssb, lora, wlan, scale)."""
     for i, a in enumerate(sys.argv):
         if a == "--only" and i + 1 < len(sys.argv):
             return section in sys.argv[i + 1].split(",")
@@ -730,6 +730,90 @@ def lora_section(quick):
           flush=True)
 
 
+def wlan_section(quick):
+    """The WLAN transmitter (csrc/wlan.cu): the OFDM exec kernel over 4096 queued frames of 1500 bytes at BPSK 1/2 and
+    64-QAM 3/4 with pads of 5000 (tx.rs) as kernel time (CUDA events around one exec that produces every queued sample),
+    in Gsamples/s and as a fraction of 3.35 TB/s at 8 B/sample written; the same exec cut into 1 Mi-sample execs; the
+    device encoder in frames/s; and the transmit graph into a VectorSink end to end."""
+    import subprocess
+    from futuresdr_b200 import wlan
+    from futuresdr_b200.edges import Flowgraph, VectorSink
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    gpu = q[torch.cuda.current_device()] if q else "unknown"
+    print(json.dumps({"kernel": "wlan_device", "gpu": gpu}), flush=True)
+    rng = np.random.default_rng(8)
+    peak = 3.35e12
+    nf = 512 if quick else 4096
+    pays = [rng.integers(0, 256, 1500, dtype=np.uint8).tobytes() for _ in range(nf)]
+
+    def exec_rate(name, mcs, reps, cap=None):
+        tx = B.WlanTransmitter(wlan.SRC_MAC, wlan.DST_MAC, wlan.BSS_MAC, int(mcs), 5000, 5000)
+        tx.push(*pays)
+        total = tx.pending()
+        out = torch.empty(total, dtype=torch.complex64, device="cuda")
+        best = None
+        for r in range(reps + 1):
+            if r:
+                tx.push(*pays)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            e0.record()
+            if cap is None:
+                tx.exec(out)
+            else:
+                for o in range(0, total, cap):
+                    tx.exec(out[o:o + cap])
+            e1.record()
+            torch.cuda.synchronize()
+            sec = e0.elapsed_time(e1) * 1e-3
+            if r:                                             # the first exec warms up (module load)
+                best = sec if best is None else min(best, sec)
+        print(json.dumps({"kernel": f"wlan_exec_{name}", "frames": nf, "samples": total,
+                          "execs": 1 if cap is None else -(-total // cap), "ms": round(best * 1e3, 3),
+                          "Gsamples_s": round(total / best / 1e9, 3),
+                          "frac_of_3p35_TBs": round(total * 8 / best / peak, 3)}), flush=True)
+        tx.close()
+        del out
+        torch.cuda.empty_cache()
+
+    exec_rate(f"{nf}x1500B_bpsk12_pad5000", wlan.Mcs.BPSK_1_2, 2 if quick else 5)
+    exec_rate(f"{nf}x1500B_qam64_34_pad5000", wlan.Mcs.QAM64_3_4, 2 if quick else 5)
+    exec_rate(f"{nf}x1500B_qam64_34_pad5000_1Mi_execs", wlan.Mcs.QAM64_3_4, 2 if quick else 3, cap=1 << 20)
+    for mcs in (wlan.Mcs.BPSK_1_2, wlan.Mcs.QAM64_3_4):
+        wlan.encode(pays[:16], mcs)
+        torch.cuda.synchronize()
+        best = None
+        for _ in range(3):
+            t0 = time.perf_counter()
+            wlan.encode(pays, mcs)
+            torch.cuda.synchronize()
+            sec = time.perf_counter() - t0
+            best = sec if best is None else min(best, sec)
+        print(json.dumps({"kernel": f"wlan_encode_1500B_{mcs.name.lower()}", "frames": nf, "ms": round(best * 1e3, 3),
+                          "frames_s": round(nf / best, 1), "note": "host clock: upload, three launches, synchronise"}),
+              flush=True)
+    n_graph = 128 if quick else 1024
+    best = None
+    for _ in range(2):
+        fg = Flowgraph()
+        tx = wlan.transmitter(fg, default_mcs=wlan.Mcs.QAM16_1_2)
+        sink = VectorSink(np.complex64)
+        fg.connect(tx, sink)
+        tx.push(*pays[:n_graph])
+        total = tx.pending()
+        tx.finish()
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fg.run(buffer_items=4 << 20)
+        sec = time.perf_counter() - t0
+        best = sec if best is None else min(best, sec)
+    print(json.dumps({"kernel": "wlan_tx_graph_qam16_12_1500B_pad5000", "frames": n_graph, "samples": total,
+                      "s": round(best, 4), "Msamples_s_end_to_end": round(total / best / 1e6, 2),
+                      "note": "WlanTransmitter + VectorSink (D2H to host memory) driven by edges.Flowgraph"}),
+          flush=True)
+
+
 def main():
     quick = "--quick" in sys.argv
     n = (16 if quick else 64) * 1024 * 1024
@@ -925,6 +1009,8 @@ def main():
         ssb_section(quick)
     if want("lora"):
         lora_section(quick)
+    if want("wlan"):
+        wlan_section(quick)
     if want("scale"):
         # element-wise scale (the Vulkan/wgpu shader)
         sc = B.Apply(B.ApplyOp.ScaleF32, 12.0)

@@ -13,3 +13,5 @@ timeout 600 compute-sanitizer --tool memcheck --print-limit 5 python -m pytest t
 timeout 600 compute-sanitizer --tool racecheck --print-limit 5 python -m pytest tests/test_gpu_ssb.py -m gpu -q -x -k "not 40mi and not loopback and not graph and not random" 2>&1 | tail -8
 timeout 600 compute-sanitizer --tool memcheck --print-limit 5 python -m pytest tests/test_gpu_lora.py -m gpu -q -x -k "slicing or sync_word or finish or refuses" 2>&1 | tail -8
 timeout 600 compute-sanitizer --tool racecheck --print-limit 5 python -m pytest tests/test_gpu_lora.py -m gpu -q -x -k "sync_word or finish" 2>&1 | tail -8
+timeout 600 compute-sanitizer --tool memcheck --print-limit 5 python -m pytest tests/test_gpu_wlan.py -m gpu -q -x -k "slicing or pads or refusals or finish or stale" 2>&1 | tail -8
+timeout 600 compute-sanitizer --tool racecheck --print-limit 5 python -m pytest tests/test_gpu_wlan.py -m gpu -q -x -k "slicing or pads" 2>&1 | tail -8
