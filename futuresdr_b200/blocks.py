@@ -203,14 +203,9 @@ class FirBuilder:
         return Fir(PolyphaseResamplingFir(interp, decim, taps, sample_dtype, ctx))
 
 
-class Iir(Block):
-    """blocks::Iir (src/blocks/iir.rs:8-176): generic over a ``StatefulFilter`` core (an ``IirFilter``)."""
-
-    def __init__(self, core: IirFilter):
-        self.filter = core
-        self.in_dtype = self.out_dtype = core.sample_dtype
-        self._ports()
-        self.input.set_min_items(core.length())              # iir.rs:133
+class Iir(Fir):
+    """blocks::Iir (src/blocks/iir.rs:8-176): generic over a ``StatefulFilter`` core (an ``IirFilter``).  Its input
+    minimum (iir.rs:133) and its work and finish rule (iir.rs:156-175) are Fir's."""
 
     @classmethod
     def new(cls, a_taps, b_taps, sample_dtype=np.float32, ctx: Optional[Context] = None) -> "Iir":
@@ -219,14 +214,6 @@ class Iir(Block):
     @classmethod
     def with_core(cls, core: IirFilter) -> "Iir":
         return cls(core)
-
-    def work(self, io: WorkIo):
-        i, o = self.input.slice(), self.output.slice()        # iir.rs:162-163
-        consumed, produced, status = self.filter.filter(i, o)
-        self.input.consume(consumed)
-        self.output.produce(produced)
-        if self.input.finished() and status != ComputationStatus.InsufficientOutput:   # iir.rs:170-172
-            io.finished = True
 
 
 class IirBuilder:
@@ -471,15 +458,21 @@ class Apply(Block, Handle):
         check(lib.b2s_apply_reset(self._h), self.ctx.handle)
 
     def work(self, io: WorkIo):
-        i, o = self.input.slice(), self.output.slice()
-        i_len = i.numel()
-        m = min(i_len, o.numel())                                               # apply.rs:109
-        if m > 0:
-            self.apply(i, o)
-            self.input.consume(m)
-            self.output.produce(m)
-        if self.input.finished() and m == i_len:                                 # apply.rs:126-128
-            io.finished = True
+        _apply_work(self, self.apply, io)
+
+
+def _apply_work(block: Block, closure, io: WorkIo):
+    """Apply::work (apply.rs:109-128): ``closure(i, o)`` over min(len) items of the block's slices; the block finishes
+    once its input is finished and every item on it was processed."""
+    i, o = block.input.slice(), block.output.slice()
+    i_len = i.numel()
+    m = min(i_len, o.numel())                                                   # apply.rs:109
+    if m > 0:
+        closure(i, o)
+        block.input.consume(m)
+        block.output.produce(m)
+    if block.input.finished() and m == i_len:                                   # apply.rs:126-128
+        io.finished = True
 
 
 class ApplyNMOp(enum.IntEnum):
@@ -617,15 +610,7 @@ class Mixer(Block, Handle):
         check(lib.b2s_mixer_reset(self._h), self.ctx.handle)
 
     def work(self, io: WorkIo):
-        i, o = self.input.slice(), self.output.slice()
-        i_len = i.numel()
-        m = min(i_len, o.numel())                                               # apply.rs:109
-        if m > 0:
-            self.mix(i, o)
-            self.input.consume(m)
-            self.output.produce(m)
-        if self.input.finished() and m == i_len:                                 # apply.rs:126-128
-            io.finished = True
+        _apply_work(self, self.mix, io)
 
 
 class XlatingFir(Block):
@@ -1023,6 +1008,39 @@ class MovingAverage(Block, Handle):
             io.finished = True
 
 
+class _Records:
+    """One record list of a block, handed out by ``drain(handle, host, cap, &n)`` (a b2s_*_drain_* function).  ``read``
+    drains it until a short read and returns every record so far, a cumulative numpy structured array of ``dtype`` in
+    stream order; draining synchronises.  ``clear`` forgets the records, as the block's reset does."""
+    chunk = 1 << 16        # records per drain call; the loop ends on a short read, so the result does not depend on it
+
+    def __init__(self, drain, dtype):
+        self.drain, self.dtype = drain, np.dtype(dtype)
+        self.clear()
+
+    def clear(self):
+        self._parts = []
+
+    def read(self, h, ctx_handle) -> np.ndarray:
+        while True:
+            buf = np.zeros(self.chunk, self.dtype)
+            n = C.c_size_t(0)
+            check(self.drain(h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)), ctx_handle)
+            self._parts.append(buf[:n.value])
+            if n.value < buf.size:
+                out = np.concatenate(self._parts)
+                self._parts = [out]
+                return out
+
+
+def _payload_batch(payloads):
+    """Payloads (a str as UTF-8, or bytes-like) as the push and encode calls take them: (their bytes, those joined,
+    their lengths as a c_size_t array).  The array has at least one element, so an empty batch passes a valid
+    pointer."""
+    data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+    return data, b"".join(data), (C.c_size_t * max(len(data), 1))(*[len(d) for d in data])
+
+
 ADSB_PACKET = np.dtype([("preamble_index", np.uint64), ("preamble_correlation", np.float32),
                         ("crc_passed", np.int32), ("bytes", np.uint8, 14)], align=True)   # b2s_adsb_packet
 ADSB_DETECTION = np.dtype([("index", np.uint64), ("value", np.float32)], align=True)      # b2s_adsb_detection
@@ -1053,7 +1071,8 @@ class AdsbDemod(Block, Handle):
               self.ctx.handle)
         dev = _ctx_device(self.ctx)
         self.in_samples, self.in_nf, self.in_preamble_cor = (Reader(_F32, dev) for _ in range(3))
-        self._pk, self._det = [], []
+        self._packets = _Records(lib.b2s_adsb_drain_packets, ADSB_PACKET)
+        self._detections = _Records(lib.b2s_adsb_drain_detections, ADSB_DETECTION)
 
     def stream_inputs(self):
         return ["in_samples", "in_nf", "in_preamble_cor"]
@@ -1070,28 +1089,16 @@ class AdsbDemod(Block, Handle):
 
     def reset(self):
         check(lib.b2s_adsb_reset(self._h), self.ctx.handle)
-        self._pk, self._det = [], []
-
-    def _drain(self, fn, dtype, acc):
-        while True:
-            buf = np.zeros(1 << 16, dtype)
-            n = C.c_size_t(0)
-            check(fn(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)), self.ctx.handle)
-            acc.append(buf[:n.value])
-            if n.value < buf.size:
-                return np.concatenate(acc)
+        self._packets.clear()
+        self._detections.clear()
 
     def packets(self) -> np.ndarray:
         """Every packet so far (ADSB_PACKET records, in index order)."""
-        out = self._drain(lib.b2s_adsb_drain_packets, ADSB_PACKET, self._pk)
-        self._pk = [out]
-        return out
+        return self._packets.read(self._h, self.ctx.handle)
 
     def detections(self) -> np.ndarray:
         """Every detector tag so far (ADSB_DETECTION records, in index order; equal indices can repeat)."""
-        out = self._drain(lib.b2s_adsb_drain_detections, ADSB_DETECTION, self._det)
-        self._det = [out]
-        return out
+        return self._detections.read(self._h, self.ctx.handle)
 
     def work(self, io: WorkIo):
         ports = (self.in_samples, self.in_nf, self.in_preamble_cor)
@@ -1146,111 +1153,132 @@ class ClockRecoveryMm(Block, Handle):
             io.finished = True
 
 
+class _Decoder(Block, Handle):
+    """The body of the decoders that turn one stream input into records, with no stream output: ``exec``, ``reset``, the
+    record reader and ``work``.  A subclass names its ABI functions and record type, calls ``__init__`` and then
+    creates ``self._h``."""
+    out_dtype = None
+    _exec = _reset = _drain = _record = None
+
+    def __init__(self, ctx: Optional[Context]):
+        self.ctx = ctx or default_context()
+        self.input = Reader(self.in_dtype, _ctx_device(self.ctx))
+        self._records = _Records(self._drain, self._record)
+
+    def exec(self, i: torch.Tensor) -> int:
+        c = C.c_size_t(0)
+        check(self._exec(self._h, _ptr(i), i.numel(), C.byref(c)), self.ctx.handle)
+        return c.value
+
+    def reset(self):
+        check(self._reset(self._h), self.ctx.handle)
+        self._records.clear()
+
+    def work(self, io: WorkIo):
+        i = self.input.slice()
+        self.input.consume(self.exec(i))
+        if self.input.finished():                       # zigbee decoder.rs:174-176, keyfob decoder.rs:120-122
+            io.finished = True
+
+
 ZIGBEE_FRAME = np.dtype([("index", np.uint64), ("len", np.uint32), ("crc_ok", np.int32), ("bytes", np.uint8, 128)],
                         align=True)                                                          # b2s_zigbee_frame
 
 
-class ZigbeeDecoder(Block, Handle):
+class ZigbeeDecoder(_Decoder):
     """examples/zigbee/src/decoder.rs:78-183 with Mac::check_crc (mac.rs:62-85) as a device block: one f32 stream
     input, no stream output.  The frames the reference posts come out of ``frames()``, a cumulative numpy structured
     array (ZIGBEE_FRAME: the stream index of the chip that completed the frame, its length, whether its FCS checks,
     its bytes); reading it synchronises.  Every exec consumes its whole slice and never synchronises."""
     _destroy = lib.b2s_zigbee_destroy
+    _exec, _reset = lib.b2s_zigbee_exec, lib.b2s_zigbee_reset
+    _drain, _record = lib.b2s_zigbee_drain_frames, ZIGBEE_FRAME
     in_dtype = np.float32
-    out_dtype = None
 
     def __init__(self, threshold: int = 6, ctx: Optional[Context] = None):
-        self.ctx = ctx or default_context()
+        super().__init__(ctx)
         self.threshold = int(threshold)
         self._h = C.c_void_p()
         check(lib.b2s_zigbee_create(self.ctx.handle, C.c_uint32(self.threshold), C.byref(self._h)), self.ctx.handle)
-        self.input = Reader(self.in_dtype, _ctx_device(self.ctx))
-        self._fr = []
-
-    def exec(self, i: torch.Tensor) -> int:
-        c = C.c_size_t(0)
-        check(lib.b2s_zigbee_exec(self._h, _ptr(i), i.numel(), C.byref(c)), self.ctx.handle)
-        return c.value
-
-    def reset(self):
-        check(lib.b2s_zigbee_reset(self._h), self.ctx.handle)
-        self._fr = []
 
     def frames(self) -> np.ndarray:
         """Every frame so far (ZIGBEE_FRAME records, in stream order)."""
-        while True:
-            buf = np.zeros(1 << 12, ZIGBEE_FRAME)
-            n = C.c_size_t(0)
-            check(lib.b2s_zigbee_drain_frames(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
-                  self.ctx.handle)
-            self._fr.append(buf[:n.value])
-            if n.value < buf.size:
-                break
-        out = np.concatenate(self._fr)
-        self._fr = [out]
-        return out
-
-    def work(self, io: WorkIo):
-        i = self.input.slice()
-        self.input.consume(self.exec(i))
-        if self.input.finished():                                               # decoder.rs:174-176
-            io.finished = True
+        return self._records.read(self._h, self.ctx.handle)
 
 
 KEYFOB_CODE = np.dtype([("index", np.uint64), ("n_bits", np.uint32), ("label", np.int32), ("bits", np.uint8, 32)],
                        align=True)                                                           # b2s_keyfob_code
 
 
-class KeyfobDecoder(Block, Handle):
+class KeyfobDecoder(_Decoder):
     """examples/keyfob/src/decoder.rs:64-127 with print (:36-52) as a device block: one u8 stream input, no stream
     output.  The strings the reference logs come out of ``codes()``, a cumulative numpy structured array (KEYFOB_CODE:
     the stream position of the flushing edge, the length after the prefix strip, the label of the last 8 bits, the
     first 256 bits MSB first); reading it synchronises.  Every exec consumes its whole slice and never synchronises."""
     _destroy = lib.b2s_keyfob_destroy
+    _exec, _reset = lib.b2s_keyfob_exec, lib.b2s_keyfob_reset
+    _drain, _record = lib.b2s_keyfob_drain_codes, KEYFOB_CODE
     in_dtype = np.uint8
-    out_dtype = None
 
     def __init__(self, ctx: Optional[Context] = None):
-        self.ctx = ctx or default_context()
+        super().__init__(ctx)
         self._h = C.c_void_p()
         check(lib.b2s_keyfob_create(self.ctx.handle, C.byref(self._h)), self.ctx.handle)
-        self.input = Reader(self.in_dtype, _ctx_device(self.ctx))
-        self._cd = []
-
-    def exec(self, i: torch.Tensor) -> int:
-        c = C.c_size_t(0)
-        check(lib.b2s_keyfob_exec(self._h, _ptr(i), i.numel(), C.byref(c)), self.ctx.handle)
-        return c.value
-
-    def reset(self):
-        check(lib.b2s_keyfob_reset(self._h), self.ctx.handle)
-        self._cd = []
 
     def codes(self) -> np.ndarray:
         """Every code so far (KEYFOB_CODE records, in stream order)."""
-        while True:
-            buf = np.zeros(1 << 12, KEYFOB_CODE)
-            n = C.c_size_t(0)
-            check(lib.b2s_keyfob_drain_codes(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
-                  self.ctx.handle)
-            self._cd.append(buf[:n.value])
-            if n.value < buf.size:
-                break
-        out = np.concatenate(self._cd)
-        self._cd = [out]
-        return out
+        return self._records.read(self._h, self.ctx.handle)
+
+
+class _Transmitter(Block, Handle):
+    """The body of the device transmitters, sources with one Complex32 output: ``finish``, ``pending``, ``exec``,
+    ``reset``, ``bursts`` and ``work``.  A subclass names its ABI functions and burst record type, calls ``__init__``
+    and then creates ``self._h``."""
+    in_dtype = None
+    out_dtype = np.complex64
+    _finish = _pending = _exec = _reset = _drain = _record = None
+
+    def __init__(self, ctx: Optional[Context]):
+        self.ctx = ctx or default_context()
+        self.input = None
+        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
+        self._records = _Records(self._drain, self._record)
+
+    def finish(self):
+        check(self._finish(self._h), self.ctx.handle)
+
+    def pending(self) -> int:
+        """Queued samples not yet produced."""
+        v = C.c_uint64(0)
+        check(self._pending(self._h, C.byref(v)), self.ctx.handle)
+        return v.value
+
+    def exec(self, o: torch.Tensor) -> tuple[int, bool]:
+        """Write the next samples into the device slice ``o`` (asynchronous) -> (produced, finished)."""
+        p, f = C.c_size_t(0), C.c_int32(0)
+        check(self._exec(self._h, _ptr(o), o.numel(), C.byref(p), C.byref(f)), self.ctx.handle)
+        return p.value, bool(f.value)
+
+    def reset(self):
+        check(self._reset(self._h), self.ctx.handle)
+        self._records.clear()
+
+    def bursts(self) -> np.ndarray:
+        """Every burst_start tag so far (the class's burst records, in stream order)."""
+        return self._records.read(self._h, self.ctx.handle)
 
     def work(self, io: WorkIo):
-        i = self.input.slice()
-        self.input.consume(self.exec(i))
-        if self.input.finished():                                               # decoder.rs:120-122
+        o = self.output.slice()
+        p, finished = self.exec(o)
+        self.output.produce(p)
+        if finished:
             io.finished = True
 
 
 LORA_BURST = np.dtype([("index", np.uint64), ("len", np.uint64)], align=True)                   # b2s_lora_burst
 
 
-class LoraTransmitter(Block, Handle):
+class LoraTransmitter(_Transmitter):
     """examples/lora/src/transmitter.rs:12-168 (Encoder + Modulator) as a device source: no input port, one Complex32
     output.  ``push`` is the ``msg`` handler (bytes or str payloads, encoded on the device at once), ``set_sync_word``
     the ``synch_word`` handler and ``finish`` its Pmt::Finished.  ``work`` fills the output slice with the next samples
@@ -1258,12 +1286,12 @@ class LoraTransmitter(Block, Handle):
     returns the burst_start tags (stream index, length) of the frames started so far, a cumulative LORA_BURST array.
     Finish rule: finished once ``finish`` has been called and every queued sample has been produced."""
     _destroy = lib.b2s_lora_tx_destroy
-    in_dtype = None
-    out_dtype = np.complex64
+    _finish, _pending, _exec = lib.b2s_lora_tx_finish, lib.b2s_lora_tx_pending, lib.b2s_lora_tx_exec
+    _reset, _drain, _record = lib.b2s_lora_tx_reset, lib.b2s_lora_tx_drain_bursts, LORA_BURST
 
     def __init__(self, sf: int, code_rate: int, has_crc: bool, ldro_enabled: bool, implicit_header: bool,
                  oversampling: int, sync_symbols, preamble_len: int, pad: int, ctx: Optional[Context] = None):
-        self.ctx = ctx or default_context()
+        super().__init__(ctx)
         self.sf, self.code_rate, self.has_crc = int(sf), int(code_rate), bool(has_crc)
         self.ldro_enabled, self.implicit_header = bool(ldro_enabled), bool(implicit_header)
         self.oversampling, self.preamble_len, self.pad = int(oversampling), int(preamble_len), int(pad)
@@ -1272,15 +1300,10 @@ class LoraTransmitter(Block, Handle):
         check(lib.b2s_lora_tx_create(self.ctx.handle, self.sf, self.code_rate, int(self.has_crc),
                                      int(self.ldro_enabled), int(self.implicit_header), self.oversampling, sw,
                                      self.preamble_len, self.pad, C.byref(self._h)), self.ctx.handle)
-        self.input = None
-        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
-        self._bu = []
 
     def push(self, *payloads):
         """Queue frames (transmitter.rs:77-78: Pmt::Blob or Pmt::String); all or nothing."""
-        data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
-        lens = (C.c_size_t * max(len(data), 1))(*[len(d) for d in data])
-        buf = b"".join(data)
+        data, buf, lens = _payload_batch(payloads)
         check(lib.b2s_lora_tx_push(self._h, C.c_char_p(buf) if buf else None, lens, len(data)), self.ctx.handle)
 
     def set_sync_word(self, word):
@@ -1290,51 +1313,11 @@ class LoraTransmitter(Block, Handle):
         s0, s1 = SynchWord.from_pmt(word).expand()
         check(lib.b2s_lora_tx_set_sync_word(self._h, s0, s1), self.ctx.handle)
 
-    def finish(self):
-        check(lib.b2s_lora_tx_finish(self._h), self.ctx.handle)
-
-    def pending(self) -> int:
-        """Queued samples not yet produced."""
-        v = C.c_uint64(0)
-        check(lib.b2s_lora_tx_pending(self._h, C.byref(v)), self.ctx.handle)
-        return v.value
-
-    def exec(self, o: torch.Tensor) -> tuple[int, bool]:
-        """Write the next samples into the device slice ``o`` (asynchronous) -> (produced, finished)."""
-        p, f = C.c_size_t(0), C.c_int32(0)
-        check(lib.b2s_lora_tx_exec(self._h, _ptr(o), o.numel(), C.byref(p), C.byref(f)), self.ctx.handle)
-        return p.value, bool(f.value)
-
-    def reset(self):
-        check(lib.b2s_lora_tx_reset(self._h), self.ctx.handle)
-        self._bu = []
-
-    def bursts(self) -> np.ndarray:
-        """Every burst_start tag so far (LORA_BURST records, in stream order)."""
-        while True:
-            buf = np.zeros(1 << 12, LORA_BURST)
-            n = C.c_size_t(0)
-            check(lib.b2s_lora_tx_drain_bursts(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
-                  self.ctx.handle)
-            self._bu.append(buf[:n.value])
-            if n.value < buf.size:
-                break
-        out = np.concatenate(self._bu)
-        self._bu = [out]
-        return out
-
-    def work(self, io: WorkIo):
-        o = self.output.slice()
-        p, finished = self.exec(o)
-        self.output.produce(p)
-        if finished:
-            io.finished = True
-
 
 WLAN_BURST = np.dtype([("index", np.uint64), ("len", np.uint64)], align=True)                   # b2s_wlan_burst
 
 
-class WlanTransmitter(Block, Handle):
+class WlanTransmitter(_Transmitter):
     """The WLAN transmit chain of examples/wlan/src/bin/tx.rs:44-66 (Mac -> Encoder -> Mapper -> Fft(64, Inverse,
     shift, sqrt(1/52)) -> Prefix) as a device source: no input port, one Complex32 output.  ``push`` is the Mac's
     ``tx`` handler: payloads (bytes or str) at the default MCS, or per-frame MCS numbers (-1: the default), framed and
@@ -1343,12 +1326,12 @@ class WlanTransmitter(Block, Handle):
     frames started so far, a cumulative WLAN_BURST array.  Finished once ``finish`` has been called and every queued
     sample has been produced."""
     _destroy = lib.b2s_wlan_tx_destroy
-    in_dtype = None
-    out_dtype = np.complex64
+    _finish, _pending, _exec = lib.b2s_wlan_tx_finish, lib.b2s_wlan_tx_pending, lib.b2s_wlan_tx_exec
+    _reset, _drain, _record = lib.b2s_wlan_tx_reset, lib.b2s_wlan_tx_drain_bursts, WLAN_BURST
 
     def __init__(self, src_mac, dst_mac, bss_mac, default_mcs: int, pad_front: int, pad_tail: int,
                  ctx: Optional[Context] = None):
-        self.ctx = ctx or default_context()
+        super().__init__(ctx)
         self.addrs = tuple(bytes(a) for a in (src_mac, dst_mac, bss_mac))
         if any(len(a) != 6 for a in self.addrs):
             raise ValueError("WlanTransmitter: MAC addresses are 6 bytes")
@@ -1356,64 +1339,22 @@ class WlanTransmitter(Block, Handle):
         self._h = C.c_void_p()
         check(lib.b2s_wlan_tx_create(self.ctx.handle, *[C.c_char_p(a) for a in self.addrs], self.default_mcs,
                                      self.pad_front, self.pad_tail, C.byref(self._h)), self.ctx.handle)
-        self.input = None
-        self.output = Writer(self.out_dtype, _ctx_device(self.ctx))
-        self._bu = []
 
     def push(self, *payloads, mcs=None):
         """Queue frames, all or nothing.  ``mcs``: None (every frame at the default MCS, Pmt::Blob) or one MCS
         number per payload, -1 meaning the default (the (data, mcs) pair)."""
-        data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+        data, buf, lens = _payload_batch(payloads)
         n = len(data)
-        lens = (C.c_size_t * max(n, 1))(*[len(d) for d in data])
         m = None
         if mcs is not None:
             if len(mcs) != n:
                 raise ValueError(f"WlanTransmitter.push: {len(mcs)} MCS for {n} payloads")
             m = (C.c_int32 * max(n, 1))(*[int(v) for v in mcs])
-        buf = b"".join(data)
         check(lib.b2s_wlan_tx_push(self._h, C.c_char_p(buf) if buf else None, lens, m, n), self.ctx.handle)
-
-    def finish(self):
-        check(lib.b2s_wlan_tx_finish(self._h), self.ctx.handle)
-
-    def pending(self) -> int:
-        """Queued samples not yet produced."""
-        v = C.c_uint64(0)
-        check(lib.b2s_wlan_tx_pending(self._h, C.byref(v)), self.ctx.handle)
-        return v.value
-
-    def exec(self, o: torch.Tensor) -> tuple[int, bool]:
-        """Write the next samples into the device slice ``o`` (asynchronous) -> (produced, finished)."""
-        p, f = C.c_size_t(0), C.c_int32(0)
-        check(lib.b2s_wlan_tx_exec(self._h, _ptr(o), o.numel(), C.byref(p), C.byref(f)), self.ctx.handle)
-        return p.value, bool(f.value)
 
     def reset(self):
         """Back to the created state: scrambler seed 1, sequence number 0, a zero bit buffer, nothing queued."""
-        check(lib.b2s_wlan_tx_reset(self._h), self.ctx.handle)
-        self._bu = []
-
-    def bursts(self) -> np.ndarray:
-        """Every burst_start tag so far (WLAN_BURST records, in stream order)."""
-        while True:
-            buf = np.zeros(1 << 12, WLAN_BURST)
-            n = C.c_size_t(0)
-            check(lib.b2s_wlan_tx_drain_bursts(self._h, buf.ctypes.data_as(C.c_void_p), buf.size, C.byref(n)),
-                  self.ctx.handle)
-            self._bu.append(buf[:n.value])
-            if n.value < buf.size:
-                break
-        out = np.concatenate(self._bu)
-        self._bu = [out]
-        return out
-
-    def work(self, io: WorkIo):
-        o = self.output.slice()
-        p, finished = self.exec(o)
-        self.output.produce(p)
-        if finished:
-            io.finished = True
+        super().reset()
 
 
 class _FanOut(Block):

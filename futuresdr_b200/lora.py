@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from ._lib import check, lib
-from .blocks import LoraTransmitter
+from .blocks import LoraTransmitter, _payload_batch
 from .context import default_context
 
 PREAMBLE_LEN = 8                         # default_values.rs:7
@@ -151,23 +151,16 @@ def encode(payloads, sf, code_rate, has_crc, ldro_enabled, implicit_header, ctx=
     """Encoder::encode of each payload, as one batch on the device: a list of device tensors, one per payload, of its
     u16 symbols held in torch.int16 (``.cpu().numpy().view(np.uint16)`` reads them back)."""
     ctx = ctx or default_context()
-    data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+    data, buf, lens = _payload_batch(payloads)
     counts = [symbol_count(sf, code_rate, has_crc, ldro_enabled, implicit_header, len(d)) for d in data]
     dev = torch.device("cuda", ctx.device)
-    buf = b"".join(data)
-    d_pay = torch.frombuffer(bytearray(buf), dtype=torch.uint8).to(dev) if buf else torch.zeros(1, dtype=torch.uint8,
-                                                                                              device=dev)
+    d_pay = torch.frombuffer(bytearray(buf or b"\0"), dtype=torch.uint8).to(dev)     # a valid pointer when empty
     d_sym = torch.zeros(max(sum(counts), 1), dtype=torch.int16, device=dev)
-    lens = (C.c_size_t * max(len(data), 1))(*[len(d) for d in data])
     n = C.c_size_t(0)
     check(lib.b2s_lora_encode(ctx.handle, int(sf), int(code_rate), int(has_crc), int(ldro_enabled),
                               int(implicit_header), C.c_void_p(d_pay.data_ptr()), lens, len(data),
                               C.c_void_p(d_sym.data_ptr()), d_sym.numel(), C.byref(n)), ctx.handle)
-    out, o = [], 0
-    for c in counts:
-        out.append(d_sym[o:o + c])
-        o += c
-    return out
+    return list(d_sym[:sum(counts)].split(counts))
 
 
 def transmitter(fg, bw=Bandwidth.BW125, sf=SpreadingFactor.SF7, code_rate=CodeRate.CR_4_5, has_crc=HAS_CRC,

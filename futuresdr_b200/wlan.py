@@ -13,7 +13,7 @@ from dataclasses import dataclass
 import torch
 
 from ._lib import WLAN_MAX_PAYLOAD, WLAN_MAX_PSDU, check, lib  # noqa: F401
-from .blocks import WlanTransmitter
+from .blocks import WlanTransmitter, _payload_batch
 from .context import default_context
 
 PAD_FRONT = 5000                          # bin/tx.rs:40
@@ -96,7 +96,7 @@ def encode(payloads, mcs, src_mac=SRC_MAC, dst_mac=DST_MAC, bss_mac=BSS_MAC, seq
     per payload; frame i has sequence number ``sequence_number + i`` and scrambler seed ``scrambler_seed + i``, both
     wrapping as the reference's do."""
     ctx = ctx or default_context()
-    data = [p.encode() if isinstance(p, str) else bytes(p) for p in payloads]
+    data, buf, lens = _payload_batch(payloads)
     n = len(data)
     ms = [int(mcs)] * n if isinstance(mcs, (int, enum.IntEnum)) else [int(m) for m in mcs]
     if len(ms) != n:
@@ -104,22 +104,15 @@ def encode(payloads, mcs, src_mac=SRC_MAC, dst_mac=DST_MAC, bss_mac=BSS_MAC, seq
     rows = [1 + FrameParam.new(m, len(d) + 28).n_symbols if len(d) <= WLAN_MAX_PAYLOAD else 0
             for m, d in zip(ms, data)]
     dev = torch.device("cuda", ctx.device)
-    buf = b"".join(data)
-    d_pay = torch.frombuffer(bytearray(buf), dtype=torch.uint8).to(dev) if buf else torch.zeros(1, dtype=torch.uint8,
-                                                                                              device=dev)
+    d_pay = torch.frombuffer(bytearray(buf or b"\0"), dtype=torch.uint8).to(dev)     # a valid pointer when empty
     d_sym = torch.zeros(max(sum(rows), 1), 48, dtype=torch.uint8, device=dev)
-    lens = (C.c_size_t * max(n, 1))(*[len(d) for d in data])
     mc = (C.c_int32 * max(n, 1))(*ms)
     got = C.c_size_t(0)
     addrs = [C.c_char_p(bytes(a)) for a in (src_mac, dst_mac, bss_mac)]
     check(lib.b2s_wlan_encode(ctx.handle, *addrs, int(sequence_number), int(scrambler_seed),
                               C.c_void_p(d_pay.data_ptr()), lens, mc, n, C.c_void_p(d_sym.data_ptr()),
                               d_sym.shape[0], C.byref(got)), ctx.handle)
-    out, o = [], 0
-    for r in rows:
-        out.append(d_sym[o:o + r])
-        o += r
-    return out
+    return list(d_sym[:sum(rows)].split(rows))
 
 
 def transmitter(fg, default_mcs=Mcs.QPSK_1_2, src_mac=SRC_MAC, dst_mac=DST_MAC, bss_mac=BSS_MAC,

@@ -712,6 +712,22 @@ private:
     const Instance &inst_; size_t max_calls_; Handle<b2s_boxavg, b2s_boxavg_destroy> h_;
 };
 
+// Every record a b2s_*_drain_* function hands out for the block h, in stream order: it drains until a short read.
+// Draining synchronises.
+template <typename H, typename E>
+std::vector<E> drain_records(int32_t (*fn)(H *, E *, size_t, size_t *), H *h, const b2s_ctx *ctx) {
+    constexpr size_t chunk = 4096;
+    std::vector<E> out;
+    for (;;) {
+        const size_t k = out.size();
+        out.resize(k + chunk);
+        size_t n = 0;
+        check(fn(h, out.data() + k, chunk, &n), ctx);
+        out.resize(k + n);
+        if (n < chunk) return out;
+    }
+}
+
 // ≙ the ADS-B receiver's PreambleDetector -> Demodulator -> Decoder::check_crc (examples/adsb/src/preamble_detector.rs
 // :65-146, demodulator.rs:49-113, decoder.rs:57-73) as one block (b2s_adsb_*).  Three f32 stream inputs, no stream
 // output; the detector's tags and the demodulated frames are drained from the block.  work() runs one exec and
@@ -741,25 +757,12 @@ public:
         if (done) io.finished = true;
     }
     // every packet / detection since the last drain, in stream order (synchronises)
-    std::vector<b2s_adsb_packet> drain_packets() {
-        return drain<b2s_adsb_packet>(b2s_adsb_drain_packets);
-    }
+    std::vector<b2s_adsb_packet> drain_packets() { return drain_records(b2s_adsb_drain_packets, h_.get(), inst_.get()); }
     std::vector<b2s_adsb_detection> drain_detections() {
-        return drain<b2s_adsb_detection>(b2s_adsb_drain_detections);
+        return drain_records(b2s_adsb_drain_detections, h_.get(), inst_.get());
     }
     Reader<float> in_samples, in_nf, in_preamble_cor;
 private:
-    template <typename E, typename F> std::vector<E> drain(F fn) {
-        std::vector<E> out;
-        for (;;) {
-            const size_t k = out.size();
-            out.resize(k + 4096);
-            size_t n = 0;
-            check(fn(h_.get(), out.data() + k, 4096, &n), inst_.get());
-            out.resize(k + n);
-            if (n < 4096) return out;
-        }
-    }
     const Instance &inst_; Handle<b2s_adsb, b2s_adsb_destroy> h_;
 };
 
@@ -816,17 +819,7 @@ public:
         if (input.finished()) io.finished = true;
     }
     // every frame since the last drain, in stream order (synchronises)
-    std::vector<b2s_zigbee_frame> drain_frames() {
-        std::vector<b2s_zigbee_frame> out;
-        for (;;) {
-            const size_t k = out.size();
-            out.resize(k + 1024);
-            size_t n = 0;
-            check(b2s_zigbee_drain_frames(h_.get(), out.data() + k, 1024, &n), inst_.get());
-            out.resize(k + n);
-            if (n < 1024) return out;
-        }
-    }
+    std::vector<b2s_zigbee_frame> drain_frames() { return drain_records(b2s_zigbee_drain_frames, h_.get(), inst_.get()); }
     Reader<float> input;
 private:
     const Instance &inst_; Handle<b2s_zigbee, b2s_zigbee_destroy> h_;
@@ -851,17 +844,7 @@ public:
         if (input.finished()) io.finished = true;
     }
     // every code since the last drain, in stream order (synchronises)
-    std::vector<b2s_keyfob_code> drain_codes() {
-        std::vector<b2s_keyfob_code> out;
-        for (;;) {
-            const size_t k = out.size();
-            out.resize(k + 1024);
-            size_t n = 0;
-            check(b2s_keyfob_drain_codes(h_.get(), out.data() + k, 1024, &n), inst_.get());
-            out.resize(k + n);
-            if (n < 1024) return out;
-        }
-    }
+    std::vector<b2s_keyfob_code> drain_codes() { return drain_records(b2s_keyfob_drain_codes, h_.get(), inst_.get()); }
     Reader<uint8_t> input;
 private:
     const Instance &inst_; Handle<b2s_keyfob, b2s_keyfob_destroy> h_;
@@ -878,6 +861,13 @@ inline size_t lora_encode(const Instance &inst, int sf, int code_rate, bool has_
     return n;
 }
 
+// A batch of payloads as the push calls take it: (the bytes back to back, one length per payload)
+inline std::pair<std::vector<uint8_t>, std::vector<size_t>> pack_payloads(const std::vector<std::vector<uint8_t>> &payloads) {
+    std::pair<std::vector<uint8_t>, std::vector<size_t>> b;
+    for (const auto &p : payloads) { b.first.insert(b.first.end(), p.begin(), p.end()); b.second.push_back(p.size()); }
+    return b;
+}
+
 // ≙ examples/lora/src/transmitter.rs:12-168: a source of Complex<f32> (std::complex<float>) samples; push is the msg
 // handler, set_sync_word the synch_word handler (expanded symbols), finish its Pmt::Finished
 class LoraTransmitter {
@@ -889,9 +879,7 @@ public:
                                  sync_symbols.data(), preamble_len, pad, out_ptr(h_)), inst.get());
     }
     void push(const std::vector<std::vector<uint8_t>> &payloads) {
-        std::vector<uint8_t> bytes;
-        std::vector<size_t> lens;
-        for (const auto &p : payloads) { bytes.insert(bytes.end(), p.begin(), p.end()); lens.push_back(p.size()); }
+        const auto [bytes, lens] = pack_payloads(payloads);
         check(b2s_lora_tx_push(h_.get(), bytes.data(), lens.data(), lens.size()), inst_.get());
     }
     void set_sync_word(uint32_t s0, uint32_t s1) { check(b2s_lora_tx_set_sync_word(h_.get(), s0, s1), inst_.get()); }
@@ -915,17 +903,7 @@ public:
         if (f) io.finished = true;
     }
     // the burst_start tags since the last drain, in stream order
-    std::vector<b2s_lora_burst> drain_bursts() {
-        std::vector<b2s_lora_burst> out;
-        for (;;) {
-            const size_t k = out.size();
-            out.resize(k + 1024);
-            size_t n = 0;
-            check(b2s_lora_tx_drain_bursts(h_.get(), out.data() + k, 1024, &n), inst_.get());
-            out.resize(k + n);
-            if (n < 1024) return out;
-        }
-    }
+    std::vector<b2s_lora_burst> drain_bursts() { return drain_records(b2s_lora_tx_drain_bursts, h_.get(), inst_.get()); }
     Writer<std::complex<float>> output;
 private:
     const Instance &inst_; Handle<b2s_lora_tx, b2s_lora_tx_destroy> h_;
@@ -958,9 +936,7 @@ public:
     // mcs empty: every frame at the default MCS; otherwise one per payload, -1 meaning the default
     void push(const std::vector<std::vector<uint8_t>> &payloads, const std::vector<int32_t> &mcs = {}) {
         if (!mcs.empty() && mcs.size() != payloads.size()) throw Error(B2S_EINVAL, "wlan push: one MCS per payload");
-        std::vector<uint8_t> bytes;
-        std::vector<size_t> lens;
-        for (const auto &p : payloads) { bytes.insert(bytes.end(), p.begin(), p.end()); lens.push_back(p.size()); }
+        const auto [bytes, lens] = pack_payloads(payloads);
         check(b2s_wlan_tx_push(h_.get(), bytes.data(), lens.data(), mcs.empty() ? nullptr : mcs.data(), lens.size()),
               inst_.get());
     }
@@ -984,17 +960,7 @@ public:
         if (f) io.finished = true;
     }
     // the burst_start tags since the last drain, in stream order
-    std::vector<b2s_wlan_burst> drain_bursts() {
-        std::vector<b2s_wlan_burst> out;
-        for (;;) {
-            const size_t k = out.size();
-            out.resize(k + 1024);
-            size_t n = 0;
-            check(b2s_wlan_tx_drain_bursts(h_.get(), out.data() + k, 1024, &n), inst_.get());
-            out.resize(k + n);
-            if (n < 1024) return out;
-        }
-    }
+    std::vector<b2s_wlan_burst> drain_bursts() { return drain_records(b2s_wlan_tx_drain_bursts, h_.get(), inst_.get()); }
     Writer<std::complex<float>> output;
 private:
     const Instance &inst_; Handle<b2s_wlan_tx, b2s_wlan_tx_destroy> h_;
