@@ -8,7 +8,10 @@
 // inverse transform all happen in ONE kernel with the block resident in (padded) shared memory
 // -- HBM sees 8 B in (x NF/V overlap, mostly L2 hits) + 8 B out per sample, instead of the
 // 4*N FLOP per sample of the direct form (4096 FLOP/sample at 1024 taps).  Radix-16 Stockham passes from fft_common.cuh; H is computed in f64 on the host.
-// Parity: |err| <~ 1e-6 * rms(y) * sqrt(log2 NF), far inside 1e-5 * ||taps||_1 * max|x|.
+// Parity: the error follows the block's INPUT, not y: |err| <= 8 * 2^-24 * log2(NF) * (||taps||_2 * rms(x_block) +
+// rms(circular output of the block)) -- a full-scale stopband tone gets an error near rms(y) -- and a NaN/Inf input
+// poisons every output of each block that reads it (include/b200sdr.h, B2S_ALGO_FFT; tests/test_gpu_fir_fft_numerics.py).
+// Most of the error is the Stockham core's product-tree twiddles (fft_common.cuh): about 3x what exact twiddles give.
 #include <cmath>
 
 #include "fft_common.cuh"

@@ -70,7 +70,21 @@ typedef enum {
                           * outputs are unaffected and no finite output is ever wrong.  f32 DENORMAL samples may count as
                           * zero (tensor-core operands may be flushed to zero).  Streams that may carry
                           * non-finite samples and need the reference's exact propagation: use B2S_ALGO_DIRECT. */
-    B2S_ALGO_FFT    = 3, /* overlap-save FFT convolution (c32 samples, 64..2049 taps, decim == 1)  */
+    B2S_ALGO_FFT    = 3, /* overlap-save FFT convolution (c32 samples, 64..2049 taps, decim == 1).
+                          * Numerics: block b of a call reads the NF = 4096 inputs x_b = x[s, s+NF) (zeros past the end),
+                          * s = b*V, and writes outputs [s, s+V), V = NF-(ntaps-1), through two single-precision FFTs and
+                          * H = FFT(taps)/NF rounded to f32.  Error: |y_k - exact| <= 8 * 2^-24 * log2(NF) *
+                          * (||taps||_2 * rms(x_b) + rms(c_b)), c_b the block's circular output (rms <= max|G| rms(x_b)):
+                          * it follows the block's INPUT, not y -- a stopband output carries an input-sized error.
+                          * Non-finite input: a NaN/Inf sample at index i makes every output of every block whose window
+                          * holds i non-finite (all inside [i-NF+1, i+NF-ntaps], a superset of the reference's
+                          * [i-ntaps+1, i]; the last block reads its whole window, also samples past what its outputs
+                          * need); all other outputs are unaffected.  Finite range: outputs are finite while
+                          * 4096 * max|x| * max(1, ||taps||_1) < 2^128; past it each output is within the bound or
+                          * non-finite, never a wrong finite value.  Tiny input: below max|x| ~ 2^-100 the products
+                          * X.H reach the subnormal range and the bound holds plus ||taps||_1 * 2^-126, down to
+                          * denormal-only input.  Streams that need the reference's exact propagation: use
+                          * B2S_ALGO_DIRECT. */
     B2S_ALGO_SCAN   = 4  /* IIR only (b2s_iir_set_algo): single-pass chained scan, see b2s_iir below;
                           * b2s_fir_set_algo rejects it */
 } b2s_algo;
