@@ -7,7 +7,7 @@ PolyphaseResamplingFir}, futuredsp::{firdes::{hilbert, lowpass}, windows::hammin
 FirBuilder, Fft, Apply, PfbArbResampler, SignalSource, SignalSourceBuilder, FixedPointPhase, Head,
 Combine, Split, Delay, StreamDuplicator, StreamDeinterleaver}, the WLAN / M17 receivers' MovingAverage, the ZigBee
 receiver's ClockRecoveryMm and Decoder, the keyfob receiver's Decoder, ApplyNM and the SSB example's oscillator mixers,
-the LoRa Transmitter, the WLAN transmit chain,
+the LoRa Transmitter, the WLAN and ZigBee transmit chains,
 runtime::mocker::Mocker) so the parity tests read like the reference's own tests.
 Importing this package loads libb200sdr.so and raises if it is missing: no CPU fallback.
 """
@@ -24,7 +24,7 @@ from .blocks import (  # noqa: F401
     FixedPointPhase, Head, SignalSource, SignalSourceBuilder, SignalWave,
     Combine, CombineOp, Delay, Split, SplitOp, StreamDeinterleaver, StreamDuplicator, MovingAverage,
     AdsbDemod, ClockRecoveryMm, ZigbeeDecoder, KeyfobDecoder, KEYFOB_CODE, ApplyNM, ApplyNMOp, Mixer, MixOp,
-    LoraTransmitter, LORA_BURST, WlanTransmitter, WLAN_BURST,
+    LoraTransmitter, LORA_BURST, WlanTransmitter, WLAN_BURST, ZigbeeTransmitter, ZIGBEE_BURST,
 )
 from . import adsb, firdes, keyfob, lora, ssb, windows, wlan, zigbee  # noqa: F401
 # host edges (VectorSource/Sink, FileSource/Sink, H2D/D2H ring, run_chain, Flowgraph): futuresdr_b200.edges

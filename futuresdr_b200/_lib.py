@@ -29,6 +29,8 @@ FANOUT_MAX_OUTPUTS = 256
 LORA_MAX_PAYLOAD = 255
 WLAN_MAX_PAYLOAD = 1500
 WLAN_MAX_PSDU = 1528
+ZIGBEE_MAX_PAYLOAD = 116
+ZIGBEE_PADDING = 40000
 
 _vp, _sz, _i32, _f32 = C.c_void_p, C.c_size_t, C.c_int32, C.c_float
 _szp, _i32p, _vpp, _f32p = C.POINTER(C.c_size_t), C.POINTER(C.c_int32), C.POINTER(C.c_void_p), C.POINTER(C.c_float)
@@ -199,6 +201,14 @@ SIGNATURES = {
     "b2s_wlan_tx_pending": (_i32, [_vp, C.POINTER(C.c_uint64)]),
     "b2s_wlan_tx_exec": (_i32, [_vp, _vp, _sz, _szp, _i32p]),
     "b2s_wlan_tx_drain_bursts": (_i32, [_vp, _vp, _sz, _szp]),
+    "b2s_zigbee_tx_create": (_i32, [_vp, _sz, _vpp]),
+    "b2s_zigbee_tx_destroy": (None, [_vp]),
+    "b2s_zigbee_tx_reset": (_i32, [_vp]),
+    "b2s_zigbee_tx_push": (_i32, [_vp, _vp, _szp, _sz, _szp]),
+    "b2s_zigbee_tx_finish": (_i32, [_vp]),
+    "b2s_zigbee_tx_pending": (_i32, [_vp, C.POINTER(C.c_uint64)]),
+    "b2s_zigbee_tx_exec": (_i32, [_vp, _vp, _sz, _szp, _i32p]),
+    "b2s_zigbee_tx_drain_bursts": (_i32, [_vp, _vp, _sz, _szp]),
 }
 
 

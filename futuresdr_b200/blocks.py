@@ -1357,6 +1357,45 @@ class WlanTransmitter(_Transmitter):
         super().reset()
 
 
+ZIGBEE_BURST = np.dtype([("index", np.uint64), ("len", np.uint64)], align=True)               # b2s_zigbee_burst
+
+
+class ZigbeeTransmitter(_Transmitter):
+    """The ZigBee transmit chain of examples/zigbee/src/bin/tx.rs:37-56 (Mac -> modulator -> IqDelay) as a device
+    source: no input port, one Complex32 output.  ``push`` is the Mac's ``tx`` handler: each bytes-like payload is
+    framed on the host and queued; one over 116 bytes is dropped on its own, as the Mac drops it, and ``push`` returns
+    how many were dropped.  ``work`` fills the output slice with the next samples of the concatenated frames, each
+    with ``pad`` zeros before and after it; the stream is bit-identical to the reference's for every slicing.
+    ``bursts()`` returns the burst_start tags (stream index, length) of the frames started so far, a cumulative
+    ZIGBEE_BURST array.  Finished once ``finish`` has been called and every queued sample has been produced."""
+    _destroy = lib.b2s_zigbee_tx_destroy
+    _finish, _pending, _exec = lib.b2s_zigbee_tx_finish, lib.b2s_zigbee_tx_pending, lib.b2s_zigbee_tx_exec
+    _reset, _drain, _record = lib.b2s_zigbee_tx_reset, lib.b2s_zigbee_tx_drain_bursts, ZIGBEE_BURST
+
+    def __init__(self, pad: int = _lib.ZIGBEE_PADDING, ctx: Optional[Context] = None):
+        super().__init__(ctx)
+        self.pad = int(pad)
+        if self.pad < 0:
+            raise ValueError("ZigbeeTransmitter: pad must not be negative")
+        self._h = C.c_void_p()
+        check(lib.b2s_zigbee_tx_create(self.ctx.handle, self.pad, C.byref(self._h)), self.ctx.handle)
+
+    def push(self, *payloads) -> int:
+        """Queue frames (Pmt::Blob payloads: bytes-like objects; a str raises TypeError) -> the number dropped for
+        being over 116 bytes."""
+        if any(isinstance(p, str) for p in payloads):
+            raise TypeError("ZigbeeTransmitter.push: payloads are bytes-like, not str")
+        data, buf, lens = _payload_batch([bytes(memoryview(p)) for p in payloads])
+        dropped = C.c_size_t(0)
+        check(lib.b2s_zigbee_tx_push(self._h, C.c_char_p(buf) if buf else None, lens, len(data), C.byref(dropped)),
+              self.ctx.handle)
+        return dropped.value
+
+    def reset(self):
+        """Back to the created state: sequence number 0, nothing queued."""
+        super().reset()
+
+
 class _FanOut(Block):
     """One input, ``n`` outputs in the list attribute ``self._list``, moved by one b2s_fanout_exec launch."""
     _list = ""

@@ -1,5 +1,6 @@
-// tx_common.cuh -- the host-side bookkeeping the device transmitters share (lora.cu, wlan.cu): device rings that grow
-// on push, and the queue of frames not yet fully produced with its burst_start records.
+// tx_common.cuh -- what the device transmitters share (lora.cu, wlan.cu, zigbee_tx.cu): device rings that grow on push,
+// the queue of frames not yet fully produced with its burst_start records, and the exec kernels' frame search and
+// streaming stores.
 #pragma once
 
 #include <algorithm>
@@ -104,3 +105,40 @@ template <typename Burst> struct TxQueue {
         return k;
     }
 };
+
+// The last of the n frame records frames[(f_lo + i) & mask], i < n, ascending in .start, whose start is at or before t:
+// a 32-ary search by one whole warp; every lane returns the index i.
+template <typename Rec>
+__device__ __forceinline__ unsigned long long tx_first_frame(const Rec *frames, unsigned long long mask,
+                                                             unsigned long long f_lo, unsigned long long n,
+                                                             unsigned long long t) {
+    const unsigned lane = threadIdx.x & 31;
+    unsigned long long lo = 0;
+    while (n > 1) {
+        const unsigned long long step = (n + 31) / 32, i = lo + lane * step;
+        const bool le = lane * step < n && frames[(f_lo + i) & mask].start <= t;
+        const unsigned bal = __ballot_sync(~0u, le);
+        const unsigned last = bal ? 31 - __clz(bal) : 0;
+        lo += last * step;
+        n = min(step, n - last * step);
+    }
+    return lo;
+}
+
+// dst[i] = f(i) for i in [i0, i1) by the CTA's Threads threads, two samples per 16-byte streaming store where dst + i
+// is 16-byte aligned (the output is only 8-byte aligned)
+template <int Threads, typename I, typename F>
+__device__ __forceinline__ void store_range(float2 *dst, I i0, I i1, F f) {
+    if (i0 >= i1) return;
+    if ((reinterpret_cast<uintptr_t>(dst + i0) & 15) != 0) {
+        if (threadIdx.x == 0) __stcs(dst + i0, f(i0));
+        ++i0;
+    }
+    const I n2 = (i1 - i0) / 2;
+    for (I p = threadIdx.x; p < n2; p += Threads) {
+        const I i = i0 + 2 * p;
+        const float2 v0 = f(i), v1 = f(i + 1);
+        __stcs(reinterpret_cast<float4 *>(dst + i), make_float4(v0.x, v0.y, v1.x, v1.y));
+    }
+    if (((i1 - i0) & 1) && threadIdx.x == Threads - 1) __stcs(dst + i1 - 1, f(i1 - 1));
+}

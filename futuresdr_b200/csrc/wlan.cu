@@ -405,43 +405,16 @@ __device__ __forceinline__ float2 window(float2 a, float2 b) {     // 0.5 * (a +
     return make_float2(__fmul_rn(0.5f, __fadd_rn(a.x, b.x)), __fmul_rn(0.5f, __fadd_rn(a.y, b.y)));
 }
 
-// dst[i] = f(i) for i in [i0, i1) by the CTA's threads, two samples per 16-byte streaming store where dst + i is
-// 16-byte aligned (the output is only 8-byte aligned)
-template <typename I, typename F>
-__device__ __forceinline__ void store_range(float2 *dst, I i0, I i1, F f) {
-    if (i0 >= i1) return;
-    if ((reinterpret_cast<uintptr_t>(dst + i0) & 15) != 0) {
-        if (threadIdx.x == 0) __stcs(dst + i0, f(i0));
-        ++i0;
-    }
-    const I n2 = (i1 - i0) / 2;
-    for (I p = threadIdx.x; p < n2; p += kExecThreads) {
-        const I i = i0 + 2 * p;
-        const float2 v0 = f(i), v1 = f(i + 1);
-        __stcs(reinterpret_cast<float4 *>(dst + i), make_float4(v0.x, v0.y, v1.x, v1.y));
-    }
-    if (((i1 - i0) & 1) && threadIdx.x == kExecThreads - 1) __stcs(dst + i1 - 1, f(i1 - 1));
-}
-
 __global__ void __launch_bounds__(kExecThreads, 5) wlan_exec_kernel(const ExecParams a) {
     __shared__ __align__(16) float2 s_y[kG.fpb * kG.np];
     __shared__ OfdmSym s_rec[kG.fpb];
     __shared__ unsigned long long s_f;
     const unsigned long long t0 = a.pos + (unsigned long long)blockIdx.x * a.tile;
     const unsigned long long t1 = min(t0 + a.tile, a.pos + a.cnt);
-    // the last frame starting at or before t0: a 32-ary search by warp 0 over the records' starts
+    // the last frame starting at or before t0, by warp 0
     if (threadIdx.x < 32) {
-        const int lane = threadIdx.x;
-        unsigned long long lo = 0, n = a.n_frames;
-        while (n > 1) {
-            const unsigned long long step = (n + 31) / 32, i = lo + lane * step;
-            const bool le = lane * step < n && a.frames[(a.f_lo + i) & a.frame_mask].start <= t0;
-            const unsigned bal = __ballot_sync(~0u, le);
-            const unsigned last = bal ? 31 - __clz(bal) : 0;
-            lo += last * step;
-            n = min(step, n - last * step);
-        }
-        if (lane == 0) s_f = lo;
+        const unsigned long long f = tx_first_frame(a.frames, a.frame_mask, a.f_lo, a.n_frames, t0);
+        if (threadIdx.x == 0) s_f = f;
     }
     __syncthreads();
     const int t = threadIdx.x % kG.t, fl = threadIdx.x / kG.t;
@@ -457,8 +430,8 @@ __global__ void __launch_bounds__(kExecThreads, 5) wlan_exec_kernel(const ExecPa
         auto plain = [&](unsigned long long r) {
             return (r >= a.pad_front && r < d0) ? scale06(a.sync[r - a.pad_front]) : make_float2(0.0f, 0.0f);
         };
-        store_range(o, ra, min(rb, sa), plain);
-        store_range(o, max(ra, sb), rb, plain);
+        store_range<kExecThreads>(o, ra, min(rb, sa), plain);
+        store_range<kExecThreads>(o, max(ra, sb), rb, plain);
         const unsigned long long qa = max(ra, sa), qb = min(rb, sb);
         if (qa >= qb) continue;
         const unsigned long long ka = (qa - d0) / 80, kb = (qb - 1 - d0) / 80;   // kb may be len: the tail window
@@ -490,7 +463,7 @@ __global__ void __launch_bounds__(kExecThreads, 5) wlan_exec_kernel(const ExecPa
             const unsigned long long base = d0 + 80 * c0;
             const unsigned u0 = (unsigned)(max(qa, d0 + 80 * kw) - base), u1 = (unsigned)(min(qb, d0 + 80 * (kend + 1)) - base);
             const unsigned last = (unsigned)(len - c0);                // the slot of the tail window sample, if any
-            store_range(o + base, u0, u1, [&](unsigned u) {
+            store_range<kExecThreads>(o + base, u0, u1, [&](unsigned u) {
                 const unsigned slot = u / 80, s = u - 80 * slot;
                 const float2 *y = s_y + slot * kG.np;
                 float2 v;

@@ -742,6 +742,46 @@ int32_t b2s_wlan_tx_pending(const b2s_wlan_tx *p, uint64_t *samples);   /* queue
 int32_t b2s_wlan_tx_exec(b2s_wlan_tx *p, void *d_out, size_t n_out_cap, size_t *produced, int32_t *finished);
 int32_t b2s_wlan_tx_drain_bursts(b2s_wlan_tx *p, b2s_wlan_burst *host, size_t cap, size_t *n);
 
+/* ---- the ZigBee transmitter (≙ examples/zigbee/src/mac.rs:135-252, modulator.rs:4-342 and iq_delay.rs:11-139: the
+ * Mac -> modulator -> IqDelay chain of bin/tx.rs:37-56).  A payload of n bytes (at most B2S_ZIGBEE_MAX_PAYLOAD)
+ * becomes the Mac's frame of n + 16 bytes: 00 00 00 a7, n + 11, 41 88, the sequence number, aa 1a ff ff 44 33, the
+ * payload and the FCS (calc_crc over bytes 5 .. 14 + n, little endian).  The modulator makes 128 samples of each byte
+ * (16 DSSS chips per nibble, low nibble first, each chip 4 samples of SHAPE, in f32); IqDelay delays Q by two
+ * samples and pads each frame with pad zeros before and after it.  A frame has 2 pad + 128 (n + 16) + 2 samples.
+ * There is no FEC: push frames the payloads on the host and copies their bytes to the device.
+ * Transmitter: a source of Complex<f32> samples, the concatenation of IqDelay's frames, bit-identical to the reference
+ * (the sign of every zero included) under any slicing of the stream.
+ *   create:       pad is IqDelay's PADDING (B2S_ZIGBEE_PADDING in the reference); above 2^32 - 1 is B2S_EINVAL.
+ *   push:         the Mac's `tx` handler for n_frames payloads (HOST memory, back to back).  A payload above
+ *                 B2S_ZIGBEE_MAX_PAYLOAD is dropped on its own, as the Mac drops it, and the others are queued in order;
+ *                 *n_dropped counts the dropped ones.  The sequence number (a u8) advances per queued frame only.  Frames
+ *                 are never dropped for queue length (the Mac's 128-frame bound depends on its scheduler).  May wait
+ *                 for the context's stream when a device buffer grows.
+ *   exec:         writes the next min(n_out_cap, pending) samples to d_out (8-byte aligned); one exec may span several
+ *                 frames.  Stream-ordered, never synchronises.  *finished is set once finish has been called and every
+ *                 queued sample has been produced, the last frame's tail pad included (the reference's graph never
+ *                 finishes).
+ *   drain_bursts: the burst_start tags (iq_delay.rs:112-118) of the frames whose first sample has been produced, in
+ *                 stream order, up to cap of them (*n); they are removed.  A tag sits on the frame's first front-pad
+ *                 sample and its value is the frame's length.
+ *   reset:        the created state: sequence number 0, no queue, position 0, no finish. */
+#define B2S_ZIGBEE_MAX_PAYLOAD 116
+#define B2S_ZIGBEE_PADDING     40000
+typedef struct {
+    uint64_t index;       /* stream index of the frame's first sample */
+    uint64_t len;         /* the frame's samples */
+} b2s_zigbee_burst;
+typedef struct b2s_zigbee_tx b2s_zigbee_tx;
+int32_t b2s_zigbee_tx_create(b2s_ctx *ctx, size_t pad, b2s_zigbee_tx **out);
+void    b2s_zigbee_tx_destroy(b2s_zigbee_tx *p);
+int32_t b2s_zigbee_tx_reset(b2s_zigbee_tx *p);
+int32_t b2s_zigbee_tx_push(b2s_zigbee_tx *p, const uint8_t *payloads, const size_t *lengths, size_t n_frames,
+                           size_t *n_dropped);
+int32_t b2s_zigbee_tx_finish(b2s_zigbee_tx *p);
+int32_t b2s_zigbee_tx_pending(const b2s_zigbee_tx *p, uint64_t *samples);   /* queued samples not yet produced */
+int32_t b2s_zigbee_tx_exec(b2s_zigbee_tx *p, void *d_out, size_t n_out_cap, size_t *produced, int32_t *finished);
+int32_t b2s_zigbee_tx_drain_bursts(b2s_zigbee_tx *p, b2s_zigbee_burst *host, size_t cap, size_t *n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -966,6 +966,48 @@ private:
     const Instance &inst_; Handle<b2s_wlan_tx, b2s_wlan_tx_destroy> h_;
 };
 
+// ≙ examples/zigbee/src/bin/tx.rs:37-56 without the radio sink (Mac -> modulator -> IqDelay): a source of Complex<f32>
+// (std::complex<float>) samples; push is the Mac's tx handler and returns how many payloads it dropped for being over
+// B2S_ZIGBEE_MAX_PAYLOAD bytes; finish ends the stream after the last frame's tail pad
+class ZigbeeTransmitter {
+public:
+    explicit ZigbeeTransmitter(const Instance &inst, size_t pad = B2S_ZIGBEE_PADDING) : output(inst), inst_(inst) {
+        check(b2s_zigbee_tx_create(inst.get(), pad, out_ptr(h_)), inst.get());
+    }
+    size_t push(const std::vector<std::vector<uint8_t>> &payloads) {
+        const auto [bytes, lens] = pack_payloads(payloads);
+        size_t dropped = 0;
+        check(b2s_zigbee_tx_push(h_.get(), bytes.data(), lens.data(), lens.size(), &dropped), inst_.get());
+        return dropped;
+    }
+    void finish() { check(b2s_zigbee_tx_finish(h_.get()), inst_.get()); }
+    void reset() { check(b2s_zigbee_tx_reset(h_.get()), inst_.get()); }
+    uint64_t pending() const {
+        uint64_t v = 0;
+        check(b2s_zigbee_tx_pending(h_.get(), &v), inst_.get());
+        return v;
+    }
+    // (produced, finished) of one exec into a device slice
+    std::pair<size_t, bool> exec(std::complex<float> *d_out, size_t cap) {
+        size_t p = 0;
+        int32_t f = 0;
+        check(b2s_zigbee_tx_exec(h_.get(), d_out, cap, &p, &f), inst_.get());
+        return {p, f != 0};
+    }
+    void work(WorkIo &io) {
+        auto [p, f] = exec(output.slice(), output.capacity());
+        output.produce(p);
+        if (f) io.finished = true;
+    }
+    // the burst_start tags since the last drain, in stream order
+    std::vector<b2s_zigbee_burst> drain_bursts() {
+        return drain_records(b2s_zigbee_tx_drain_bursts, h_.get(), inst_.get());
+    }
+    Writer<std::complex<float>> output;
+private:
+    const Instance &inst_; Handle<b2s_zigbee_tx, b2s_zigbee_tx_destroy> h_;
+};
+
 // One input, N outputs moved by one b2s_fanout_exec launch (T: 4- or 8-byte items)
 template <typename T, int32_t Deinterleave> class FanOut {
     static_assert(sizeof(T) == 4 || sizeof(T) == 8, "stream fan-out: 4- or 8-byte items");
