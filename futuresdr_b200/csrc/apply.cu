@@ -24,16 +24,37 @@ namespace {
 
 // arg(v * conj(last)) with num_complex's Mul: re = a.re*b.re - a.im*b.im, im = a.re*b.im + a.im*b.re,
 // b = conj(last) = (lr, -li).  __fmul_rn/__fsub_rn keep the products un-fused like the Rust code.
-// atan2 for finite inputs in ~25 instructions (CUDA's atan2f is ~60 on its fast path and made the
-// demodulator issue-bound at half the HBM roofline): a = min/max of the magnitudes (MUFU.RCP based
-// division), atan(a) = a * P(a^2) with a degree-8 minimax P (max error 1.1e-7 rad on [0,1] in f32 Horner
-// form, coefficients fitted in scripts -- see DESIGN.md 4.6), then the octant is unfolded with the SIGN
-// BITS so that +-0 behave like libm: atan2(+0,-0) = pi, atan2(0,+0) = 0 (the demodulator's first
-// sample multiplies by conj(0)).  Total error < 3e-7 rad; parity bar 1e-5*pi (tests/test_gpu_blocks.py).
-__device__ __forceinline__ float atan2_finite(float y, float x) {
+// atan2 in ~30 instructions (CUDA's atan2f is ~60 on its fast path and made the demodulator issue-bound
+// at half the HBM roofline): a = min/max of the magnitudes (MUFU.RCP based division), atan(a) = a * P(a^2)
+// with a degree-8 minimax P (max error 1.1e-7 rad on [0,1] in f32 Horner form, coefficients fitted in
+// scripts -- see DESIGN.md 4.6), then the octant is unfolded with the SIGN BITS so that +-0 behave like
+// libm: atan2(+0,-0) = pi, atan2(0,+0) = 0 (the demodulator's first sample multiplies by conj(0)).
+// Error <= 4e-7 rad against atan2 in float64 (measured max 3.0e-7 on an H100;
+// tests/test_gpu_apply_numerics.py derives the bound).  The special values are libm's: (+-inf, +-inf)
+// gives +-pi/4 or +-3pi/4, (+-inf, finite) an axis, and a NaN part NaN.  Three changes keep them (six
+// instructions in all), and none changes an output whose parts are finite and at most 2^126:
+//   * __fdividef (div.approx.f32) returns 0 for divisors in (2^126, 2^128), so such a pair is scaled
+//     by 1/4 first (exact for the divisor; a dividend it pushes into the denormals has a zero quotient);
+//   * inf/inf is NaN, so two infinite parts take the quotient 1;
+//   * max.NaN / min.NaN keep a NaN part where fmaxf / fminf drop it, and the quotient carries it through.
+__device__ __forceinline__ float max_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+__device__ __forceinline__ float min_nan(float a, float b) {
+    float r;
+    asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+
+__device__ __forceinline__ float atan2_poly(float y, float x) {
     const float ax = fabsf(x), ay = fabsf(y);
-    const float mx = fmaxf(ax, ay), mn = fminf(ax, ay);
-    const float a = mx > 0.0f ? __fdividef(mn, mx) : 0.0f;
+    const float mx0 = max_nan(ax, ay), mn0 = min_nan(ax, ay);
+    const bool big = mx0 > 0x1p126f;
+    const float mx = big ? 0.25f * mx0 : mx0, mn = big ? 0.25f * mn0 : mn0;
+    const float q = mx <= 0.0f ? 0.0f : __fdividef(mn, mx);
+    const float a = mn0 == INFINITY ? 1.0f : q;
     const float s = a * a;
     float p = 0.0029408063273876905f;
     p = fmaf(p, s, -0.0164317823946476f);
@@ -54,13 +75,16 @@ __device__ __forceinline__ float quad_demod_one(float2 v, float2 last) {
     const float cr = last.x, ci = -last.y;
     const float pr = __fsub_rn(__fmul_rn(v.x, cr), __fmul_rn(v.y, ci));
     const float pi = __fadd_rn(__fmul_rn(v.x, ci), __fmul_rn(v.y, cr));
-    return atan2_finite(pi, pr);
+    return atan2_poly(pi, pr);
 }
 
 template <int OP>
 __global__ void apply_kernel(const void *__restrict__ vin, void *__restrict__ vout, long long n, float param,
                              const float2 *__restrict__ carry) {
     const long long stride = (long long)gridDim.x * blockDim.x;
+    // four items in flight per thread; nvcc picks 4 by itself except for the demodulators, whose inline asm
+    // (max_nan / min_nan) its unroller prices too high
+#pragma unroll 4
     for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
         if constexpr (OP == B2S_OP_SCALE_F32) {
             ((float *)vout)[j] = ((const float *)vin)[j] * param;

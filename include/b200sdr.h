@@ -243,8 +243,9 @@ void    b2s_apply_destroy(b2s_apply *a);
 int32_t b2s_apply_reset(b2s_apply *a); /* closure state back to its initial value */
 /* m = min(n_in, n_out_cap) items are processed (apply.rs:109), except by B2S_OP_C32_TO_I16_IQ (above).
  * Element-wise ops may run in place (d_in == d_out);
- * the stateful demodulators (B2S_OP_QUAD_DEMOD*) need disjoint slices (B2S_EINVAL otherwise) and FINITE input
- * (their atan2 is a finite-input polynomial: inf/inf gives NaN where libm gives +-pi/4, +-3pi/4). */
+ * the stateful demodulators (B2S_OP_QUAD_DEMOD*) need disjoint slices (B2S_EINVAL otherwise).  Their output is
+ * the arg of the f32 product with libm atan2's special values, within 4e-7 rad: (+-inf, +-inf) gives +-pi/4 or
+ * +-3pi/4, signed zeros give +-0 or +-pi, and a NaN part gives NaN. */
 int32_t b2s_apply_exec(b2s_apply *a, const void *d_in, size_t n_in, void *d_out, size_t n_out_cap,
                        size_t *consumed, size_t *produced);
 
