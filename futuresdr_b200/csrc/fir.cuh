@@ -18,6 +18,8 @@ struct b2s_fir {
     int tc_kblocks = 0;
     bool tc_ready = false;
     int tc_flags = 0;            // bring-up switches (env B2S_TC_FLAGS)
+    Buf<unsigned> d_tc_sched;    // per-launch tile counters {next tile, CTAs done}, zero between launches
+    unsigned tc_launches = 0;
 
     // ---- FFT overlap-save form (fir_fft.cu): H[NF] then W_NF[NF], built lazily
     Buf<float2> d_fftH;

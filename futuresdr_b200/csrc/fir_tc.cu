@@ -69,6 +69,7 @@ constexpr int kRegsAtLaunch = 65536 / kThreadsTC / 8 * 8;
 constexpr int kMathRegs = 176, kProdRegs = 48, kLoaderRegs = 24;
 static_assert(kNumMathThreads * kMathRegs + kNumProducerThreads * kProdRegs + kNumLoaderThreads * kLoaderRegs <=
               kThreadsTC * kRegsAtLaunch, "setmaxnreg budget exceeds the CTA's register allocation");
+constexpr int kSchedSlots = 64;              // tile counters per plan (launches of a plan that may be in flight at once)
 constexpr int kAtomsOut = 16;                // N = 128 columns = 16 swizzle atoms of 8 rows
 constexpr int kMaxDK = 3;                    // K <= 384
 // K-steps one math warpgroup issues per tile: its 64 phases start on a multiple of 16 and lead + ntaps <= 128*DK - 127,
@@ -79,7 +80,25 @@ constexpr int kStageBytes = 2 * kSplitBytesMax;                       // hi + lo
 constexpr int kACores = kMaxDK * 16 + 15;    // core matrices of the aliased Toeplitz strip (K/8 + 128/8 - 1)
 constexpr int kABytes = kACores * 128;       // per precision (hi, lo)
 constexpr int kSmemTC = kStages * kStageBytes + kRawSlots * kRawSlotBytes + 2 * kABytes + 1024 /*align*/ + 256 /*barriers*/;
+static_assert(8 * (2 * kStages + 2 * kRawSlots) + 16 + 4 * kStages <= 256, "barriers and tile numbers exceed their 256 bytes");
 static_assert(kSmemTC <= 227 * 1024, "tensor FIR shared memory exceeds the 227 KiB per-CTA limit");
+
+// -DB2S_TC_TIMELINE (scripts/tc_timeline.py): every CTA writes %globaltimer stamps of the launch's edges, one thread per
+// role, into g_tc_timeline[cta][TL_*]; b2s_tc_timeline_read copies them out.  The default build has none of it.
+enum TcStamp { TL_ENTRY, TL_FIRST_COPY, TL_LAST_COPY, TL_FIRST_FULL, TL_FIRST_STORE, TL_LAST_STORE, TL_CONV_EXIT,
+               TL_EXIT, TL_NSTAMPS };
+#ifdef B2S_TC_TIMELINE
+constexpr int kTlCtas = 1024;
+__device__ unsigned long long g_tc_timeline[kTlCtas * TL_NSTAMPS];
+#define TC_STAMP(k)                                                                          \
+    do {                                                                                     \
+        unsigned long long t_;                                                               \
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t_)::"memory");                     \
+        if (blockIdx.x < kTlCtas) g_tc_timeline[blockIdx.x * TL_NSTAMPS + (k)] = t_;         \
+    } while (0)
+#else
+#define TC_STAMP(k) do {} while (0)
+#endif
 
 // ---- PTX helpers ------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -229,6 +248,7 @@ struct TcParams {
     unsigned *pub_flag;          // *pub_flag = pub_value (release, system scope) as soon as the kernel runs: everything queued
     unsigned pub_value;          // before it on the stream (the chunk this rank owns) is in HBM
     unsigned *status;            // device status word of the context: bit0 = a flag wait timed out
+    unsigned *sched;             // {next tile, CTAs done}: zero at launch, zero again when the last CTA is done
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -256,8 +276,15 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
     auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
     auto rfull_bar = [&](int r) { return bar_base + 8u * (2 * kStages + r); };
     auto rempty_bar = [&](int r) { return bar_base + 8u * (2 * kStages + kRawSlots + r); };
+    // tile numbers handed down the pipeline (-1: no more tiles): loader -> converters per tile (ring of 4, indexed by
+    // the CTA's tile count; the loader runs less than one tile ahead), converters -> math per operand stage
+    const uint32_t tile_ring = bar_base + 8u * (2 * kStages + 2 * kRawSlots);
+    const uint32_t stage_tile = tile_ring + 16u;
+    volatile int *tile_ring_gen = reinterpret_cast<volatile int *>(gen_base + (tile_ring - base));
+    volatile int *stage_tile_gen = reinterpret_cast<volatile int *>(gen_base + (stage_tile - base));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) TC_STAMP(TL_ENTRY);
     if (prm.pub_flag && blockIdx.x == 0 && threadIdx.x == 0) {
         __threadfence_system();
         asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(prm.pub_flag), "r"(prm.pub_value) : "memory");
@@ -275,20 +302,28 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         for (int r = 0; r < kRawSlots; r++) { mbar_init(rfull_bar(r), 1); mbar_init(rempty_bar(r), kProdWarps); }
         fence_barrier_init();
     }
-    // ---- one-time: the aliased Toeplitz strip.  Core matrix s, row r, element e (byte 128*s + 16*r + 2*e) holds
-    // A[p'][kappa] for every p' = 8a + r, kappa = 8j + e with a + j = s:  g[kappa - p - lead], p = 127 - p'
-    // (`lead` zero taps in front meet the dummy items).
-    const int a_elems = (K / 8 + 15) * 64;
-    for (int i = threadIdx.x; i < a_elems; i += kThreadsTC) {
-        const int s = i >> 6, r = (i >> 3) & 7, e = i & 7;
-        const int t = 8 * s + r + e - 127 - prm.lead;
-        const float gv = (t >= 0 && t < prm.ntaps) ? __ldg(prm.g + t) : 0.0f;
-        const __nv_bfloat16 hi = __float2bfloat16_rn(gv);
-        a_gen[i] = hi;
-        a_gen[kABytes / 2 + i] = __float2bfloat16_rn(gv - __bfloat162float(hi));
-    }
-    fence_proxy_async();                             // generic-proxy stores -> visible to wgmma (async proxy)
-    __syncthreads();
+    __syncthreads();                                 // barriers initialised: the loader starts streaming right away
+
+    // ---- one-time, by the converters and the math warpgroups while the loader already streams: the aliased Toeplitz
+    // strip.  Core matrix s, row r, element e (byte 128*s + 16*r + 2*e) holds A[p'][kappa] for every p' = 8a + r,
+    // kappa = 8j + e with a + j = s:  g[kappa - p - lead], p = 127 - p' (`lead` zero taps in front meet the dummy
+    // items).  Only the math warpgroups read it: the converters help build it and go on without waiting.
+    auto build_strip = [&](auto wait_c) {
+        const int a_elems = (K / 8 + 15) * 64;
+        for (int i = threadIdx.x; i < a_elems; i += kNumMathThreads + kNumProducerThreads) {
+            const int s = i >> 6, r = (i >> 3) & 7, e = i & 7;
+            const int t = 8 * s + r + e - 127 - prm.lead;
+            const float gv = (t >= 0 && t < prm.ntaps) ? __ldg(prm.g + t) : 0.0f;
+            const __nv_bfloat16 hi = __float2bfloat16_rn(gv);
+            a_gen[i] = hi;
+            a_gen[kABytes / 2 + i] = __float2bfloat16_rn(gv - __bfloat162float(hi));
+        }
+        fence_proxy_async();                         // generic-proxy stores -> visible to wgmma (async proxy)
+        if constexpr (decltype(wait_c)::value)       // named barrier 1: warps 0-15, never the loader
+            asm volatile("bar.sync 1, %0;" ::"n"(kNumMathThreads + kNumProducerThreads) : "memory");
+        else
+            asm volatile("bar.arrive 1, %0;" ::"n"(kNumMathThreads + kNumProducerThreads) : "memory");
+    };
 
     // A tile's contiguous input span (TILE_BLOCKS + DK - 1 blocks of 128 items) travels through the raw
     // ring in slots of 8 KiB = 512 float4 (8 complex blocks / 16 real blocks); 9 slots per tile.
@@ -303,12 +338,30 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         // One thread streams the input with bulk async copies (cp.async.bulk): the copies complete on the
         // slot's mbarrier (complete_tx), so HBM latency is absorbed by the 48 KiB ring and never by a
         // converter warp's registers.
+        // The CTA takes tiles from the launch's counter as its ring frees up, so an SM that streams faster takes more
+        // tiles and all SMs run out of work within about one tile time of each other.
         setmaxnreg_dec<kLoaderRegs>();
         if (warp != kTmaWarp) return;
         if (elect_one()) {
             int rs = 0;
             uint32_t rphase = 0;
-            for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+            for (int k = 0;; k++) {
+                const int tile = (int)atomicAdd(prm.sched, 1u);
+                if (tile >= prm.num_tiles) {
+                    // no tile left: the end mark goes down the pipeline in place of a tile's first slot
+                    mbar_wait(rempty_bar(rs), rphase ^ 1);
+                    tile_ring_gen[k & 3] = -1;
+                    mbar_arrive(rfull_bar(rs));
+                    // the last CTA to find the counter spent zeroes it for the next launch on this slot
+                    __threadfence();
+                    if (atomicAdd(prm.sched + 1, 1u) == gridDim.x - 1) {
+                        __threadfence();
+                        atomicExch(prm.sched, 0u);
+                        atomicExch(prm.sched + 1, 0u);
+                    }
+                    break;
+                }
+                tile_ring_gen[k & 3] = tile;          // published by the first slot's arrive (release)
                 const long long item0 = (long long)tile * TILE_ITEMS;
 #pragma unroll 1
                 for (int s = 0; s < SLOTS_PER_TILE; s++) {
@@ -353,9 +406,11 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
                     } else {
                         mbar_arrive(rfull_bar(rs));          // nothing to copy (tile past the end): just hand it over
                     }
+                    if (k == 0 && s == 0) TC_STAMP(TL_FIRST_COPY);
                     if (++rs == kRawSlots) { rs = 0; rphase ^= 1; }
                 }
             }
+            TC_STAMP(TL_LAST_COPY);
         }
         __syncwarp();
     } else if (warp >= kProdWarp0) {
@@ -365,6 +420,7 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         // loops are fully unrolled, so every shared-memory address is
         //     stage base + per-thread constant + compile-time constant + one of 8 precomputed swizzle offsets.
         // Per float4: one LDS.128, two XU conversions per value pair, 4 (8 for aliased rows) 32-bit stores.
+        build_strip(std::false_type{});
         setmaxnreg_dec<kProdRegs>();
         const int tid = threadIdx.x - 32 * kProdWarp0;                   // 0..255
         const int fo = tid % F4_PER_BLOCK, rowsel = tid / F4_PER_BLOCK;  // rowsel 0..3 (complex) / 0..7 (real)
@@ -464,11 +520,19 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
 
         int stage = 0, rs = 0;
         uint32_t phase = 0, rphase = 0;
-        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+        for (int k = 0;; k++) {
+            mbar_wait(rfull_bar(rs), rphase);        // the tile's first slot, or the end mark
+            const int tile = tile_ring_gen[k & 3];
+            mbar_wait(empty_bar(stage), phase ^ 1);
+            if (threadIdx.x == 32 * kProdWarp0) stage_tile_gen[stage] = tile;   // published by this warp's arrive
+            if (tile < 0) {                          // no more tiles: pass the end mark on to the math warpgroups
+                __syncwarp();
+                if (lane == 0) mbar_arrive(full_bar(stage));
+                break;
+            }
             const long long item0 = (long long)tile * TILE_ITEMS;
             const bool interior = item0 + (long long)in_blocks * 128 <= prm.n_in &&
                                   !(tile == 0 && (prm.lead | prm.hist_items) != 0);   // tile 0 zeroes the dummy items
-            mbar_wait(empty_bar(stage), phase ^ 1);
             unsigned char *stage_ptr = gen_base + stage * kStageBytes;
             if (interior) convert_tile(std::true_type{}, stage_ptr, item0, rs, rphase);
             else convert_tile(std::false_type{}, stage_ptr, item0, rs, rphase);
@@ -477,11 +541,13 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
             if (lane == 0) mbar_arrive(full_bar(stage));
             if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
+        if (threadIdx.x == 32 * kProdWarp0) TC_STAMP(TL_CONV_EXIT);
     } else {
         // ================================ MATH WARPGROUPS ======================================
         // Warpgroup wg computes the accumulator rows p' = 64*wg .. 64*wg+63 (output phases p = 127 - p') of
         // all 128 columns.  Thread (warp w, lane) holds rows 16*(w%4) + lane/4 + {0, 8} of its warpgroup and
         // columns 8*gamma + 2*(lane%4) + {0, 1}: acc[4*gamma + 2*h + e].
+        build_strip(std::true_type{});
         setmaxnreg_inc<kMathRegs>();
         // warp-uniform by construction (a broadcast): the K-step loop below branches on it, and wgmma.mma_async in a
         // loop the compiler must assume divergent is serialised
@@ -524,9 +590,8 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
 
         int stage = 0;
         uint32_t phase = 0;
-        // wait for the stage, issue its MMAs into acc and commit them
+        // issue the full stage's MMAs into acc and commit them
         auto mma_tile = [&](float (&acc)[64]) {
-            mbar_wait(full_bar(stage), phase);
             wgmma_fence();                           // earlier register reads of acc precede the async writes
             // Shared-memory addresses stay below 2^18, so a byte offset moves a descriptor's start field by offset / 16
             // without a carry: the per-K-step descriptors are the tile's base descriptors plus small offsets.
@@ -586,11 +651,19 @@ __global__ void __launch_bounds__(kThreadsTC, 1) fir_tc_kernel(const TcParams pr
         float acc[64];
 #pragma unroll
         for (int i = 0; i < 64; i++) acc[i] = 0.0f;
-        for (int tile = blockIdx.x; tile < prm.num_tiles; tile += gridDim.x) {
+        for (int k = 0;; k++) {
+            mbar_wait(full_bar(stage), phase);
+            // the stage's tile, or the end mark; a broadcast, so that the loop is warp-uniform by construction
+            const int tile = __shfl_sync(0xffffffffu, stage_tile_gen[stage], 0);
+            if (tile < 0) break;
             mma_tile(acc);
+            if (threadIdx.x == 0 && k == 0) TC_STAMP(TL_FIRST_FULL);   // (+ its MMAs issued)
             release_stage();
+            if (threadIdx.x == 0) TC_STAMP(TL_LAST_STORE);            // (overwritten until the last tile)
             store_tile(acc, tile);
+            if (threadIdx.x == 0 && k == 0) TC_STAMP(TL_FIRST_STORE);
         }
+        if (threadIdx.x == 0) TC_STAMP(TL_EXIT);
     }
 }
 
@@ -621,6 +694,8 @@ int32_t fir_tc_prepare(b2s_fir *f) {
                             "budget assumes %d", attr.numRegs, kRegsAtLaunch);
     }
     if (const char *e = getenv("B2S_TC_FLAGS")) f->tc_flags = atoi(e);
+    B2S_TRY(f->d_tc_sched.alloc(ctx, 2 * kSchedSlots, "tensor FIR: tile counters"));
+    B2S_CUDA(ctx, cudaMemset(f->d_tc_sched.get(), 0, 2 * kSchedSlots * sizeof(unsigned)));
     f->tc_ready = true;
     return B2S_OK;
 }
@@ -665,6 +740,9 @@ int32_t fir_tc_launch_hist(b2s_fir *f, const FirHist *h, const void *d_in, size_
     prm.pub_flag = h ? h->publish_flag : nullptr;
     prm.pub_value = h ? h->publish_value : 0;
     prm.status = ctx->d_status;
+    // a launch's tile counter: one of kSchedSlots per plan in turn, so launches of the plan in flight at the same time
+    // (on different streams) use different counters
+    prm.sched = f->d_tc_sched.get() + 2 * (f->tc_launches++ % kSchedSlots);
     prm.out = (float *)d_out;
     prm.g = f->d_ptaps.get() + (size_t)f->decim * f->Upad;      // plain reversed taps (fir_direct_prepare)
     prm.n_in = (long long)(lead + n_hist + n_in);
@@ -682,6 +760,19 @@ int32_t fir_tc_launch_hist(b2s_fir *f, const FirHist *h, const void *d_in, size_
     B2S_CHECK_LAUNCH(ctx);
     return B2S_OK;
 }
+
+#ifdef B2S_TC_TIMELINE
+// Copies the stamps of the most recent launch for CTAs [0, ctas) into host[cta * TL_NSTAMPS + stamp] (nanoseconds,
+// %globaltimer) and clears them; returns TL_NSTAMPS, or -1 on a CUDA error.  Synchronous.
+extern "C" int b2s_tc_timeline_read(unsigned long long *host, int ctas) {
+    const size_t bytes = sizeof(unsigned long long) * TL_NSTAMPS * (size_t)std::min(std::max(ctas, 0), kTlCtas);
+    void *d = nullptr;
+    if (cudaGetSymbolAddress(&d, g_tc_timeline) != cudaSuccess) return -1;
+    if (cudaMemcpy(host, d, bytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -1;
+    if (cudaMemset(d, 0, sizeof(unsigned long long) * TL_NSTAMPS * kTlCtas) != cudaSuccess) return -1;
+    return TL_NSTAMPS;
+}
+#endif
 
 int32_t fir_tc_launch(b2s_fir *f, const void *d_in, size_t n_in, void *d_out, size_t n_out,
                       cudaStream_t stream) {
